@@ -181,9 +181,9 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         case KVP_SCORER_KEYDIFF: *launches_out = 5; break;  // memset, anchor partials, merge, score, select+compact
         case KVP_SCORER_SNAPKV: *launches_out = 5; break;  // memset, stats, colsum, finalize, select+compact
         case KVP_SCORER_EXPECTED_ATTENTION: {
-            // press defaults (use_covariance + use_vnorm): memset, logits, value norms (side stream), finalize,
-            // select+compact
-            *launches_out = 5;
+            // press defaults (use_covariance + use_vnorm): memset, logits (which also writes the value norms),
+            // finalize, select+compact
+            *launches_out = 4;
             break;
         }
         default: return KVP_ERR_BAD_ARGUMENT;

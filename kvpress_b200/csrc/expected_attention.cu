@@ -9,15 +9,14 @@
 // The reference materialises repeat_kv(K)^T twice and a [B,Hq,D,S] einsum intermediate; here
 //   kernel 1 (ea_logits_kernel, persistent, one CTA per SM, warp-specialised):
 //       TMA streams 128-position K tiles (SWIZZLE_128B) into a ring; two consumer warpgroups compute
-//       Y = K_tile[64 x D] * Sigma_g^T per head with wgmma (accumulators in registers) and finish
-//       logit = sum_n k_n (Y_n + 2 sqrt(d) mu_n) / (2d) with the k rows taken from the same shared-memory tile,
+//       Y = K_tile[64 x D] * Sigma_g^T per head with wgmma (K rows from registers, accumulators in registers) and
+//       finish logit = sum_n k_n (Y_n + 2 sqrt(d) mu_n) / (2d) with the same k registers,
 //       keep online softmax statistics and store fp32 logits. Sigma of up to four heads (the unit) stays resident
 //       in shared memory while the CTA works on that unit.
-//   ea_vnorm_kernel (side stream, next to kernel 1): ||v_s|| for every position.
+//       Three otherwise idle warps of the producer warpgroup stream V next to the MMAs and write ||v_s||.
 //   kernel 2 (ea_finalize_kernel): combines the per-CTA softmax statistics, forms the final score in
 //       fp32, rounds it ONCE to the cache dtype, and emits keys + histogram for the select stage.
-// Covariance-free mode (use_covariance=False) is a plain streaming GEMV kernel.
-#include <mutex>
+// Covariance-free mode (use_covariance=False) is a plain streaming GEMV kernel that also writes ||v_s||.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -29,6 +28,7 @@ namespace kvp {
 constexpr int kEaTile = 128;      // key rows per MMA tile (M)
 constexpr int kEaThreads = 384;   // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue
 constexpr int kEaMaxParts = 160;  // upper bound on CTAs per (b,h) row (>= SM count)
+constexpr int kEaVnormLoads = 8;  // 16-byte V loads in flight per lane of a value-norm warp
 
 struct EaScratch {
     float* logits;    // [R][G][S_pad]
@@ -110,15 +110,20 @@ extern "C" int kvp_debug_ea_pair_partition(int n_units, int n_tp, int n_pairs, i
     return 0;
 }
 
-// One thread of warpgroup 0 streams the covariance of the unit's heads (resident for the unit) and the K tiles through
-// a ring; consumer warpgroup cw computes Y_g = K[64 cw .. 64 cw + 64) * Sigma_g^T (wgmma, accumulators in registers) and
-// finishes logit_g = sum_n k_n (Y_g,n + 2 sqrt(d) mu_g,n) / (2d) with the k rows read back from the same tile. A thread
-// holds two rows and D/4 columns; the four threads of a row add their partial dot products.
+// Warpgroup 0: one thread streams the covariance of the unit's heads (resident for the unit) and the K tiles through a
+// ring; warps 1-3 stream the V rows of the CTA's tiles and write ||v_s|| (units with g_off == 0 only, so each row's
+// norms are computed once). Consumer warpgroup cw loads its 64 rows of the tile into registers once (ldmatrix),
+// releases the stage, computes Y_g = K[64 cw .. 64 cw + 64) * Sigma_g^T per head (wgmma, A from registers,
+// accumulators in registers) and finishes logit_g = sum_n k_n (Y_g,n + 2 sqrt(d) mu_g,n) / (2d) with the same k
+// registers: the A fragment of k-step kk holds columns 16 kk + 2 qd + {0, 1, 8, 9} of rows r0 and r0 + 8, which are the
+// accumulator columns 8 j + 2 qd + {0, 1} for j = 2 kk, 2 kk + 1. A thread holds two rows and D/4 columns; the four
+// threads of a row add their partial dot products.
 template <typename T, int D, int GR>
 __global__ void __launch_bounds__(kEaThreads, 1)
 ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapCov,
-                 const T* __restrict__ mu, int H, int Hq, int S, int n_sink, int R, int n_tiles128, int n_workers,
-                 int n_parts, EaScratch sc, int S_pad, int g_total, int n_split) {
+                 const T* __restrict__ mu, const T* __restrict__ V, Strides3 vs, int use_vnorm, int H, int Hq, int S,
+                 int n_sink, int R, int n_tiles128, int n_workers, int n_parts, EaScratch sc, int S_pad, int g_total,
+                 int n_split) {
     using L = EaSmem<D, GR>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     // dynamic shared memory is only guaranteed 16-B aligned: round up to 1024 B for the swizzle
@@ -142,7 +147,7 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
         umma::prefetch_tmap(&mapCov);
         for (int i = 0; i < kStages; ++i) {
             umma::mbar_init(&k_full[i], 1);
-            umma::mbar_init(&k_empty[i], 8);  // lane 0 of each consumer warp, after its MMAs and k-row reads
+            umma::mbar_init(&k_empty[i], 8);  // lane 0 of each consumer warp, once its k rows are in registers
         }
         umma::mbar_init(cov_full, 1);
         umma::mbar_fence_init();
@@ -176,8 +181,8 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
         __syncthreads();
 
         if (wg == 0) {
-            // ===== TMA producer =====
             if (tid == 0) {
+                // ===== TMA producer =====
                 umma::mbar_arrive_expect_tx(cov_full, (uint32_t)(n_real * L::kPanels * L::kCovHeadPanel));
                 for (int kp = 0; kp < L::kPanels; ++kp)
                     for (int g = 0; g < n_real; ++g)
@@ -191,11 +196,16 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                         umma::tma_load_4d(s_stage + stage * L::kStageBytes + kp * (kEaTile * 128), &mapK,
                                           &k_full[stage], kp * 64, t * kEaTile, h, b);
                 }
+            } else if (warp > 0 && use_vnorm && g_off == 0) {
+                // ===== value norms of this CTA's positions of the row, next to the MMAs =====
+                row_norm_span<T, D / 8, kEaVnormLoads>(V, vs, b, h, t_begin * kEaTile, min(t_end * kEaTile, S), D,
+                                                       sc.vnorm + (size_t)row * S_pad, warp - 1, 3);
             }
         } else {
             // ===== consumers: wgmma + epilogue; thread = rows r0, r0 + 8 of the tile =====
             const int cw = wg - 1, qd = lane & 3;
             const int r0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);
+            const int r_ld = cw * 64 + (warp & 3) * 16 + (lane & 15);  // the row this lane addresses for ldmatrix
             float run_m[GR], run_z[GR];
 #pragma unroll
             for (int g = 0; g < GR; ++g) {
@@ -206,8 +216,15 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
             for (int t = t_begin; t < t_end; ++t, ++k_it) {
                 const int stage = k_it % kStages;
                 umma::mbar_wait(&k_full[stage], (k_it / kStages) & 1);
-                const unsigned char* krow = s_stage + stage * L::kStageBytes;
-                const uint32_t a_base = umma::smem_u32(krow) + cw * 64 * 128;
+                const uint32_t k_base = umma::smem_u32(s_stage + stage * L::kStageBytes);
+                uint32_t ka[D / 16][4];  // this warp's 16 rows of the tile: the A fragment of each k-step
+#pragma unroll
+                for (int kk = 0; kk < D / 16; ++kk)
+                    umma::ldmatrix_x4(ka[kk], k_base + (kk >> 2) * (kEaTile * 128) +
+                                                  umma::sw128_offset(r_ld, 2 * (kk & 3) + (lane >> 4)));
+                // the k rows are in registers: hand the stage back to the producer before the MMAs
+                __syncwarp();
+                if (lane == 0) umma::mbar_arrive(&k_empty[stage]);
                 float lg[GR][2];
 #pragma unroll
                 for (int g = 0; g < GR; ++g) {
@@ -216,24 +233,21 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                     float acc[D / 2];
                     umma::wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < D / 16; ++k) {
-                        const int kp = k >> 2, kk = k & 3;
-                        umma::wgmma_ss<D, F16Traits<T>::kMmaFormat>(
-                            acc, umma::smem_desc_sw128(a_base + kp * (kEaTile * 128) + kk * 32),
-                            umma::smem_desc_sw128(umma::smem_u32(s_cov + (kp * GR + g) * L::kCovHeadPanel) + kk * 32),
-                            k > 0);
+                    for (int kk = 0; kk < D / 16; ++kk) {
+                        const int kp = kk >> 2, ks = kk & 3;
+                        umma::wgmma_rs<D, F16Traits<T>::kMmaFormat>(
+                            acc, ka[kk],
+                            umma::smem_desc_sw128(umma::smem_u32(s_cov + (kp * GR + g) * L::kCovHeadPanel) + ks * 32),
+                            kk > 0);
                     }
                     umma::wgmma_commit();
                     umma::wgmma_wait_all();
                     float l0 = 0.f, l1 = 0.f;
 #pragma unroll
                     for (int j = 0; j < D / 8; ++j) {
-                        // columns 8j + 2 qd, +1: 16-byte chunk j % 8 of panel j / 8, bytes 4 qd .. 4 qd + 3
-                        const unsigned char* pj = krow + (j >> 3) * (kEaTile * 128) + 4 * qd;
-                        const float2 k0 = F16Traits<T>::unpack2(
-                            *reinterpret_cast<const uint32_t*>(pj + umma::sw128_offset(r0, j & 7)));
-                        const float2 k1 = F16Traits<T>::unpack2(
-                            *reinterpret_cast<const uint32_t*>(pj + umma::sw128_offset(r0 + 8, j & 7)));
+                        // columns 8j + 2 qd, +1 of rows r0 (fragment register 0 or 2) and r0 + 8 (1 or 3)
+                        const float2 k0 = F16Traits<T>::unpack2(ka[j >> 1][(j & 1) * 2]);
+                        const float2 k1 = F16Traits<T>::unpack2(ka[j >> 1][(j & 1) * 2 + 1]);
                         const float2 bb = *reinterpret_cast<const float2*>(&s_bias[g * D + 8 * j + 2 * qd]);
                         l0 = fmaf(k0.x, acc[4 * j] + bb.x, l0);
                         l0 = fmaf(k0.y, acc[4 * j + 1] + bb.y, l0);
@@ -243,9 +257,6 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                     lg[g][0] = l0;
                     lg[g][1] = l1;
                 }
-                // K stage done (MMAs complete, k rows read): release it before the global stores below
-                __syncwarp();
-                if (lane == 0) umma::mbar_arrive(&k_empty[stage]);
 #pragma unroll
                 for (int g = 0; g < GR; ++g) {
 #pragma unroll
@@ -303,11 +314,13 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
     }
 }
 
-// ---- covariance-free logits: mu.k / sqrt(d) with plain streaming loads (use_covariance=False) -------
+// ---- covariance-free logits: mu.k / sqrt(d) with plain streaming loads (use_covariance=False); the same CTA
+// writes ||v_s|| of its positions first when the score uses the value norms -----------------------------------------
 template <typename T, int LPR>
 __global__ void __launch_bounds__(256)
-ea_mu_logits_kernel(const T* __restrict__ K, Strides3 ks, const T* __restrict__ mu, int H, int Hq, int G,
-                    int S, int D, int n_sink, int n_parts, EaScratch sc, int S_pad) {
+ea_mu_logits_kernel(const T* __restrict__ K, Strides3 ks, const T* __restrict__ mu, const T* __restrict__ V,
+                    Strides3 vs, int use_vnorm, int H, int Hq, int G, int S, int D, int n_sink, int n_parts,
+                    EaScratch sc, int S_pad) {
     __shared__ float s_mu[8 * 256];
     __shared__ float s_red[8][8][2];
     const int chunk = blockIdx.x, row = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -316,6 +329,9 @@ ea_mu_logits_kernel(const T* __restrict__ K, Strides3 ks, const T* __restrict__ 
     const float scale = 1.0f / sqrtf((float)D);
     for (int i = tid; i < G * D; i += 256)
         s_mu[i] = F16Traits<T>::to_float(reinterpret_cast<const uint16_t*>(mu)[(size_t)hq0 * D + i]);
+    if (use_vnorm)
+        row_norm_span<T, LPR, 8>(V, vs, b, h, chunk * kScoreChunkGeneric, min((chunk + 1) * kScoreChunkGeneric, S), D,
+                                 sc.vnorm + (size_t)row * S_pad, warp, 8);
     __syncthreads();
     constexpr int RPW = 32 / LPR;
     constexpr int TOK_PER_WARP = kScoreChunkGeneric / 8;
@@ -402,20 +418,6 @@ ea_mu_logits_kernel(const T* __restrict__ K, Strides3 ks, const T* __restrict__ 
         }
         sc.partial[((size_t)row * G + tid) * n_parts + chunk] = make_float2(m, z);
     }
-}
-
-// ---- ||v_s||_2 for every position: plain streaming kernel, launched on a side stream so that it shares
-// the SMs with the tensor-bound logits kernel (which leaves ~70 % of the HBM bandwidth idle) -----------
-template <typename T, int LPR>
-__global__ void __launch_bounds__(kTileThreads, 4)
-ea_vnorm_kernel(const T* __restrict__ V, Strides3 vs, int H, int S, int D, float* __restrict__ vnorm,
-                int S_pad) {
-    __shared__ float s_norm[kTile];
-    const int tile = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
-    row_norm_chunk<T, LPR>(V, vs, row / H, row % H, tile, S, D, s_norm);
-    __syncthreads();
-    const int s = tile * kTile + tid;
-    if (s < S) vnorm[(size_t)row * S_pad + s] = s_norm[tid];
 }
 
 // ---- finalize: softmax normalisation, group mean, * ||v||, ONE rounding, keys + histogram -----------
@@ -550,8 +552,9 @@ cudaError_t launch_fill_sentinel(int dtype, void* scores_out, int R, int S, int 
 
 // ---- host launcher -----------------------------------------------------------------------------------
 template <typename T, int D, int GR>
-static cudaError_t launch_ea_logits_t(const Dims& d, const void* K, const void* mu, const void* cov, int n_sink,
-                                      const Workspace& ws, const EaScratch& sc, int* n_parts_out, cudaStream_t st) {
+static cudaError_t launch_ea_logits_t(const Dims& d, const void* K, const void* V, const void* mu, const void* cov,
+                                      int use_vnorm, int n_sink, const Workspace& ws, const EaScratch& sc,
+                                      int* n_parts_out, cudaStream_t st) {
     using L = EaSmem<D, GR>;
     const int n_tiles128 = (d.S + kEaTile - 1) / kEaTile;
     const int g_total = d.Hq / d.H;
@@ -591,48 +594,9 @@ static cudaError_t launch_ea_logits_t(const Dims& d, const void* K, const void* 
     auto kern = ea_logits_kernel<T, D, GR>;
     static PerDeviceOnce smem_set;  // one per <T, D, GR> instantiation of this launcher
     if ((e = ensure_dynamic_smem(kern, smem, smem_set)) != cudaSuccess) return e;
-    kern<<<n_workers, kEaThreads, smem, st>>>(mapK, mapCov, static_cast<const T*>(mu), d.H, d.Hq, d.S, n_sink, d.R,
-                                              n_tiles128, n_workers, n_parts, sc, ws.S_pad, g_total, n_split);
-    return cudaPeekAtLastError();
-}
-
-// Side stream + fork/join events for the concurrent V-norm kernel: created once per device, never
-// modified afterwards (the only process-wide state of the library besides cached device properties).
-struct EaSideStream {
-    cudaStream_t stream = nullptr;
-    cudaEvent_t fork = nullptr, join = nullptr;
-    bool ok = false;
-};
-static std::mutex g_ea_enqueue_mu;  // serialises fork..join enqueues that share the side stream / events
-static EaSideStream* ea_side_stream() {
-    static EaSideStream per_device[64];
-    static std::mutex mu;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-    std::lock_guard<std::mutex> lock(mu);
-    EaSideStream& s = per_device[dev];
-    if (!s.ok) {
-        if (cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking) != cudaSuccess) return nullptr;
-        if (cudaEventCreateWithFlags(&s.fork, cudaEventDisableTiming) != cudaSuccess) return nullptr;
-        if (cudaEventCreateWithFlags(&s.join, cudaEventDisableTiming) != cudaSuccess) return nullptr;
-        s.ok = true;
-    }
-    return &s;
-}
-
-template <typename T>
-static cudaError_t launch_ea_vnorm_t(const Dims& d, const void* V, const Workspace& ws, const EaScratch& sc,
-                                     cudaStream_t st) {
-    dim3 grid(ws.n_tiles, d.R);
-    const int nvec = d.D / 8;
-#define KVP_EA_VN(LPR)                                                                               \
-    ea_vnorm_kernel<T, LPR><<<grid, kTileThreads, 0, st>>>(static_cast<const T*>(V), d.vs, d.H, d.S, d.D, \
-                                                           sc.vnorm, ws.S_pad)
-    if (nvec <= 4) KVP_EA_VN(4);
-    else if (nvec <= 8) KVP_EA_VN(8);
-    else if (nvec <= 16) KVP_EA_VN(16);
-    else KVP_EA_VN(32);
-#undef KVP_EA_VN
+    kern<<<n_workers, kEaThreads, smem, st>>>(mapK, mapCov, static_cast<const T*>(mu), static_cast<const T*>(V), d.vs,
+                                              use_vnorm, d.H, d.Hq, d.S, n_sink, d.R, n_tiles128, n_workers, n_parts,
+                                              sc, ws.S_pad, g_total, n_split);
     return cudaPeekAtLastError();
 }
 
@@ -646,17 +610,7 @@ static cudaError_t launch_ea_t(const Dims& d, int dtype, const void* K, const vo
     const EaScratch sc = carve_ea(d, ws);
     int n_parts = 0;
     cudaError_t e = cudaSuccess;
-    // Value norms: ea_vnorm_kernel runs on an internal side stream next to the score kernel: fork here, join before
-    // the finalize kernel.
-    EaSideStream* side = use_vnorm ? ea_side_stream() : nullptr;
-    // host threads enqueueing on different streams of one device share the side stream and its two
-    // events: hold the lock for the (host-only, microseconds) fork..join enqueue sequence
-    std::unique_lock<std::mutex> enqueue_lock(g_ea_enqueue_mu, std::defer_lock);
-    if (side != nullptr) enqueue_lock.lock();
-    if (side != nullptr) {
-        if ((e = cudaEventRecord(side->fork, st)) != cudaSuccess) return e;
-        if ((e = cudaStreamWaitEvent(side->stream, side->fork, 0)) != cudaSuccess) return e;
-    }
+    // the logits kernels also write the value norms (use_vnorm): V is not touched otherwise and may be null
     if (cov != nullptr) {
         // tensor-core path: head_dim 64 or 128; the G query heads of a kv head are cut into units of four resident
         // heads (Llama-3.1-8B: 4, Llama-3.1-70B: 8), of two for other group sizes (an odd G leaves its last unit one
@@ -665,21 +619,22 @@ static cudaError_t launch_ea_t(const Dims& d, int dtype, const void* K, const vo
         if (d.D != 128 && d.D != 64) return cudaErrorNotSupported;
         const bool d128 = d.D == 128;
         if (G % 4 == 0)
-            e = d128 ? launch_ea_logits_t<T, 128, 4>(d, K, mu, cov, n_sink, ws, sc, &n_parts, st)
-                     : launch_ea_logits_t<T, 64, 4>(d, K, mu, cov, n_sink, ws, sc, &n_parts, st);
+            e = d128 ? launch_ea_logits_t<T, 128, 4>(d, K, V, mu, cov, use_vnorm, n_sink, ws, sc, &n_parts, st)
+                     : launch_ea_logits_t<T, 64, 4>(d, K, V, mu, cov, use_vnorm, n_sink, ws, sc, &n_parts, st);
         else if (G == 1)
-            e = d128 ? launch_ea_logits_t<T, 128, 1>(d, K, mu, cov, n_sink, ws, sc, &n_parts, st)
-                     : launch_ea_logits_t<T, 64, 1>(d, K, mu, cov, n_sink, ws, sc, &n_parts, st);
+            e = d128 ? launch_ea_logits_t<T, 128, 1>(d, K, V, mu, cov, use_vnorm, n_sink, ws, sc, &n_parts, st)
+                     : launch_ea_logits_t<T, 64, 1>(d, K, V, mu, cov, use_vnorm, n_sink, ws, sc, &n_parts, st);
         else
-            e = d128 ? launch_ea_logits_t<T, 128, 2>(d, K, mu, cov, n_sink, ws, sc, &n_parts, st)
-                     : launch_ea_logits_t<T, 64, 2>(d, K, mu, cov, n_sink, ws, sc, &n_parts, st);
+            e = d128 ? launch_ea_logits_t<T, 128, 2>(d, K, V, mu, cov, use_vnorm, n_sink, ws, sc, &n_parts, st)
+                     : launch_ea_logits_t<T, 64, 2>(d, K, V, mu, cov, use_vnorm, n_sink, ws, sc, &n_parts, st);
     } else {
         n_parts = (d.S + kScoreChunkGeneric - 1) / kScoreChunkGeneric;
         dim3 grid(n_parts, d.R);
 #define KVP_EA_MU(LPR)                                                                                   \
-    ea_mu_logits_kernel<T, LPR><<<grid, 256, 0, st>>>(static_cast<const T*>(K), d.ks,                     \
-                                                      static_cast<const T*>(mu), d.H, d.Hq, G, d.S, d.D, \
-                                                      n_sink, n_parts, sc, ws.S_pad)
+    ea_mu_logits_kernel<T, LPR><<<grid, 256, 0, st>>>(static_cast<const T*>(K), d.ks,                      \
+                                                      static_cast<const T*>(mu), static_cast<const T*>(V), \
+                                                      d.vs, use_vnorm, d.H, d.Hq, G, d.S, d.D, n_sink,     \
+                                                      n_parts, sc, ws.S_pad)
         if (nvec <= 4) KVP_EA_MU(4);
         else if (nvec <= 8) KVP_EA_MU(8);
         else if (nvec <= 16) KVP_EA_MU(16);
@@ -688,15 +643,6 @@ static cudaError_t launch_ea_t(const Dims& d, int dtype, const void* K, const vo
         e = cudaPeekAtLastError();
     }
     if (e != cudaSuccess) return e;
-    if (use_vnorm) {
-        // launched AFTER the logits kernel so that its CTAs fill the resources the logits CTAs leave free
-        cudaStream_t vst = side != nullptr ? side->stream : st;
-        if ((e = launch_ea_vnorm_t<T>(d, V, ws, sc, vst)) != cudaSuccess) return e;
-        if (side != nullptr) {  // join
-            if ((e = cudaEventRecord(side->join, side->stream)) != cudaSuccess) return e;
-            if ((e = cudaStreamWaitEvent(st, side->join, 0)) != cudaSuccess) return e;
-        }
-    }
     dim3 grid2((d.S + kEaFinalPos - 1) / kEaFinalPos, d.R);
     ea_finalize_kernel<T><<<grid2, kTileThreads, 0, st>>>(G, d.S, n_sink, use_vnorm, eps, n_parts, sc, ws,
                                                           static_cast<uint16_t*>(scores_out));

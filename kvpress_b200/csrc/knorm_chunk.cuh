@@ -113,50 +113,51 @@ __device__ __forceinline__ void knorm_score_chunk(const T* __restrict__ K, Strid
     }
 }
 
-// ||x_s||_2 in fp32 for the 256 positions of `chunk` of one (b, h) row into shared memory (same access
-// pattern as knorm_score_chunk; loads are L2-evict-first: V is read exactly once).
-template <typename T, int LPR>
-__device__ __forceinline__ void row_norm_chunk(const T* __restrict__ X, Strides3 xs, int b, int h, int chunk,
-                                               int S, int D, float* snorm) {
-    const int tid = threadIdx.x;
-    const int warp = tid >> 5, lane = tid & 31;
+// ||x_s||_2 in fp32 of positions [s_begin, s_end) of one (b, h) row, written to out[s]. `n_warps` warps share the span
+// (this is warp `wi` of them) in batches of U loads per lane; a sub-warp of LPR lanes covers a 2*D-byte row. Loads are
+// L2-evict-first: the rows are read exactly once. Each row's sum of squares is formed as in knorm_score_chunk (per lane
+// an even/odd FMA pair over its 8 elements, then the lane tree over xor LPR/2 .. 1 of RowSums), so the norms do not
+// depend on U, on the span or on how many warps share it.
+template <typename T, int LPR, int U>
+__device__ __forceinline__ void row_norm_span(const T* __restrict__ X, Strides3 xs, int b, int h, int s_begin,
+                                              int s_end, int D, float* __restrict__ out, int wi, int n_warps) {
+    const int lane = threadIdx.x & 31;
     constexpr int RPW = 32 / LPR;
-    constexpr int TOK_PER_WARP = kScoreChunk / (kTileThreads / 32);
-    constexpr int ITERS = TOK_PER_WARP / RPW;
-    constexpr int U = (ITERS < 8) ? ITERS : 8;
+    constexpr int kRows = RPW * U;  // rows per warp batch
     const int sub = lane % LPR, rsel = lane / LPR;
     const int nvec = D >> 3;
     const T* base = X + (int64_t)b * xs.b + (int64_t)h * xs.h + (int64_t)sub * 8;
-    const int s_warp = chunk * kScoreChunk + warp * TOK_PER_WARP;
     const uint64_t pol = l2_policy_evict_first();
 #pragma unroll 1
-    for (int it = 0; it < ITERS; it += U) {
+    for (int s0 = s_begin + wi * kRows; s0 < s_end; s0 += n_warps * kRows) {
         int4 v[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
-            const int s = s_warp + (it + u) * RPW + rsel;
+            const int s = s0 + u * RPW + rsel;
             v[u] = make_int4(0, 0, 0, 0);
-            if (s < S && sub < nvec) v[u] = ldg_hint(base + (int64_t)s * xs.s, pol);
+            if (s < s_end && sub < nvec) v[u] = ldg_hint(base + (int64_t)s * xs.s, pol);
         }
         float ssu[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             const uint32_t w[4] = {(uint32_t)v[u].x, (uint32_t)v[u].y, (uint32_t)v[u].z, (uint32_t)v[u].w};
-            float s0 = 0.f, s1 = 0.f;
+            float f0 = 0.f, f1 = 0.f;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const float2 f = F16Traits<T>::unpack2(w[j]);
-                s0 = fmaf(f.x, f.x, s0);
-                s1 = fmaf(f.y, f.y, s1);
+                f0 = fmaf(f.x, f.x, f0);
+                f1 = fmaf(f.y, f.y, f1);
             }
-            ssu[u] = s0 + s1;
+            ssu[u] = f0 + f1;
         }
         using RS = RowSums<LPR, U>;
         RS::reduce(ssu, sub);
         if ((sub & RS::kIdleMask) == 0) {
 #pragma unroll
-            for (int i = 0; i < RS::kSlots; ++i)
-                snorm[warp * TOK_PER_WARP + (it + RS::row_of(sub) + i) * RPW + rsel] = sqrtf(ssu[i]);
+            for (int i = 0; i < RS::kSlots; ++i) {
+                const int s = s0 + (RS::row_of(sub) + i) * RPW + rsel;
+                if (s < s_end) out[s] = sqrtf(ssu[i]);
+            }
         }
     }
 }

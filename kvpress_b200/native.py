@@ -293,7 +293,7 @@ class GraphedCall:
         self._fn = fn
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):  # warm-up off the capture: lazy inits (func attributes, side stream, ...)
+        with torch.cuda.stream(side):  # warm-up off the capture: lazy inits (func attributes, ...)
             for _ in range(max(1, warmup)):
                 fn()
         torch.cuda.current_stream().wait_stream(side)
