@@ -29,13 +29,10 @@
  *   - Selection rule: the n_kept largest scores per (b, h) row; ties at the threshold are
  *     resolved towards the LOWEST position (deterministic; torch.topk leaves it unspecified).
  *   - Caller owns all memory (outputs + workspace of kvp_workspace_bytes()). The library
- *     allocates no device memory and never synchronises the stream (kvp_workspace_check excepted). Process-wide state is limited to write-once caches of device
- *     properties (SM count, occupancy, function attributes) and, for the covariance-free ExpectedAttention
- *     scan with use_vnorm (the tensor-core kernels take the value norms themselves), ONE internal side
- *     stream + two events per device: the ||v|| kernel is forked onto it
- *     and joined back into the caller's stream before the call returns; host threads enqueueing
- *     ExpectedAttention calls on the same device serialise on a mutex for those few microseconds.
- *     Calls are re-entrant per (stream, workspace); every call is CUDA-graph capturable.
+ *     allocates no device memory and never synchronises the stream (kvp_workspace_check excepted).
+ *     Every kernel runs on the caller's stream. The only process-wide state is write-once caches of
+ *     per-device properties: SM count, occupancy and function attributes. Calls are re-entrant per
+ *     (stream, workspace); every call is CUDA-graph capturable.
  *   - Return value: KVP_OK (0) or a negative kvp_status. No exceptions cross this boundary.
  */
 #ifndef KVPRESS_B200_H

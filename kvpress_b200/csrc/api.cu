@@ -1,9 +1,8 @@
 // api.cu — the extern "C" surface declared in include/kvpress_b200.h.
 // Validates the problem, carves the caller's workspace and enqueues the kernels on the caller's
-// stream. Never allocates, never synchronises (except the *_host convenience call), never throws.
+// stream. Never allocates, never synchronises (except kvp_workspace_check), never throws.
 #include <stdio.h>
 #include <stdlib.h>
-#include <string.h>
 
 #include "common.cuh"
 
@@ -11,16 +10,19 @@ namespace kvp {
 
 static thread_local char g_last_cuda_error[256] = "";
 
-static int fail_cuda(cudaError_t e) {
-    snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e),
-             cudaGetErrorString(e));
+// kvp_status of a CUDA call. The KeyDiff, SnapKV and ExpectedAttention score launchers report a shape they have no
+// kernel for as cudaErrorNotSupported.
+static int status(cudaError_t e, int scorer = KVP_SCORER_GENERIC) {
+    if (e == cudaSuccess) return KVP_OK;
+    if (e == cudaErrorNotSupported && (scorer == KVP_SCORER_KEYDIFF || scorer == KVP_SCORER_SNAPKV ||
+                                       scorer == KVP_SCORER_EXPECTED_ATTENTION))
+        return KVP_ERR_UNSUPPORTED_SHAPE;
+    snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
     // launch-configuration errors are not sticky: clear them, or the cudaPeekAtLastError() of every later call
     // (of this library or of torch) would report this failure again
     cudaGetLastError();
     return KVP_ERR_CUDA;
 }
-
-static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 static int validate(const kvp_problem* p, Dims* d, bool need_kv_strides = true) {
     if (p == nullptr) return KVP_ERR_NULL_POINTER;
@@ -52,67 +54,118 @@ static int validate(const kvp_problem* p, Dims* d, bool need_kv_strides = true) 
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-struct WsLayout {
-    size_t keys_off, hist_off, sfx_off, meta_off, prefix_off, scorer_off, total;
-    int S_pad, n_tiles;
-    size_t hist_bytes, scorer_bytes;
-};
-
-static WsLayout layout(const Dims& d, int scorer, int window) {
-    WsLayout L;
-    L.n_tiles = (d.S + kTile - 1) / kTile;
-    L.S_pad = L.n_tiles * kTile;
-    size_t off = 0;
-    // one zeroed region (a single memset node per call): hist_hi, hist_lo, counters, tile_prefix
-    L.hist_off = off;
-    off = align_up(off + ((size_t)d.R * 256 * 2 + (size_t)d.R * 3 + 64) * sizeof(uint32_t), 256);
-    L.prefix_off = off;
-    off = align_up(off + (size_t)d.R * L.n_tiles * sizeof(uint2), 256);
-    L.hist_bytes = off - L.hist_off;
-    L.keys_off = off;
-    off = align_up(off + (size_t)d.R * L.S_pad * sizeof(uint16_t), 256);
-    L.sfx_off = off;
-    off = align_up(off + (size_t)d.R * L.n_tiles * kSfxStride * sizeof(uint16_t), 256);
-    L.meta_off = off;
-    off = align_up(off + (size_t)d.R * sizeof(uint2), 256);
-    L.scorer_off = off;
-    L.scorer_bytes = 0;
-    if (scorer == KVP_SCORER_SNAPKV) L.scorer_bytes = snapkv_scratch_bytes(d, window);
-    if (scorer == KVP_SCORER_EXPECTED_ATTENTION) L.scorer_bytes = ea_scratch_bytes(d);
-    if (scorer == KVP_SCORER_KEYDIFF) L.scorer_bytes = keydiff_scratch_bytes(d);
-    off = align_up(off + L.scorer_bytes, 256);
-    L.total = off;
-    return L;
-}
-
-static int carve(const Dims& d, int scorer, int window, void* workspace, size_t bytes,
-                 Workspace* ws, WsLayout* Lout) {
-    const WsLayout L = layout(d, scorer, window);
-    if (workspace == nullptr) return KVP_ERR_NULL_POINTER;
-    if (!aligned16(workspace)) return KVP_ERR_BAD_STRIDE;
-    if (bytes < L.total) return KVP_ERR_WORKSPACE_TOO_SMALL;
-    char* base = static_cast<char*>(workspace);
-    ws->hist_hi = reinterpret_cast<uint32_t*>(base + L.hist_off);
-    ws->hist_lo = ws->hist_hi + (size_t)d.R * 256;
-    ws->counters = ws->hist_lo + (size_t)d.R * 256;
-    ws->keys = reinterpret_cast<uint16_t*>(base + L.keys_off);
-    ws->tile_sfx = reinterpret_cast<uint16_t*>(base + L.sfx_off);
-    ws->row_meta = reinterpret_cast<uint2*>(base + L.meta_off);
-    ws->tile_prefix = reinterpret_cast<uint2*>(base + L.prefix_off);
+// The workspace of a call: sized when `base` is null, carved otherwise. Returns the total bytes and, in *zeroed, the
+// leading bytes every call clears with one memset: the histograms, the counters and the tile prefixes. The
+// histograms are whole KiB per row, so hist_lo and the counters follow hist_hi without padding.
+static size_t layout(const Dims& d, int scorer, int window, void* base, Workspace* ws, size_t* zeroed) {
+    Carve c(base);
     ws->R = d.R;
-    ws->scorer = base + L.scorer_off;
-    ws->scorer_bytes = L.scorer_bytes;
-    ws->S_pad = L.S_pad;
-    ws->n_tiles = L.n_tiles;
-    *Lout = L;
-    return KVP_OK;
+    ws->n_tiles = (d.S + kTile - 1) / kTile;
+    ws->S_pad = ws->n_tiles * kTile;
+    ws->hist_hi = c.take<uint32_t>((size_t)d.R * 256);
+    ws->hist_lo = c.take<uint32_t>((size_t)d.R * 256);
+    ws->counters = c.take<uint32_t>((size_t)d.R * 3 + 64);
+    ws->tile_prefix = c.take<uint2>((size_t)d.R * ws->n_tiles);
+    *zeroed = c.bytes;
+    ws->keys = c.take<uint16_t>((size_t)d.R * ws->S_pad);
+    ws->tile_sfx = c.take<uint16_t>((size_t)d.R * ws->n_tiles * kSfxStride);
+    ws->row_meta = c.take<uint2>(d.R);
+    ws->scorer_bytes = scorer == KVP_SCORER_SNAPKV               ? snapkv_scratch_bytes(d, window)
+                       : scorer == KVP_SCORER_EXPECTED_ATTENTION ? ea_scratch_bytes(d)
+                       : scorer == KVP_SCORER_KEYDIFF            ? keydiff_scratch_bytes(d)
+                                                                 : 0;
+    ws->scorer = c.take<char>(ws->scorer_bytes);
+    return c.bytes;
 }
+
+// One call on a carved workspace.
+struct Call {
+    Dims d;
+    Workspace ws;
+    size_t zeroed;  // see layout()
+    cudaStream_t st;
+    int carve(int scorer, int window, void* workspace, size_t bytes) {
+        if (workspace == nullptr) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(workspace)) return KVP_ERR_BAD_STRIDE;
+        return bytes < layout(d, scorer, window, workspace, &ws, &zeroed) ? KVP_ERR_WORKSPACE_TOO_SMALL : KVP_OK;
+    }
+    int zero() const { return status(cudaMemsetAsync(ws.hist_hi, 0, zeroed, st)); }
+};
 
 static int check_io(const void* K, const void* V, const void* K_out, const void* V_out) {
     if (!K || !V || !K_out || !V_out) return KVP_ERR_NULL_POINTER;
     if (!aligned16(K) || !aligned16(V) || !aligned16(K_out) || !aligned16(V_out))
         return KVP_ERR_BAD_STRIDE;
     return KVP_OK;
+}
+
+// K and V, where a compress call writes the kept rows, and how the selection stage treats them.
+struct Io {
+    const void* K;
+    const void* V;
+    void* K_out;
+    void* V_out;
+    int32_t* idx_out;
+    const float* inv_freq;  // kvp_scores_compress_rerotate: the kept keys are re-rotated
+};
+
+enum class Kind {
+    compress,  // selects and compacts K / V
+    select,    // kvp_scores_select: selects into idx_out; no K / V, so no K / V strides
+    score,     // scores only: no n_kept == 0 short cut, no selection
+};
+
+// The checks of every call that carves a workspace, in the order they are made (the first failure is returned):
+// validate -> n_kept == 0 short cut (compress, select) -> check_io (compress) -> the entry point's operand checks ->
+// carve. A compress or select call with c->d.n_kept == 0 on return has nothing to do.
+template <typename Operands>
+static int prepare(Kind kind, const kvp_problem* p, int scorer, int window, const Io& io, Operands operands,
+                   void* workspace, size_t workspace_bytes, kvp_stream_t stream, Call* c) {
+    int rc = validate(p, &c->d, kind != Kind::select);
+    if (rc) return rc;
+    if (kind != Kind::score && c->d.n_kept == 0) return KVP_OK;
+    if (kind == Kind::compress && (rc = check_io(io.K, io.V, io.K_out, io.V_out))) return rc;
+    if ((rc = operands(c->d))) return rc;
+    c->st = static_cast<cudaStream_t>(stream);
+    return c->carve(scorer, window, workspace, workspace_bytes);
+}
+
+// prepare -> memset (unless zero == false) -> score -> selection (compress, select).
+// `score(const Call&)` enqueues the score stage and returns its cudaError_t.
+template <typename Operands, typename Score>
+static int run(Kind kind, const kvp_problem* p, int scorer, int window, const Io& io, Operands operands, Score score,
+               void* workspace, size_t workspace_bytes, kvp_stream_t stream, bool zero = true) {
+    Call c;
+    int rc = prepare(kind, p, scorer, window, io, operands, workspace, workspace_bytes, stream, &c);
+    if (rc || (kind != Kind::score && c.d.n_kept == 0)) return rc;
+    if (zero && (rc = c.zero())) return rc;
+    if ((rc = status(score(c), scorer))) return rc;
+    if (kind == Kind::score) return KVP_OK;
+    if (io.inv_freq)
+        return status(launch_select_compact_rerotate(c.d, p->dtype, io.K, io.V, io.K_out, io.V_out, io.idx_out, c.ws,
+                                                     io.inv_freq, c.st));
+    if (kind == Kind::select) c.d.ks = c.d.vs = {0, 0, 0};
+    return status(launch_select_compact(c.d, io.K, io.V, io.K_out, io.V_out, io.idx_out, c.ws, c.st));
+}
+
+static int no_operands(const Dims&) { return KVP_OK; }
+
+enum class KnormPath { cluster, fused, two_kernels };
+
+// The kernels kvp_knorm_compress runs. `d` is null for a problem that failed validation: kvp_launches_per_compress
+// still counts one, by its size alone.
+static KnormPath knorm_path(const kvp_problem& p, const Dims* d) {
+    // DecodingPress-sized caches: one launch of the cluster kernel (knorm_cluster.cu), no memset, no scratch
+    if (d != nullptr && knorm_cluster_applicable(*d)) return KnormPath::cluster;
+    // Small caches beyond the cluster path are launch-latency-bound: one persistent kernel does score + select +
+    // compact. Large caches measured faster as two kernels (the fused kernel's mixed read/write item stream costs
+    // more HBM efficiency than the saved launch; K re-reads miss L2 anyway).
+    static const size_t fused_max_bytes = [] {  // A/B knob: KVP_KNORM_FUSED_MAX_MB (default 32)
+        const char* v = getenv("KVP_KNORM_FUSED_MAX_MB");
+        return (size_t)((v && *v) ? atoll(v) : 32) << 20;
+    }();
+    const size_t k_bytes = (size_t)p.B * p.Hkv * p.S * p.D * 2;
+    return k_bytes <= fused_max_bytes ? KnormPath::fused : KnormPath::two_kernels;
 }
 
 }  // namespace kvp
@@ -146,24 +199,23 @@ int kvp_workspace_bytes(const kvp_problem* p, int scorer, size_t* bytes_out) {
     if (rc) return rc;
     if (!bytes_out) return KVP_ERR_NULL_POINTER;
     // window only changes the SnapKV scratch; size for the largest supported window
-    *bytes_out = layout(d, scorer, 256).total;
+    Workspace ws;
+    size_t zeroed;
+    *bytes_out = layout(d, scorer, 256, nullptr, &ws, &zeroed);
     return KVP_OK;
 }
 
 int kvp_workspace_check(const kvp_problem* p, int scorer, const void* workspace, size_t workspace_bytes,
                         kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d, false);
-    if (rc) return rc;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, scorer, 256, const_cast<void*>(workspace), workspace_bytes, &ws, &L))) return rc;
+    Call c;
+    int rc = validate(p, &c.d, false);
+    if (rc || (rc = c.carve(scorer, 256, const_cast<void*>(workspace), workspace_bytes))) return rc;
     uint32_t flag = 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    cudaError_t e = cudaMemcpyAsync(&flag, ws.counters + kCounterErrSlot(d.R), sizeof(flag),
+    cudaError_t e = cudaMemcpyAsync(&flag, c.ws.counters + kCounterErrSlot(c.d.R), sizeof(flag),
                                     cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) return fail_cuda(e);
+    if (e != cudaSuccess) return status(e);
     return flag ? KVP_ERR_KERNEL_TIMEOUT : KVP_OK;
 }
 
@@ -174,18 +226,15 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         case KVP_SCORER_GENERIC: *launches_out = 3; break;  // memset, keys, select+compact
         case KVP_SCORER_KNORM: {  // cluster kernel | memset + (fused | score, select+compact)
             Dims d;
-            if (validate(p, &d, false) == KVP_OK && knorm_cluster_applicable(d)) *launches_out = 1;
-            else *launches_out = ((size_t)p->B * p->Hkv * p->S * p->D * 2 <= ((size_t)32 << 20)) ? 2 : 3;
+            const KnormPath path = knorm_path(*p, validate(p, &d, false) == KVP_OK ? &d : nullptr);
+            *launches_out = path == KnormPath::cluster ? 1 : path == KnormPath::fused ? 2 : 3;
             break;
         }
         case KVP_SCORER_KEYDIFF: *launches_out = 5; break;  // memset, anchor partials, merge, score, select+compact
         case KVP_SCORER_SNAPKV: *launches_out = 5; break;  // memset, stats, colsum, finalize, select+compact
-        case KVP_SCORER_EXPECTED_ATTENTION: {
-            // press defaults (use_covariance + use_vnorm): memset, logits (which also writes the value norms),
-            // finalize, select+compact
-            *launches_out = 4;
-            break;
-        }
+        // press defaults (use_covariance + use_vnorm): memset, logits (which also writes the value norms), finalize,
+        // select+compact
+        case KVP_SCORER_EXPECTED_ATTENTION: *launches_out = 4; break;
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -199,86 +248,47 @@ int kvp_knorm_score(const kvp_problem* p, const void* K, void* scores_out, kvp_s
     if (!K || !scores_out) return KVP_ERR_NULL_POINTER;
     if (!aligned16(K)) return KVP_ERR_BAD_STRIDE;
     Workspace ws = {};
-    cudaError_t e = launch_knorm_score(d, p->dtype, K, ws, scores_out, false,
-                                       static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? KVP_OK : fail_cuda(e);
-}
-
-static int select_and_compact(const Dims& d, const void* K, const void* V, void* K_out,
-                              void* V_out, int32_t* idx_out, const Workspace& ws,
-                              cudaStream_t st) {
-    cudaError_t e = launch_select_compact(d, K, V, K_out, V_out, idx_out, ws, st);
-    return e == cudaSuccess ? KVP_OK : fail_cuda(e);
+    return status(launch_knorm_score(d, p->dtype, K, ws, scores_out, false, static_cast<cudaStream_t>(stream)));
 }
 
 int kvp_knorm_compress(const kvp_problem* p, const void* K, const void* V, void* K_out,
                        void* V_out, int32_t* idx_out, void* scores_out, void* workspace,
                        size_t workspace_bytes, kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d);
-    if (rc) return rc;
-    if (d.n_kept == 0) return KVP_OK;
-    if ((rc = check_io(K, V, K_out, V_out))) return rc;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_KNORM, 0, workspace, workspace_bytes, &ws, &L))) return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // DecodingPress-sized caches: one launch of the cluster kernel (knorm_cluster.cu), no memset, no scratch
-    cudaError_t e = launch_knorm_cluster(d, p->dtype, K, V, K_out, V_out, idx_out, scores_out, st);
-    if (e != cudaErrorNotSupported) return e == cudaSuccess ? KVP_OK : fail_cuda(e);
-    e = cudaMemsetAsync(ws.hist_hi, 0, L.hist_bytes, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    // Small caches beyond the cluster path are launch-latency-bound: one persistent kernel does
-    // score + select + compact. Large caches measured faster as two kernels (the fused kernel's mixed
-    // read/write item stream costs more HBM efficiency than the saved launch; K re-reads miss L2 anyway).
-    const size_t k_bytes = (size_t)d.R * d.S * d.D * 2;
-    static const size_t fused_max_bytes = [] {  // A/B knob: KVP_KNORM_FUSED_MAX_MB (default 32)
-        const char* v = getenv("KVP_KNORM_FUSED_MAX_MB");
-        return (size_t)((v && *v) ? atoll(v) : 32) << 20;
-    }();
-    if (k_bytes <= fused_max_bytes) {
-        e = launch_knorm_fused(d, p->dtype, K, V, K_out, V_out, idx_out, scores_out, ws, st);
-        if (e != cudaErrorNotSupported) return e == cudaSuccess ? KVP_OK : fail_cuda(e);
+    const Io io = {K, V, K_out, V_out, idx_out, nullptr};
+    Call c;
+    int rc = prepare(Kind::compress, p, KVP_SCORER_KNORM, 0, io, no_operands, workspace, workspace_bytes, stream, &c);
+    if (rc || c.d.n_kept == 0) return rc;
+    const KnormPath path = knorm_path(*p, &c.d);
+    if (path == KnormPath::cluster)
+        return status(launch_knorm_cluster(c.d, p->dtype, K, V, K_out, V_out, idx_out, scores_out, c.st));
+    if ((rc = c.zero())) return rc;
+    if (path == KnormPath::fused) {
+        // cudaErrorNotSupported: more work items than the fused kernel's queue addresses; two kernels instead
+        const cudaError_t e = launch_knorm_fused(c.d, p->dtype, K, V, K_out, V_out, idx_out, scores_out, c.ws, c.st);
+        if (e != cudaErrorNotSupported) return status(e);
     }
-    e = launch_knorm_score(d, p->dtype, K, ws, scores_out, true, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    return select_and_compact(d, K, V, K_out, V_out, idx_out, ws, st);
+    if ((rc = status(launch_knorm_score(c.d, p->dtype, K, c.ws, scores_out, true, c.st)))) return rc;
+    return status(launch_select_compact(c.d, K, V, K_out, V_out, idx_out, c.ws, c.st));
 }
 
 // ---- KeyDiff -------------------------------------------------------------------------------------
 int kvp_keydiff_score(const kvp_problem* p, const void* K, void* scores_out, void* workspace,
                       size_t workspace_bytes, kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d);
-    if (rc) return rc;
-    if (!K || !scores_out) return KVP_ERR_NULL_POINTER;
-    if (!aligned16(K)) return KVP_ERR_BAD_STRIDE;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_KEYDIFF, 0, workspace, workspace_bytes, &ws, &L))) return rc;
-    cudaError_t e = launch_keydiff_score(d, p->dtype, K, ws, scores_out, false, static_cast<cudaStream_t>(stream));
-    if (e == cudaErrorNotSupported) return KVP_ERR_UNSUPPORTED_SHAPE;
-    return e == cudaSuccess ? KVP_OK : fail_cuda(e);
+    auto operands = [&](const Dims&) {
+        if (!K || !scores_out) return KVP_ERR_NULL_POINTER;
+        return aligned16(K) ? KVP_OK : KVP_ERR_BAD_STRIDE;
+    };
+    auto score = [&](const Call& c) { return launch_keydiff_score(c.d, p->dtype, K, c.ws, scores_out, false, c.st); };
+    // the score kernel writes no keys and no histogram when the selection is skipped: nothing to clear
+    return run(Kind::score, p, KVP_SCORER_KEYDIFF, 0, {}, operands, score, workspace, workspace_bytes, stream, false);
 }
 
 int kvp_keydiff_compress(const kvp_problem* p, const void* K, const void* V, void* K_out, void* V_out,
                          int32_t* idx_out, void* scores_out, void* workspace, size_t workspace_bytes,
                          kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d);
-    if (rc) return rc;
-    if (d.n_kept == 0) return KVP_OK;
-    if ((rc = check_io(K, V, K_out, V_out))) return rc;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_KEYDIFF, 0, workspace, workspace_bytes, &ws, &L))) return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    cudaError_t e = cudaMemsetAsync(ws.hist_hi, 0, L.hist_bytes, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    e = launch_keydiff_score(d, p->dtype, K, ws, scores_out, true, st);
-    if (e == cudaErrorNotSupported) return KVP_ERR_UNSUPPORTED_SHAPE;
-    if (e != cudaSuccess) return fail_cuda(e);
-    return select_and_compact(d, K, V, K_out, V_out, idx_out, ws, st);
+    auto score = [&](const Call& c) { return launch_keydiff_score(c.d, p->dtype, K, c.ws, scores_out, true, c.st); };
+    return run(Kind::compress, p, KVP_SCORER_KEYDIFF, 0, {K, V, K_out, V_out, idx_out, nullptr}, no_operands, score,
+               workspace, workspace_bytes, stream);
 }
 
 // ---- StreamingLLM --------------------------------------------------------------------------------
@@ -289,9 +299,7 @@ int kvp_streaming_score(const kvp_problem* p, int32_t n_sink, void* scores_out,
     if (rc) return rc;
     if (!scores_out) return KVP_ERR_NULL_POINTER;
     if (n_sink < 0) return KVP_ERR_BAD_ARGUMENT;
-    cudaError_t e = launch_streaming_score(d, p->dtype, n_sink, scores_out,
-                                           static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? KVP_OK : fail_cuda(e);
+    return status(launch_streaming_score(d, p->dtype, n_sink, scores_out, static_cast<cudaStream_t>(stream)));
 }
 
 int kvp_streaming_compress(const kvp_problem* p, int32_t n_sink, const void* K, const void* V,
@@ -302,80 +310,66 @@ int kvp_streaming_compress(const kvp_problem* p, int32_t n_sink, const void* K, 
     if (n_sink < 0) return KVP_ERR_BAD_ARGUMENT;
     if (d.n_kept == 0) return KVP_OK;
     if ((rc = check_io(K, V, K_out, V_out))) return rc;
-    cudaError_t e = launch_streaming_compress(d, n_sink, K, V, K_out, V_out, idx_out,
-                                              static_cast<cudaStream_t>(stream));
-    return e == cudaSuccess ? KVP_OK : fail_cuda(e);
+    return status(launch_streaming_compress(d, n_sink, K, V, K_out, V_out, idx_out, static_cast<cudaStream_t>(stream)));
 }
 
 // ---- SnapKV --------------------------------------------------------------------------------------
+static int snapkv_window_ok(const Dims& d, int32_t window, int32_t kernel_size) {
+    const bool ok = window > 0 && window < d.S && kernel_size > 0 && (kernel_size & 1) == 1;
+    return ok ? KVP_OK : KVP_ERR_BAD_ARGUMENT;
+}
+
+static auto snapkv_stage(const kvp_problem* p, const void* K, const void* q_window, int32_t window,
+                         int32_t kernel_size, void* scores_out) {
+    return [=](const Call& c) {
+        return launch_snapkv_score(c.d, p->dtype, K, q_window, window, kernel_size, c.ws, scores_out, c.st);
+    };
+}
+
 int kvp_snapkv_score(const kvp_problem* p, const void* K, const void* q_window, int32_t window,
                      int32_t kernel_size, void* scores_out, void* workspace,
                      size_t workspace_bytes, kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d);
-    if (rc) return rc;
-    if (!K || !q_window || !scores_out) return KVP_ERR_NULL_POINTER;
-    if (!aligned16(K) || !aligned16(q_window)) return KVP_ERR_BAD_STRIDE;
-    if (window <= 0 || window >= d.S || kernel_size <= 0 || (kernel_size & 1) == 0)
-        return KVP_ERR_BAD_ARGUMENT;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_SNAPKV, window, workspace, workspace_bytes, &ws, &L))) return rc;
-    cudaError_t e = cudaMemsetAsync(ws.hist_hi, 0, L.hist_bytes, static_cast<cudaStream_t>(stream));
-    if (e != cudaSuccess) return fail_cuda(e);
-    e = launch_snapkv_score(d, p->dtype, K, q_window, window, kernel_size, ws, scores_out, false,
-                            static_cast<cudaStream_t>(stream));
-    if (e == cudaErrorNotSupported) return KVP_ERR_UNSUPPORTED_SHAPE;
-    return e == cudaSuccess ? KVP_OK : fail_cuda(e);
+    auto operands = [&](const Dims& d) -> int {
+        if (!K || !q_window || !scores_out) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(K) || !aligned16(q_window)) return KVP_ERR_BAD_STRIDE;
+        return snapkv_window_ok(d, window, kernel_size);
+    };
+    return run(Kind::score, p, KVP_SCORER_SNAPKV, window, {}, operands,
+               snapkv_stage(p, K, q_window, window, kernel_size, scores_out), workspace, workspace_bytes, stream);
 }
 
 int kvp_snapkv_compress(const kvp_problem* p, const void* K, const void* V,
                         const void* q_window, int32_t window, int32_t kernel_size, void* K_out,
                         void* V_out, int32_t* idx_out, void* scores_out, void* workspace,
                         size_t workspace_bytes, kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d);
-    if (rc) return rc;
-    if (d.n_kept == 0) return KVP_OK;
-    if ((rc = check_io(K, V, K_out, V_out))) return rc;
-    if (!q_window) return KVP_ERR_NULL_POINTER;
-    if (!aligned16(q_window)) return KVP_ERR_BAD_STRIDE;
-    if (window <= 0 || window >= d.S || kernel_size <= 0 || (kernel_size & 1) == 0)
-        return KVP_ERR_BAD_ARGUMENT;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_SNAPKV, window, workspace, workspace_bytes, &ws, &L))) return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    cudaError_t e = cudaMemsetAsync(ws.hist_hi, 0, L.hist_bytes, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    e = launch_snapkv_score(d, p->dtype, K, q_window, window, kernel_size, ws, scores_out, true,
-                            st);
-    if (e == cudaErrorNotSupported) return KVP_ERR_UNSUPPORTED_SHAPE;
-    if (e != cudaSuccess) return fail_cuda(e);
-    return select_and_compact(d, K, V, K_out, V_out, idx_out, ws, st);
+    auto operands = [&](const Dims& d) -> int {
+        if (!q_window) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(q_window)) return KVP_ERR_BAD_STRIDE;
+        return snapkv_window_ok(d, window, kernel_size);
+    };
+    return run(Kind::compress, p, KVP_SCORER_SNAPKV, window, {K, V, K_out, V_out, idx_out, nullptr}, operands,
+               snapkv_stage(p, K, q_window, window, kernel_size, scores_out), workspace, workspace_bytes, stream);
 }
 
 // ---- ExpectedAttention ---------------------------------------------------------------------------
+static auto ea_stage(const kvp_problem* p, const void* K, const void* V, const void* mu, const void* cov,
+                     float epsilon, int32_t n_sink, int32_t use_vnorm, void* scores_out) {
+    return [=](const Call& c) {
+        return launch_ea_score(c.d, p->dtype, K, V, mu, cov, epsilon, n_sink, use_vnorm, c.ws, scores_out, c.st);
+    };
+}
+
 int kvp_expected_attention_score(const kvp_problem* p, const void* K, const void* V,
                                  const void* mu, const void* cov, float epsilon, int32_t n_sink,
                                  int32_t use_vnorm, void* scores_out, void* workspace,
                                  size_t workspace_bytes, kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d);
-    if (rc) return rc;
-    if (!K || !mu || !scores_out || (use_vnorm && !V)) return KVP_ERR_NULL_POINTER;
-    if (!aligned16(K) || !aligned16(mu) || (cov && !aligned16(cov))) return KVP_ERR_BAD_STRIDE;
-    if (n_sink < 0 || n_sink >= d.S) return KVP_ERR_BAD_ARGUMENT;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_EXPECTED_ATTENTION, 0, workspace, workspace_bytes, &ws, &L)))
-        return rc;
-    cudaError_t e = cudaMemsetAsync(ws.hist_hi, 0, L.hist_bytes, static_cast<cudaStream_t>(stream));
-    if (e != cudaSuccess) return fail_cuda(e);
-    e = launch_ea_score(d, p->dtype, K, V, mu, cov, epsilon, n_sink, use_vnorm, ws, scores_out, false,
-                        static_cast<cudaStream_t>(stream));
-    if (e == cudaErrorNotSupported) return KVP_ERR_UNSUPPORTED_SHAPE;
-    return e == cudaSuccess ? KVP_OK : fail_cuda(e);
+    auto operands = [&](const Dims& d) {
+        if (!K || !mu || !scores_out || (use_vnorm && !V)) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(K) || !aligned16(mu) || (cov && !aligned16(cov))) return KVP_ERR_BAD_STRIDE;
+        return (n_sink < 0 || n_sink >= d.S) ? KVP_ERR_BAD_ARGUMENT : KVP_OK;
+    };
+    return run(Kind::score, p, KVP_SCORER_EXPECTED_ATTENTION, 0, {}, operands,
+               ea_stage(p, K, V, mu, cov, epsilon, n_sink, use_vnorm, scores_out), workspace, workspace_bytes, stream);
 }
 
 int kvp_expected_attention_compress(const kvp_problem* p, const void* K, const void* V,
@@ -383,90 +377,52 @@ int kvp_expected_attention_compress(const kvp_problem* p, const void* K, const v
                                     int32_t n_sink, int32_t use_vnorm, void* K_out, void* V_out,
                                     int32_t* idx_out, void* scores_out, void* workspace,
                                     size_t workspace_bytes, kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d);
-    if (rc) return rc;
-    if (d.n_kept == 0) return KVP_OK;
-    if ((rc = check_io(K, V, K_out, V_out))) return rc;
-    if (!mu) return KVP_ERR_NULL_POINTER;
-    if (!aligned16(mu) || (cov && !aligned16(cov))) return KVP_ERR_BAD_STRIDE;
-    if (n_sink < 0 || n_sink >= d.S) return KVP_ERR_BAD_ARGUMENT;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_EXPECTED_ATTENTION, 0, workspace, workspace_bytes, &ws, &L)))
-        return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    cudaError_t e = cudaMemsetAsync(ws.hist_hi, 0, L.hist_bytes, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    e = launch_ea_score(d, p->dtype, K, V, mu, cov, epsilon, n_sink, use_vnorm, ws, scores_out,
-                        true, st);
-    if (e == cudaErrorNotSupported) return KVP_ERR_UNSUPPORTED_SHAPE;
-    if (e != cudaSuccess) return fail_cuda(e);
-    return select_and_compact(d, K, V, K_out, V_out, idx_out, ws, st);
+    // V is checked with the other cache operands even when the score does not read it (use_vnorm == 0)
+    auto operands = [&](const Dims& d) {
+        if (!mu) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(mu) || (cov && !aligned16(cov))) return KVP_ERR_BAD_STRIDE;
+        return (n_sink < 0 || n_sink >= d.S) ? KVP_ERR_BAD_ARGUMENT : KVP_OK;
+    };
+    return run(Kind::compress, p, KVP_SCORER_EXPECTED_ATTENTION, 0, {K, V, K_out, V_out, idx_out, nullptr}, operands,
+               ea_stage(p, K, V, mu, cov, epsilon, n_sink, use_vnorm, scores_out), workspace, workspace_bytes, stream);
 }
 
 // ---- generic scores ------------------------------------------------------------------------------
+// The score stage of caller-supplied scores: their ordered keys and histogram.
+static auto keys_from(const kvp_problem* p, const void* scores, const int64_t* score_stride) {
+    return [=](const Call& c) {
+        return launch_keys_from_scores(c.d, p->dtype, scores, score_stride[0], score_stride[1], c.ws, c.st);
+    };
+}
+
 int kvp_scores_compress(const kvp_problem* p, const void* scores, const int64_t* score_stride,
                         const void* K, const void* V, void* K_out, void* V_out,
                         int32_t* idx_out, void* workspace, size_t workspace_bytes,
                         kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d);
-    if (rc) return rc;
-    if (d.n_kept == 0) return KVP_OK;
-    if ((rc = check_io(K, V, K_out, V_out))) return rc;
-    if (!scores || !score_stride) return KVP_ERR_NULL_POINTER;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_GENERIC, 0, workspace, workspace_bytes, &ws, &L))) return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    cudaError_t e = cudaMemsetAsync(ws.hist_hi, 0, L.hist_bytes, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    e = launch_keys_from_scores(d, p->dtype, scores, score_stride[0], score_stride[1], ws, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    return select_and_compact(d, K, V, K_out, V_out, idx_out, ws, st);
+    auto operands = [&](const Dims&) { return (!scores || !score_stride) ? KVP_ERR_NULL_POINTER : KVP_OK; };
+    return run(Kind::compress, p, KVP_SCORER_GENERIC, 0, {K, V, K_out, V_out, idx_out, nullptr}, operands,
+               keys_from(p, scores, score_stride), workspace, workspace_bytes, stream);
 }
 
 int kvp_scores_select(const kvp_problem* p, const void* scores, const int64_t* score_stride,
                       int32_t* idx_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
-    Dims d;
-    int rc = validate(p, &d, false);
-    if (rc) return rc;
-    if (d.n_kept == 0) return KVP_OK;
-    if (!scores || !score_stride || !idx_out) return KVP_ERR_NULL_POINTER;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_GENERIC, 0, workspace, workspace_bytes, &ws, &L))) return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    cudaError_t e = cudaMemsetAsync(ws.hist_hi, 0, L.hist_bytes, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    e = launch_keys_from_scores(d, p->dtype, scores, score_stride[0], score_stride[1], ws, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    d.ks = d.vs = {0, 0, 0};
-    return select_and_compact(d, nullptr, nullptr, nullptr, nullptr, idx_out, ws, st);
+    auto operands = [&](const Dims&) { return (!scores || !score_stride || !idx_out) ? KVP_ERR_NULL_POINTER : KVP_OK; };
+    return run(Kind::select, p, KVP_SCORER_GENERIC, 0, {nullptr, nullptr, nullptr, nullptr, idx_out, nullptr},
+               operands, keys_from(p, scores, score_stride), workspace, workspace_bytes, stream);
 }
 
 int kvp_scores_compress_rerotate(const kvp_problem* p, const void* scores, const int64_t* score_stride,
                                  const void* K, const void* V, const float* inv_freq, void* K_out,
                                  void* V_out, int32_t* idx_out, void* workspace,
                                  size_t workspace_bytes, kvp_stream_t stream) {
+    // rotate_half pairs d with d + D/2; checked ahead of the n_kept == 0 short cut
     Dims d;
-    int rc = validate(p, &d);
-    if (rc) return rc;
-    if (d.D % 16 != 0) return KVP_ERR_UNSUPPORTED_SHAPE;  // rotate_half pairs d with d + D/2
-    if (d.n_kept == 0) return KVP_OK;
-    if ((rc = check_io(K, V, K_out, V_out))) return rc;
-    if (!scores || !score_stride || !inv_freq) return KVP_ERR_NULL_POINTER;
-    Workspace ws;
-    WsLayout L;
-    if ((rc = carve(d, KVP_SCORER_GENERIC, 0, workspace, workspace_bytes, &ws, &L))) return rc;
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    cudaError_t e = cudaMemsetAsync(ws.hist_hi, 0, L.hist_bytes, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    e = launch_keys_from_scores(d, p->dtype, scores, score_stride[0], score_stride[1], ws, st);
-    if (e != cudaSuccess) return fail_cuda(e);
-    e = launch_select_compact_rerotate(d, p->dtype, K, V, K_out, V_out, idx_out, ws, inv_freq, st);
-    return e == cudaSuccess ? KVP_OK : fail_cuda(e);
+    if (validate(p, &d) == KVP_OK && d.D % 16 != 0) return KVP_ERR_UNSUPPORTED_SHAPE;
+    auto operands = [&](const Dims&) {
+        return (!scores || !score_stride || !inv_freq) ? KVP_ERR_NULL_POINTER : KVP_OK;
+    };
+    return run(Kind::compress, p, KVP_SCORER_GENERIC, 0, {K, V, K_out, V_out, idx_out, inv_freq}, operands,
+               keys_from(p, scores, score_stride), workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -31,7 +31,7 @@ struct Strides3 {
     int64_t b, h, s;
 };
 
-// Device view of the scratch area (carved by carve_workspace in api.cu).
+// Device view of the scratch area (laid out by layout() in api.cu).
 struct Workspace {
     uint16_t* keys;      // [R][S_pad] ordered 16-bit keys of the scores
     uint32_t* hist_hi;   // [R][256]   histogram of key >> 8
@@ -290,6 +290,23 @@ static inline int cached_ctas_per_sm(Kern kern, int threads, PerDeviceInt& cache
     return cache.v[dev];
 }
 
+// ---- host: workspace layouts ------------------------------------------------------------------
+inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
+
+// Hands out consecutive regions of a buffer, each 256-byte aligned. With a null base every region is null and only
+// `bytes` is tallied, so one function both sizes a layout and carves it.
+struct Carve {
+    char* base;
+    size_t bytes = 0;
+    explicit Carve(void* b) : base(static_cast<char*>(b)) {}
+    template <typename T>
+    T* take(size_t count) {
+        T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+        bytes = align256(bytes + count * sizeof(T));
+        return p;
+    }
+};
+
 // ---- launchers implemented in the .cu files (host, C++ linkage) -------------------------------
 cudaError_t launch_knorm_score(const Dims& d, int dtype, const void* K, const Workspace& ws,
                                void* scores_out, bool want_keys, cudaStream_t st);
@@ -316,7 +333,7 @@ cudaError_t launch_streaming_compress(const Dims& d, int n_sink, const void* K, 
 size_t snapkv_scratch_bytes(const Dims& d, int window);
 cudaError_t launch_snapkv_score(const Dims& d, int dtype, const void* K, const void* q_window,
                                 int window, int kernel_size, const Workspace& ws,
-                                void* scores_out, bool want_keys, cudaStream_t st);
+                                void* scores_out, cudaStream_t st);
 size_t keydiff_scratch_bytes(const Dims& d);
 cudaError_t launch_keydiff_score(const Dims& d, int dtype, const void* K, const Workspace& ws,
                                  void* scores_out, bool want_keys, cudaStream_t st);
@@ -325,7 +342,6 @@ cudaError_t launch_fill_sentinel(int dtype, void* scores_out, int R, int S, int 
                                  const Workspace& ws, cudaStream_t st);
 cudaError_t launch_ea_score(const Dims& d, int dtype, const void* K, const void* V, const void* mu,
                             const void* cov, float eps, int n_sink, int use_vnorm,
-                            const Workspace& ws, void* scores_out, bool want_keys,
-                            cudaStream_t st);
+                            const Workspace& ws, void* scores_out, cudaStream_t st);
 
 }  // namespace kvp

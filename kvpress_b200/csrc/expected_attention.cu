@@ -36,28 +36,24 @@ struct EaScratch {
     float2* partial;  // [R][G][n_parts] (max, sum exp) per CTA part
 };
 
-static inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
-
-size_t ea_scratch_bytes(const Dims& d) {
+// The scratch in ws.scorer; with a null base only its size (*bytes).
+static EaScratch carve_ea(const Dims& d, void* base, size_t* bytes = nullptr) {
     const int G = d.Hq / d.H;
     const size_t S_pad = (size_t)((d.S + kTile - 1) / kTile) * kTile;
     const size_t n_parts = (size_t)((d.S + kScoreChunkGeneric - 1) / kScoreChunkGeneric);
-    const size_t parts = n_parts > kEaMaxParts ? n_parts : kEaMaxParts;
-    return align256((size_t)d.R * G * S_pad * 4) + align256((size_t)d.R * S_pad * 4) +
-           align256((size_t)d.R * G * parts * sizeof(float2));
+    Carve c(base);
+    EaScratch s;
+    s.logits = c.take<float>((size_t)d.R * G * S_pad);
+    s.vnorm = c.take<float>((size_t)d.R * S_pad);
+    s.partial = c.take<float2>((size_t)d.R * G * (n_parts > kEaMaxParts ? n_parts : kEaMaxParts));
+    if (bytes) *bytes = c.bytes;
+    return s;
 }
 
-static EaScratch carve_ea(const Dims& d, const Workspace& ws) {
-    const int G = d.Hq / d.H;
-    const size_t S_pad = (size_t)ws.S_pad;
-    char* p = static_cast<char*>(ws.scorer);
-    EaScratch s;
-    s.logits = reinterpret_cast<float*>(p);
-    p += align256((size_t)d.R * G * S_pad * 4);
-    s.vnorm = reinterpret_cast<float*>(p);
-    p += align256((size_t)d.R * S_pad * 4);
-    s.partial = reinterpret_cast<float2*>(p);
-    return s;
+size_t ea_scratch_bytes(const Dims& d) {
+    size_t bytes;
+    carve_ea(d, nullptr, &bytes);
+    return bytes;
 }
 
 // ---- shared-memory carve-up of ea_logits_kernel ---------------------------------------------------
@@ -607,7 +603,7 @@ static cudaError_t launch_ea_t(const Dims& d, int dtype, const void* K, const vo
     const int G = d.Hq / d.H;
     if (G > 8) return cudaErrorNotSupported;
     const int nvec = d.D / 8;
-    const EaScratch sc = carve_ea(d, ws);
+    const EaScratch sc = carve_ea(d, ws.scorer);
     int n_parts = 0;
     cudaError_t e = cudaSuccess;
     // the logits kernels also write the value norms (use_vnorm): V is not touched otherwise and may be null
@@ -654,9 +650,8 @@ static cudaError_t launch_ea_t(const Dims& d, int dtype, const void* K, const vo
 
 cudaError_t launch_ea_score(const Dims& d, int dtype, const void* K, const void* V, const void* mu,
                             const void* cov, float eps, int n_sink, int use_vnorm,
-                            const Workspace& ws, void* scores_out, bool want_keys,
-                            cudaStream_t st) {
-    (void)want_keys;  // keys + histogram are always produced; the select stage is skipped by the caller
+                            const Workspace& ws, void* scores_out, cudaStream_t st) {
+    // keys + histogram are always produced; a score-only call skips the select stage
     if (dtype == KVP_BF16)
         return launch_ea_t<__nv_bfloat16>(d, dtype, K, V, mu, cov, eps, n_sink, use_vnorm, ws, scores_out, st);
     return launch_ea_t<__half>(d, dtype, K, V, mu, cov, eps, n_sink, use_vnorm, ws, scores_out, st);

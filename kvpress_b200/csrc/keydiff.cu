@@ -26,24 +26,22 @@ struct KeyDiffScratch {
     float* anorm;    // [R]     max(||anchor||, 1e-8)
 };
 
-static inline size_t kd_align256(size_t x) { return (x + 255) / 256 * 256; }
-
-size_t keydiff_scratch_bytes(const Dims& d) {
+// The scratch in ws.scorer; with a null base only its size (*bytes).
+static KeyDiffScratch carve_keydiff(const Dims& d, void* base, size_t* bytes = nullptr) {
     const size_t n_chunks = (size_t)((d.S + kScoreChunk - 1) / kScoreChunk);
-    return kd_align256((size_t)d.R * n_chunks * d.D * 4) + kd_align256((size_t)d.R * d.D * 4) +
-           kd_align256((size_t)d.R * 4);
+    Carve c(base);
+    KeyDiffScratch s;
+    s.partial = c.take<float>((size_t)d.R * n_chunks * d.D);
+    s.anchor = c.take<float>((size_t)d.R * d.D);
+    s.anorm = c.take<float>(d.R);
+    if (bytes) *bytes = c.bytes;
+    return s;
 }
 
-static KeyDiffScratch carve_keydiff(const Dims& d, const Workspace& ws) {
-    const size_t n_chunks = (size_t)((d.S + kScoreChunk - 1) / kScoreChunk);
-    char* p = static_cast<char*>(ws.scorer);
-    KeyDiffScratch s;
-    s.partial = reinterpret_cast<float*>(p);
-    p += kd_align256((size_t)d.R * n_chunks * d.D * 4);
-    s.anchor = reinterpret_cast<float*>(p);
-    p += kd_align256((size_t)d.R * d.D * 4);
-    s.anorm = reinterpret_cast<float*>(p);
-    return s;
+size_t keydiff_scratch_bytes(const Dims& d) {
+    size_t bytes;
+    carve_keydiff(d, nullptr, &bytes);
+    return bytes;
 }
 
 // ---- pass 1: per-CTA partial sums of the normalised keys ------------------------------------------
@@ -248,7 +246,7 @@ template <typename T>
 static cudaError_t launch_keydiff_t(const Dims& d, const void* K, const Workspace& ws, void* scores_out,
                                     bool want_keys, cudaStream_t st) {
     if (d.D > 256) return cudaErrorNotSupported;
-    const KeyDiffScratch sc = carve_keydiff(d, ws);
+    const KeyDiffScratch sc = carve_keydiff(d, ws.scorer);
     const int n_chunks = (d.S + kScoreChunk - 1) / kScoreChunk;
     dim3 grid(n_chunks, d.R);
     const int nvec = d.D / 8;

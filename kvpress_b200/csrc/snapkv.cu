@@ -43,24 +43,22 @@ struct SnapScratch {
     float* colsum;    // [R][S_pad]        sum_r p[r, j]
 };
 
-static inline size_t sn_align(size_t x) { return (x + 255) / 256 * 256; }
-
-size_t snapkv_scratch_bytes(const Dims& d, int window) {
-    const int G = d.Hq / d.H;
-    const size_t NQ = (size_t)G * window;
+// The scratch in ws.scorer; with a null base only its size (*bytes).
+static SnapScratch carve_snap(const Dims& d, int window, void* base, size_t* bytes = nullptr) {
+    const size_t NQ = (size_t)(d.Hq / d.H) * window;
     const size_t S_pad = (size_t)((d.S + kTile - 1) / kTile) * kTile;
-    return sn_align((size_t)d.R * NQ * kSnMaxParts * sizeof(float2)) + sn_align((size_t)d.R * S_pad * 4);
+    Carve c(base);
+    SnapScratch s;
+    s.partial = c.take<float2>((size_t)d.R * NQ * kSnMaxParts);
+    s.colsum = c.take<float>((size_t)d.R * S_pad);
+    if (bytes) *bytes = c.bytes;
+    return s;
 }
 
-static SnapScratch carve_snap(const Dims& d, int window, const Workspace& ws) {
-    const int G = d.Hq / d.H;
-    const size_t NQ = (size_t)G * window;
-    char* p = static_cast<char*>(ws.scorer);
-    SnapScratch s;
-    s.partial = reinterpret_cast<float2*>(p);
-    p += sn_align((size_t)d.R * NQ * kSnMaxParts * sizeof(float2));
-    s.colsum = reinterpret_cast<float*>(p);
-    return s;
+size_t snapkv_scratch_bytes(const Dims& d, int window) {
+    size_t bytes;
+    carve_snap(d, window, nullptr, &bytes);
+    return bytes;
 }
 
 // Shared-memory layout shared by both passes. Q is resident ([NQP rows x D], K-major SW128 panels),
@@ -445,7 +443,7 @@ static cudaError_t launch_snap_t(const Dims& d, int dtype, const void* K, const 
     const int sm_count = device_sm_count();
     const int G = d.Hq / d.H;
     const int NQ = G * window;
-    const SnapScratch sc = carve_snap(d, window, ws);
+    const SnapScratch sc = carve_snap(d, window, ws.scorer);
     const int n_tiles128 = (d.S + kSnTile - 1) / kSnTile;
     int ctas_per_row = sm_count / d.R;
     if (ctas_per_row < 1) ctas_per_row = 1;
@@ -521,9 +519,7 @@ static cudaError_t launch_snap_d(const Dims& d, int dtype, const void* K, const 
 }
 
 cudaError_t launch_snapkv_score(const Dims& d, int dtype, const void* K, const void* q_window, int window,
-                                int kernel_size, const Workspace& ws, void* scores_out, bool want_keys,
-                                cudaStream_t st) {
-    (void)want_keys;
+                                int kernel_size, const Workspace& ws, void* scores_out, cudaStream_t st) {
     if (dtype == KVP_BF16)
         return launch_snap_d<__nv_bfloat16>(d, dtype, K, q_window, window, kernel_size, ws, scores_out, st);
     return launch_snap_d<__half>(d, dtype, K, q_window, window, kernel_size, ws, scores_out, st);

@@ -7,6 +7,7 @@ library is missing or a tensor is not a CUDA tensor, calls raise.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import os
 from pathlib import Path
@@ -202,15 +203,7 @@ def _ptr(t: Optional[torch.Tensor]) -> int:
     return 0 if t is None else t.data_ptr()
 
 
-class _NoGuard:
-    def __enter__(self):
-        return None
-
-    def __exit__(self, *a):
-        return False
-
-
-_NO_GUARD = _NoGuard()
+_NO_GUARD = contextlib.nullcontext()
 
 
 def _guard(device: torch.device):
@@ -243,16 +236,6 @@ def launches_per_compress(p: KvpProblem, scorer: int) -> int:
     return int(out.value)
 
 
-def _alloc_out(keys: torch.Tensor, n_kept: int, want_idx: bool, want_scores: bool):
-    B, H, S, D = keys.shape
-    dev = _out_device(keys)
-    k_out = torch.empty((B, H, n_kept, D), dtype=keys.dtype, device=dev)
-    v_out = torch.empty_like(k_out)
-    idx = torch.empty((B, H, n_kept), dtype=torch.int32, device=dev) if want_idx else None
-    scores = torch.empty((B, H, S), dtype=keys.dtype, device=dev) if want_scores else None
-    return k_out, v_out, idx, scores
-
-
 _WS_CACHE: dict = {}
 
 
@@ -280,12 +263,11 @@ def _workspace(p: KvpProblem, scorer: int, device) -> torch.Tensor:
 class GraphedCall:
     """`fn()` (any sequence of native.* calls on fixed input tensors) captured into a CUDA graph.
 
-    The C-ABI calls only enqueue kernels / memset nodes on the current stream (the ExpectedAttention side
-    stream forks from and joins back into it), never synchronise and never allocate, so they are capturable
-    as they are. `replay()` costs one cudaGraphLaunch on the host instead of 1-6 launches + their argument
-    marshalling: it makes the call GPU-bound on any host (DecodingPress compactions, repeated same-shape
-    prefill layers, bench.py). Outputs are the tensors `fn` returned; they are overwritten by every replay.
-    The inputs must stay alive and at the same addresses (update them in place)."""
+    The C-ABI calls only enqueue kernels / memset nodes on the current stream, never synchronise and never
+    allocate, so they are capturable as they are. `replay()` costs one cudaGraphLaunch on the host instead of
+    1-6 launches + their argument marshalling: it makes the call GPU-bound on any host (DecodingPress
+    compactions, repeated same-shape prefill layers, bench.py). Outputs are the tensors `fn` returned; they are
+    overwritten by every replay. The inputs must stay alive and at the same addresses (update them in place)."""
 
     def __init__(self, fn, warmup: int = 2):
         if not torch.cuda.is_available():
@@ -320,35 +302,58 @@ def workspace_check(p: KvpProblem, scorer: int, workspace: torch.Tensor) -> None
            "kvp_workspace_check")
 
 
+def _enqueue(name: str, device: torch.device, p: KvpProblem, *args, scorer: Optional[int] = None) -> None:
+    """Enqueues the C-ABI call `name` as (p, *args, [workspace, its bytes,] stream) on the current stream of `device`.
+    Tensors and None in `args` are passed as addresses; `scorer` names the workspace of a call that takes one."""
+    args = [_ptr(a) if a is None or isinstance(a, torch.Tensor) else a for a in args]
+    with _guard(device):
+        if scorer is not None:
+            ws = _workspace(p, scorer, device)
+            args += [_ptr(ws), ws.numel()]
+        _check(getattr(load(), name)(ctypes.byref(p), *args, _stream()), name)
+
+
+def _score(name: str, scorer: Optional[int], keys: torch.Tensor, p: KvpProblem, *inputs) -> torch.Tensor:
+    """Scores [B, Hkv, S] of a score call (p, *inputs, scores[, workspace], stream)."""
+    scores = torch.empty(keys.shape[:3], dtype=keys.dtype, device=keys.device)
+    _enqueue(name, keys.device, p, *inputs, scores, scorer=scorer)
+    return scores
+
+
+def _compress(name: str, scorer: Optional[int], keys: torch.Tensor, values: torch.Tensor, n_kept: int, inputs: tuple,
+              return_indices: bool, return_scores: Optional[bool] = None, num_q_heads: Optional[int] = None):
+    """Outputs of a compress call (p, *inputs, K_out, V_out, idx[, scores][, workspace], stream), enqueued unless
+    n_kept == 0: (k_out, v_out, idx, scores), or (k_out, v_out, idx) for a call without a scores output
+    (return_scores None). The outputs' device guards the call: pinned host keys have none."""
+    p = make_problem(keys, values, n_kept, num_q_heads)
+    B, H, S, D = keys.shape
+    dev = _out_device(keys)
+    k_out = torch.empty((B, H, n_kept, D), dtype=keys.dtype, device=dev)
+    v_out = torch.empty_like(k_out)
+    idx = torch.empty((B, H, n_kept), dtype=torch.int32, device=dev) if return_indices else None
+    outs = (k_out, v_out, idx)
+    if return_scores is not None:
+        outs += (torch.empty((B, H, S), dtype=keys.dtype, device=dev) if return_scores else None,)
+    if n_kept > 0:
+        _enqueue(name, dev, p, *inputs, *outs, scorer=scorer)
+    return outs
+
+
 # --------------------------------------------------------------------------------------------------
 # Knorm
 # --------------------------------------------------------------------------------------------------
 def knorm_score(keys: torch.Tensor) -> torch.Tensor:
     _require_cuda_kv(keys, keys)
     keys = _normalise(keys)
-    p = make_problem(keys, keys, 0)
-    scores = torch.empty(keys.shape[:3], dtype=keys.dtype, device=keys.device)
-    with _guard(keys.device):
-        _check(load().kvp_knorm_score(ctypes.byref(p), _ptr(keys), _ptr(scores), _stream()), "kvp_knorm_score")
-    return scores
+    return _score("kvp_knorm_score", None, keys, make_problem(keys, keys, 0), keys)
 
 
 def knorm_compress(keys, values, n_kept: int, return_indices: bool = False, return_scores: bool = False,
                    _pinned_values: bool = False):
     _require_cuda_kv(keys, values, pinned_values=_pinned_values)
     keys, values = _normalise(keys), _normalise(values)
-    p = make_problem(keys, values, n_kept)
-    k_out, v_out, idx, scores = _alloc_out(keys, n_kept, return_indices, return_scores)
-    if n_kept > 0:
-        with _guard(keys.device):
-            ws = _workspace(p, SCORER_KNORM, keys.device)
-            _check(
-                load().kvp_knorm_compress(
-                    ctypes.byref(p), _ptr(keys), _ptr(values), _ptr(k_out), _ptr(v_out), _ptr(idx), _ptr(scores),
-                    _ptr(ws), ws.numel(), _stream()),
-                "kvp_knorm_compress",
-            )
-    return k_out, v_out, idx, scores
+    return _compress("kvp_knorm_compress", SCORER_KNORM, keys, values, n_kept, (keys, values), return_indices,
+                     return_scores)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -357,31 +362,15 @@ def knorm_compress(keys, values, n_kept: int, return_indices: bool = False, retu
 def keydiff_score(keys: torch.Tensor) -> torch.Tensor:
     _require_cuda_kv(keys, keys)
     keys = _normalise(keys)
-    p = make_problem(keys, keys, 0)
-    scores = torch.empty(keys.shape[:3], dtype=keys.dtype, device=keys.device)
-    with _guard(keys.device):
-        ws = _workspace(p, SCORER_KEYDIFF, keys.device)
-        _check(load().kvp_keydiff_score(ctypes.byref(p), _ptr(keys), _ptr(scores), _ptr(ws), ws.numel(), _stream()),
-               "kvp_keydiff_score")
-    return scores
+    return _score("kvp_keydiff_score", SCORER_KEYDIFF, keys, make_problem(keys, keys, 0), keys)
 
 
 def keydiff_compress(keys, values, n_kept: int, return_indices: bool = False, return_scores: bool = False,
                      _pinned_values: bool = False):
     _require_cuda_kv(keys, values, pinned_values=_pinned_values)
     keys, values = _normalise(keys), _normalise(values)
-    p = make_problem(keys, values, n_kept)
-    k_out, v_out, idx, scores = _alloc_out(keys, n_kept, return_indices, return_scores)
-    if n_kept > 0:
-        with _guard(keys.device):
-            ws = _workspace(p, SCORER_KEYDIFF, keys.device)
-            _check(
-                load().kvp_keydiff_compress(
-                    ctypes.byref(p), _ptr(keys), _ptr(values), _ptr(k_out), _ptr(v_out), _ptr(idx), _ptr(scores),
-                    _ptr(ws), ws.numel(), _stream()),
-                "kvp_keydiff_compress",
-            )
-    return k_out, v_out, idx, scores
+    return _compress("kvp_keydiff_compress", SCORER_KEYDIFF, keys, values, n_kept, (keys, values), return_indices,
+                     return_scores)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -389,27 +378,14 @@ def keydiff_compress(keys, values, n_kept: int, return_indices: bool = False, re
 # --------------------------------------------------------------------------------------------------
 def streaming_score(keys: torch.Tensor, n_kept: int, n_sink: int) -> torch.Tensor:
     _require_cuda_kv(keys, keys)
-    p = make_problem(keys, keys, n_kept)
-    scores = torch.empty(keys.shape[:3], dtype=keys.dtype, device=keys.device)
-    with _guard(keys.device):
-        _check(load().kvp_streaming_score(ctypes.byref(p), n_sink, _ptr(scores), _stream()), "kvp_streaming_score")
-    return scores
+    return _score("kvp_streaming_score", None, keys, make_problem(keys, keys, n_kept), n_sink)
 
 
 def streaming_compress(keys, values, n_kept: int, n_sink: int, return_indices: bool = False,
                        _pinned_kv: bool = False):
     _require_cuda_kv(keys, values, pinned_values=_pinned_kv, pinned_keys=_pinned_kv)
     keys, values = _normalise(keys), _normalise(values)
-    p = make_problem(keys, values, n_kept)
-    k_out, v_out, idx, _ = _alloc_out(keys, n_kept, return_indices, False)
-    if n_kept > 0:
-        with _guard(k_out.device):
-            _check(
-                load().kvp_streaming_compress(
-                    ctypes.byref(p), n_sink, _ptr(keys), _ptr(values), _ptr(k_out), _ptr(v_out), _ptr(idx), _stream()),
-                "kvp_streaming_compress",
-            )
-    return k_out, v_out, idx
+    return _compress("kvp_streaming_compress", None, keys, values, n_kept, (n_sink, keys, values), return_indices)
 
 
 # --------------------------------------------------------------------------------------------------
@@ -429,16 +405,7 @@ def snapkv_score(keys, q_window, window: int, kernel_size: int) -> torch.Tensor:
     keys = _normalise(keys)
     q_window = _check_q(q_window, keys, window)
     p = make_problem(keys, keys, 0, q_window.shape[1])
-    scores = torch.empty(keys.shape[:3], dtype=keys.dtype, device=keys.device)
-    with _guard(keys.device):
-        ws = _workspace(p, SCORER_SNAPKV, keys.device)
-        _check(
-            load().kvp_snapkv_score(
-                ctypes.byref(p), _ptr(keys), _ptr(q_window), window, kernel_size, _ptr(scores), _ptr(ws), ws.numel(),
-                _stream()),
-            "kvp_snapkv_score",
-        )
-    return scores
+    return _score("kvp_snapkv_score", SCORER_SNAPKV, keys, p, keys, q_window, window, kernel_size)
 
 
 def snapkv_compress(keys, values, q_window, window: int, kernel_size: int, n_kept: int,
@@ -446,18 +413,8 @@ def snapkv_compress(keys, values, q_window, window: int, kernel_size: int, n_kep
     _require_cuda_kv(keys, values, pinned_values=_pinned_values)
     keys, values = _normalise(keys), _normalise(values)
     q_window = _check_q(q_window, keys, window)
-    p = make_problem(keys, values, n_kept, q_window.shape[1])
-    k_out, v_out, idx, scores = _alloc_out(keys, n_kept, return_indices, return_scores)
-    if n_kept > 0:
-        with _guard(keys.device):
-            ws = _workspace(p, SCORER_SNAPKV, keys.device)
-            _check(
-                load().kvp_snapkv_compress(
-                    ctypes.byref(p), _ptr(keys), _ptr(values), _ptr(q_window), window, kernel_size, _ptr(k_out),
-                    _ptr(v_out), _ptr(idx), _ptr(scores), _ptr(ws), ws.numel(), _stream()),
-                "kvp_snapkv_compress",
-            )
-    return k_out, v_out, idx, scores
+    return _compress("kvp_snapkv_compress", SCORER_SNAPKV, keys, values, n_kept,
+                     (keys, values, q_window, window, kernel_size), return_indices, return_scores, q_window.shape[1])
 
 
 # --------------------------------------------------------------------------------------------------
@@ -480,16 +437,8 @@ def expected_attention_score(keys, values, mu, cov, epsilon: float, n_sink: int,
     keys, values = _normalise(keys), _normalise(values)
     mu, cov = _check_stats(mu, cov, keys)
     p = make_problem(keys, values, 0, mu.shape[1])
-    scores = torch.empty(keys.shape[:3], dtype=keys.dtype, device=keys.device)
-    with _guard(keys.device):
-        ws = _workspace(p, SCORER_EXPECTED_ATTENTION, keys.device)
-        _check(
-            load().kvp_expected_attention_score(
-                ctypes.byref(p), _ptr(keys), _ptr(values), _ptr(mu), _ptr(cov), float(epsilon), n_sink,
-                int(bool(use_vnorm)), _ptr(scores), _ptr(ws), ws.numel(), _stream()),
-            "kvp_expected_attention_score",
-        )
-    return scores
+    return _score("kvp_expected_attention_score", SCORER_EXPECTED_ATTENTION, keys, p, keys, values, mu, cov,
+                  float(epsilon), n_sink, int(bool(use_vnorm)))
 
 
 def expected_attention_compress(keys, values, mu, cov, epsilon: float, n_sink: int, use_vnorm: bool, n_kept: int,
@@ -497,24 +446,29 @@ def expected_attention_compress(keys, values, mu, cov, epsilon: float, n_sink: i
     _require_cuda_kv(keys, values)
     keys, values = _normalise(keys), _normalise(values)
     mu, cov = _check_stats(mu, cov, keys)
-    p = make_problem(keys, values, n_kept, mu.shape[1])
-    k_out, v_out, idx, scores = _alloc_out(keys, n_kept, return_indices, return_scores)
-    if n_kept > 0:
-        with _guard(keys.device):
-            ws = _workspace(p, SCORER_EXPECTED_ATTENTION, keys.device)
-            _check(
-                load().kvp_expected_attention_compress(
-                    ctypes.byref(p), _ptr(keys), _ptr(values), _ptr(mu), _ptr(cov), float(epsilon), n_sink,
-                    int(bool(use_vnorm)), _ptr(k_out), _ptr(v_out), _ptr(idx), _ptr(scores), _ptr(ws), ws.numel(),
-                    _stream()),
-                "kvp_expected_attention_compress",
-            )
-    return k_out, v_out, idx, scores
+    return _compress("kvp_expected_attention_compress", SCORER_EXPECTED_ATTENTION, keys, values, n_kept,
+                     (keys, values, mu, cov, float(epsilon), n_sink, int(bool(use_vnorm))), return_indices,
+                     return_scores, mu.shape[1])
 
 
 # --------------------------------------------------------------------------------------------------
 # generic scores (wrapper presses, user-defined ScorerPress subclasses)
 # --------------------------------------------------------------------------------------------------
+def _unit_stride_scores(scores: torch.Tensor):
+    """[B, H, S] scores with unit stride along S (copied only when needed) and their (b, h) element strides for the
+    C ABI, 0 along a dim of size 1."""
+    if scores.stride(2) != 1:
+        scores = scores.contiguous()
+    return scores, (ctypes.c_int64 * 2)(*(scores.stride(d) if scores.shape[d] > 1 else 0 for d in range(2)))
+
+
+def _caller_scores(scores: torch.Tensor, keys: torch.Tensor):
+    """Caller-supplied scores of the cache `keys`, checked and cast to its dtype; see _unit_stride_scores."""
+    if tuple(scores.shape) != tuple(keys.shape[:3]) or scores.device != keys.device:
+        raise RuntimeError(f"scores must be [B, Hkv, S] on the cache device, got {tuple(scores.shape)}")
+    return _unit_stride_scores(scores.to(keys.dtype))
+
+
 def scores_compress(scores: torch.Tensor, keys, values, n_kept: int, return_indices: bool = False):
     """Top-k + compaction for caller-supplied scores [B, Hkv, S] (wrapper presses, user ScorerPress subclasses).
 
@@ -524,25 +478,9 @@ def scores_compress(scores: torch.Tensor, keys, values, n_kept: int, return_indi
     `topk` would still order them."""
     _require_cuda_kv(keys, values)
     keys, values = _normalise(keys), _normalise(values)
-    if tuple(scores.shape) != tuple(keys.shape[:3]) or scores.device != keys.device:
-        raise RuntimeError(f"scores must be [B, Hkv, S] on the cache device, got {tuple(scores.shape)}")
-    scores = scores.to(keys.dtype)
-    if scores.stride(2) != 1:
-        scores = scores.contiguous()
-    p = make_problem(keys, values, n_kept)
-    k_out, v_out, idx, _ = _alloc_out(keys, n_kept, return_indices, False)
-    if n_kept > 0:
-        sstride = (ctypes.c_int64 * 2)(
-            scores.stride(0) if scores.shape[0] > 1 else 0, scores.stride(1) if scores.shape[1] > 1 else 0)
-        with _guard(keys.device):
-            ws = _workspace(p, SCORER_GENERIC, keys.device)
-            _check(
-                load().kvp_scores_compress(
-                    ctypes.byref(p), _ptr(scores), sstride, _ptr(keys), _ptr(values), _ptr(k_out), _ptr(v_out),
-                    _ptr(idx), _ptr(ws), ws.numel(), _stream()),
-                "kvp_scores_compress",
-            )
-    return k_out, v_out, idx
+    scores, sstride = _caller_scores(scores, keys)
+    return _compress("kvp_scores_compress", SCORER_GENERIC, keys, values, n_kept, (scores, sstride, keys, values),
+                     return_indices)
 
 
 def scores_select(scores: torch.Tensor, n_kept: int) -> torch.Tensor:
@@ -550,18 +488,13 @@ def scores_select(scores: torch.Tensor, n_kept: int) -> torch.Tensor:
     (ties to the lowest positions), int32 [B, H, n_kept]. No K/V involved."""
     if not scores.is_cuda or scores.dtype not in _DTYPES or scores.dim() != 3:
         raise RuntimeError(f"scores must be a CUDA bf16/fp16 [B, H, S] tensor, got {scores.dtype} on {scores.device}")
-    if scores.stride(2) != 1:
-        scores = scores.contiguous()
+    scores, sstride = _unit_stride_scores(scores)
     B, H, S = scores.shape
     p = KvpProblem()
     p.B, p.Hkv, p.Hq, p.S, p.D, p.n_kept, p.dtype = B, H, H, S, 8, int(n_kept), _DTYPES[scores.dtype]
     idx = torch.empty((B, H, n_kept), dtype=torch.int32, device=scores.device)
     if n_kept > 0:
-        sstride = (ctypes.c_int64 * 2)(scores.stride(0) if B > 1 else 0, scores.stride(1) if H > 1 else 0)
-        with _guard(scores.device):
-            ws = _workspace(p, SCORER_GENERIC, scores.device)
-            _check(load().kvp_scores_select(ctypes.byref(p), _ptr(scores), sstride, _ptr(idx), _ptr(ws), ws.numel(),
-                                            _stream()), "kvp_scores_select")
+        _enqueue("kvp_scores_select", scores.device, p, scores, sstride, idx, scorer=SCORER_GENERIC)
     return idx
 
 
@@ -570,25 +503,9 @@ def scores_compress_rerotate(scores: torch.Tensor, keys, values, n_kept: int, in
     """KeyRerotationPress: top-k + compaction with the kept keys re-rotated to their new positions."""
     _require_cuda_kv(keys, values)
     keys, values = _normalise(keys), _normalise(values)
-    if tuple(scores.shape) != tuple(keys.shape[:3]) or scores.device != keys.device:
-        raise RuntimeError(f"scores must be [B, Hkv, S] on the cache device, got {tuple(scores.shape)}")
+    scores, sstride = _caller_scores(scores, keys)
     if inv_freq.numel() * 2 != keys.shape[3]:
         raise RuntimeError(f"inv_freq must have head_dim/2 = {keys.shape[3] // 2} entries, got {inv_freq.numel()}")
-    scores = scores.to(keys.dtype)
-    if scores.stride(2) != 1:
-        scores = scores.contiguous()
     inv_freq = inv_freq.to(device=keys.device, dtype=torch.float32).contiguous()
-    p = make_problem(keys, values, n_kept)
-    k_out, v_out, idx, _ = _alloc_out(keys, n_kept, return_indices, False)
-    if n_kept > 0:
-        sstride = (ctypes.c_int64 * 2)(
-            scores.stride(0) if scores.shape[0] > 1 else 0, scores.stride(1) if scores.shape[1] > 1 else 0)
-        with _guard(keys.device):
-            ws = _workspace(p, SCORER_GENERIC, keys.device)
-            _check(
-                load().kvp_scores_compress_rerotate(
-                    ctypes.byref(p), _ptr(scores), sstride, _ptr(keys), _ptr(values), _ptr(inv_freq), _ptr(k_out),
-                    _ptr(v_out), _ptr(idx), _ptr(ws), ws.numel(), _stream()),
-                "kvp_scores_compress_rerotate",
-            )
-    return k_out, v_out, idx
+    return _compress("kvp_scores_compress_rerotate", SCORER_GENERIC, keys, values, n_kept,
+                     (scores, sstride, keys, values, inv_freq), return_indices)

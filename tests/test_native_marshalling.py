@@ -203,3 +203,88 @@ def test_stats_press_marshalling(rec):
     press.use_covariance = False
     press.compress(attn, hidden, keys, values, None, kwargs)
     assert rec.calls[-1][2][3] == 0
+
+
+class _CudaStandIn(torch.Tensor):
+    """A CPU tensor that passes scores_select's CUDA check."""
+
+    @property
+    def is_cuda(self):
+        return True
+
+
+def test_every_wrapper_passes_its_full_argument_list(rec, monkeypatch):
+    """All 13 wrappers: each argument after the kvp_problem, in order, down to the workspace and the stream."""
+    workspaces = []
+    real_workspace = native._workspace
+
+    def spy(p, scorer, device):
+        workspaces.append((scorer, real_workspace(p, scorer, device)))
+        return workspaces[-1][1]
+
+    monkeypatch.setattr(native, "_workspace", spy)
+
+    def last(name, n_kept=0, Hq=2, scorer=None):
+        """The last call's arguments; with `scorer`, its workspace (as the library sizes it) and the stream follow."""
+        got, p, a = rec.calls[-1]
+        assert got == name and (p["n_kept"], p["Hq"]) == (n_kept, Hq)
+        if scorer is None:
+            assert a[-1] == 0
+            return a[:-1]
+        s, ws = workspaces[-1]
+        problem = native.make_problem(k, v, n_kept, Hq)
+        assert s == scorer and a[-3:] == [ws.data_ptr(), native.workspace_bytes(problem, scorer), 0]
+        return a[:-3]
+
+    P = lambda t: t.data_ptr()  # noqa: E731
+    k, v = _kv(B=2, H=2, S=64, D=64)
+
+    sc = native.knorm_score(k)
+    assert last("kvp_knorm_score") == [P(k), P(sc)]
+    k_out, v_out, idx, sc = native.knorm_compress(k, v, 20, return_indices=True, return_scores=True)
+    assert last("kvp_knorm_compress", 20, scorer=native.SCORER_KNORM) == [P(k), P(v), P(k_out), P(v_out), P(idx), P(sc)]
+
+    sc = native.keydiff_score(k)
+    assert last("kvp_keydiff_score", scorer=native.SCORER_KEYDIFF) == [P(k), P(sc)]
+    k_out, v_out, idx, _ = native.keydiff_compress(k, v, 20, return_indices=True)
+    assert last("kvp_keydiff_compress", 20, scorer=native.SCORER_KEYDIFF) == [P(k), P(v), P(k_out), P(v_out), P(idx), 0]
+
+    sc = native.streaming_score(k, 20, 4)
+    assert last("kvp_streaming_score", 20) == [4, P(sc)]
+    k_out, v_out, idx = native.streaming_compress(k, v, 20, 4, return_indices=True)
+    assert last("kvp_streaming_compress", 20) == [4, P(k), P(v), P(k_out), P(v_out), P(idx)]
+
+    q = torch.randn(2, 8, 16, 64).to(torch.bfloat16)
+    sc = native.snapkv_score(k, q, 16, 5)
+    assert last("kvp_snapkv_score", Hq=8, scorer=native.SCORER_SNAPKV) == [P(k), P(q), 16, 5, P(sc)]
+    k_out, v_out, _, sc = native.snapkv_compress(k, v, q, 16, 5, 20, return_scores=True)
+    assert last("kvp_snapkv_compress", 20, Hq=8, scorer=native.SCORER_SNAPKV) == \
+        [P(k), P(v), P(q), 16, 5, P(k_out), P(v_out), 0, P(sc)]
+
+    mu = torch.randn(2, 8, 64).to(torch.bfloat16)
+    cov = torch.randn(2, 8, 64, 64).to(torch.bfloat16)
+    sc = native.expected_attention_score(k, v, mu, cov, 0.5, 4, False)
+    a = last("kvp_expected_attention_score", Hq=8, scorer=native.SCORER_EXPECTED_ATTENTION)
+    assert a == [P(k), P(v), P(mu), P(cov), pytest.approx(0.5), 4, 0, P(sc)] and isinstance(a[4], float)
+    k_out, v_out, idx, sc = native.expected_attention_compress(k, v, mu, None, 0.25, 4, True, 20, return_indices=True,
+                                                               return_scores=True)
+    assert last("kvp_expected_attention_compress", 20, Hq=8, scorer=native.SCORER_EXPECTED_ATTENTION) == \
+        [P(k), P(v), P(mu), 0, 0.25, 4, 1, P(k_out), P(v_out), P(idx), P(sc)]
+
+    scores = torch.rand(2, 2, 64).to(torch.bfloat16)
+    k_out, v_out, idx = native.scores_compress(scores, k, v, 20, return_indices=True)
+    assert last("kvp_scores_compress", 20, scorer=native.SCORER_GENERIC) == \
+        [P(scores), (2 * 64, 64), P(k), P(v), P(k_out), P(v_out), P(idx)]
+    inv_freq = torch.rand(32)
+    k_out, v_out, _ = native.scores_compress_rerotate(scores, k, v, 20, inv_freq)
+    assert last("kvp_scores_compress_rerotate", 20, scorer=native.SCORER_GENERIC) == \
+        [P(scores), (2 * 64, 64), P(k), P(v), P(inv_freq), P(k_out), P(v_out), 0]
+
+    wide = torch.rand(3, 4, 100).to(torch.float16)[:, 1:3, :50].as_subclass(_CudaStandIn)  # strided rows: in place
+    idx = native.scores_select(wide, 10)
+    name, p, a = rec.calls[-1]
+    assert name == "kvp_scores_select" and idx.shape == (3, 2, 10) and idx.dtype == torch.int32
+    assert (p["B"], p["Hkv"], p["Hq"], p["S"], p["D"], p["n_kept"], p["dtype"]) == (3, 2, 2, 50, 8, 10, 1)
+    s, ws = workspaces[-1]
+    assert s == native.SCORER_GENERIC
+    assert a == [P(wide), (4 * 100, 100), P(idx), ws.data_ptr(), ws.numel(), 0]
