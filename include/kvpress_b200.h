@@ -13,6 +13,7 @@
  *     kvp_snapkv_*             <- kvpress/presses/snapkv_press.py:41-105
  *     kvp_expected_attention_* <- kvpress/presses/expected_attention_press.py:126-165
  *     kvp_keydiff_*            <- kvpress/presses/keydiff_press.py:36-46
+ *     kvp_criticalkv_*         <- kvpress/presses/criticalkv_press.py:57-92 (on the wrapped press's scores)
  *     kvp_scores_compress      <- scorer_press.py:93-100 for an arbitrary score tensor
  *                                 (what wrapper presses / user ScorerPress subclasses need)
  *
@@ -69,7 +70,8 @@ typedef enum kvp_scorer {
     KVP_SCORER_STREAMING = 2,
     KVP_SCORER_SNAPKV = 3,
     KVP_SCORER_EXPECTED_ATTENTION = 4,
-    KVP_SCORER_KEYDIFF = 5
+    KVP_SCORER_KEYDIFF = 5,
+    KVP_SCORER_CRITICALKV = 6
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -162,6 +164,24 @@ int kvp_keydiff_score(const kvp_problem* p, const void* K, void* scores_out, voi
 int kvp_keydiff_compress(const kvp_problem* p, const void* K, const void* V, void* K_out, void* V_out,
                          int32_t* idx_out, void* scores_out, void* workspace, size_t workspace_bytes,
                          kvp_stream_t stream);
+
+/* ---- CriticalKVPress (kvpress/presses/criticalkv_press.py:57-92) on the scores of the press it wraps ----------------
+ * base_scores: [B, Hkv, S] in the K dtype with element strides score_stride (b, h; s contiguous), 2-byte aligned.
+ * wo: o_proj.weight, [hidden, Hq*D] rows with row stride wo_stride (a multiple of 8, >= Hq*D), 16-byte aligned.
+ * With G = Hq / Hkv and the query heads h = j G + g of kv head j:
+ *   norm[b,j,s]  = (1/G) sum_g sum_{n < hidden} | sum_d V[b,j,s,d] wo[n, h D + d] |
+ *   score[b,j,s] = (base_scores[b,j,s] + epsilon) * norm[b,j,s]     (fp32, one rounding to the K dtype)
+ * then the n_first positions of every row with the largest base score (ties to the lowest positions) get the dtype's
+ * largest finite value; the host computes n_first = int((1 - ratio) * S * first_stage_ratio). head_dim 64 or 128
+ * (else KVP_ERR_UNSUPPORTED_SHAPE), any G and hidden. n_first is at most S for the score call and at most n_kept for
+ * the compress call, which then keeps the n_kept best final scores (scores_out nullable). K is only gathered. */
+int kvp_criticalkv_score(const kvp_problem* p, const void* V, const void* base_scores, const int64_t* score_stride,
+                         const void* wo, int32_t hidden, int64_t wo_stride, float epsilon, int32_t n_first,
+                         void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+int kvp_criticalkv_compress(const kvp_problem* p, const void* K, const void* V, const void* base_scores,
+                            const int64_t* score_stride, const void* wo, int32_t hidden, int64_t wo_stride,
+                            float epsilon, int32_t n_first, void* K_out, void* V_out, int32_t* idx_out,
+                            void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

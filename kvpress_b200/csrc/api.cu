@@ -10,12 +10,12 @@ namespace kvp {
 
 static thread_local char g_last_cuda_error[256] = "";
 
-// kvp_status of a CUDA call. The KeyDiff, SnapKV and ExpectedAttention score launchers report a shape they have no
-// kernel for as cudaErrorNotSupported.
+// kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention and CriticalKV score launchers report a shape they
+// have no kernel for as cudaErrorNotSupported.
 static int status(cudaError_t e, int scorer = KVP_SCORER_GENERIC) {
     if (e == cudaSuccess) return KVP_OK;
     if (e == cudaErrorNotSupported && (scorer == KVP_SCORER_KEYDIFF || scorer == KVP_SCORER_SNAPKV ||
-                                       scorer == KVP_SCORER_EXPECTED_ATTENTION))
+                                       scorer == KVP_SCORER_EXPECTED_ATTENTION || scorer == KVP_SCORER_CRITICALKV))
         return KVP_ERR_UNSUPPORTED_SHAPE;
     snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
     // launch-configuration errors are not sticky: clear them, or the cudaPeekAtLastError() of every later call
@@ -73,6 +73,7 @@ static size_t layout(const Dims& d, int scorer, int window, void* base, Workspac
     ws->scorer_bytes = scorer == KVP_SCORER_SNAPKV               ? snapkv_scratch_bytes(d, window)
                        : scorer == KVP_SCORER_EXPECTED_ATTENTION ? ea_scratch_bytes(d)
                        : scorer == KVP_SCORER_KEYDIFF            ? keydiff_scratch_bytes(d)
+                       : scorer == KVP_SCORER_CRITICALKV         ? criticalkv_scratch_bytes(d)
                                                                  : 0;
     ws->scorer = c.take<char>(ws->scorer_bytes);
     return c.bytes;
@@ -235,6 +236,9 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         // press defaults (use_covariance + use_vnorm): memset, logits (which also writes the value norms), finalize,
         // select+compact
         case KVP_SCORER_EXPECTED_ATTENTION: *launches_out = 4; break;
+        // press defaults (first_stage_ratio > 0): memset, keys of the base scores, select n_first, score, force
+        // n_first, memset, keys of the final scores, select+compact
+        case KVP_SCORER_CRITICALKV: *launches_out = 8; break;
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -385,6 +389,57 @@ int kvp_expected_attention_compress(const kvp_problem* p, const void* K, const v
     };
     return run(Kind::compress, p, KVP_SCORER_EXPECTED_ATTENTION, 0, {K, V, K_out, V_out, idx_out, nullptr}, operands,
                ea_stage(p, K, V, mu, cov, epsilon, n_sink, use_vnorm, scores_out), workspace, workspace_bytes, stream);
+}
+
+// ---- CriticalKV ----------------------------------------------------------------------------------
+// The operand checks both entry points share, after their null / alignment checks; n_first_max is S for a score call,
+// n_kept for a compress call.
+static int criticalkv_args(const Dims& d, int32_t hidden, int64_t wo_stride, int32_t n_first, int32_t n_first_max) {
+    if (hidden <= 0) return KVP_ERR_BAD_ARGUMENT;
+    if (wo_stride % 8 != 0 || wo_stride < (int64_t)d.Hq * d.D) return KVP_ERR_BAD_STRIDE;
+    return (n_first < 0 || n_first > n_first_max) ? KVP_ERR_BAD_ARGUMENT : KVP_OK;
+}
+
+static bool aligned2(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 1) == 0; }
+
+int kvp_criticalkv_score(const kvp_problem* p, const void* V, const void* base_scores, const int64_t* score_stride,
+                         const void* wo, int32_t hidden, int64_t wo_stride, float epsilon, int32_t n_first,
+                         void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!V || !base_scores || !score_stride || !wo || !scores_out) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(V) || !aligned2(base_scores) || !aligned16(wo)) return KVP_ERR_BAD_STRIDE;
+        return criticalkv_args(d, hidden, wo_stride, n_first, d.S);
+    };
+    auto score = [&](const Call& c) {
+        return launch_criticalkv_score(c.d, p->dtype, V, base_scores, score_stride[0], score_stride[1], wo, hidden,
+                                       wo_stride, epsilon, n_first, c.ws, scores_out, c.st);
+    };
+    // the workspace is only read by the stage-1 selection
+    return run(Kind::score, p, KVP_SCORER_CRITICALKV, 0, {}, operands, score, workspace, workspace_bytes, stream,
+               n_first > 0);
+}
+
+int kvp_criticalkv_compress(const kvp_problem* p, const void* K, const void* V, const void* base_scores,
+                            const int64_t* score_stride, const void* wo, int32_t hidden, int64_t wo_stride,
+                            float epsilon, int32_t n_first, void* K_out, void* V_out, int32_t* idx_out,
+                            void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!base_scores || !score_stride || !wo) return KVP_ERR_NULL_POINTER;
+        if (!aligned2(base_scores) || !aligned16(wo)) return KVP_ERR_BAD_STRIDE;
+        return criticalkv_args(d, hidden, wo_stride, n_first, d.n_kept);
+    };
+    // the score stage, then the keys of the final scores for the selection: the stage-1 selection used the workspace
+    auto score = [&](const Call& c) {
+        void* out = scores_out ? scores_out : criticalkv_scratch_scores(c.d, c.ws);
+        cudaError_t e = launch_criticalkv_score(c.d, p->dtype, V, base_scores, score_stride[0], score_stride[1], wo,
+                                                hidden, wo_stride, epsilon, n_first, c.ws, out, c.st);
+        if (e == cudaSuccess && n_first > 0) e = cudaMemsetAsync(c.ws.hist_hi, 0, c.zeroed, c.st);
+        if (e == cudaSuccess)
+            e = launch_keys_from_scores(c.d, p->dtype, out, (int64_t)c.d.H * c.d.S, c.d.S, c.ws, c.st);
+        return e;
+    };
+    return run(Kind::compress, p, KVP_SCORER_CRITICALKV, 0, {K, V, K_out, V_out, idx_out, nullptr}, operands, score,
+               workspace, workspace_bytes, stream);
 }
 
 // ---- generic scores ------------------------------------------------------------------------------

@@ -43,7 +43,7 @@ struct Workspace {
     uint2* tile_prefix;  // [R][n_tiles] {kept (> T) + 1, tied (== T) + 1} positions in the tiles before;
                          // zero = row not scanned yet
     int R;
-    void* scorer;        // scorer-specific scratch (SnapKV / ExpectedAttention)
+    void* scorer;        // scorer-specific scratch (SnapKV / ExpectedAttention / KeyDiff / CriticalKV)
     size_t scorer_bytes;
     int S_pad;
     int n_tiles;
@@ -343,5 +343,10 @@ cudaError_t launch_fill_sentinel(int dtype, void* scores_out, int R, int S, int 
 cudaError_t launch_ea_score(const Dims& d, int dtype, const void* K, const void* V, const void* mu,
                             const void* cov, float eps, int n_sink, int use_vnorm,
                             const Workspace& ws, void* scores_out, cudaStream_t st);
+size_t criticalkv_scratch_bytes(const Dims& d);
+void* criticalkv_scratch_scores(const Dims& d, const Workspace& ws);
+cudaError_t launch_criticalkv_score(const Dims& d, int dtype, const void* V, const void* base, int64_t sb,
+                                    int64_t sh, const void* wo, int hidden, int64_t wo_stride, float eps, int n_first,
+                                    const Workspace& ws, void* scores_out, cudaStream_t st);
 
 }  // namespace kvp

@@ -18,7 +18,8 @@ import torch
 _LIB_NAME = "libkvpress_b200.so"
 _LIB_PATH = Path(__file__).resolve().parent / _LIB_NAME
 
-SCORER_GENERIC, SCORER_KNORM, SCORER_STREAMING, SCORER_SNAPKV, SCORER_EXPECTED_ATTENTION, SCORER_KEYDIFF = range(6)
+(SCORER_GENERIC, SCORER_KNORM, SCORER_STREAMING, SCORER_SNAPKV, SCORER_EXPECTED_ATTENTION, SCORER_KEYDIFF,
+ SCORER_CRITICALKV) = range(7)
 _DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
 
@@ -48,6 +49,8 @@ _P = ctypes.c_void_p
 _PP = ctypes.POINTER(KvpProblem)
 _SZ = ctypes.c_size_t
 _I = ctypes.c_int32
+_I64 = ctypes.c_int64
+_PI64 = ctypes.POINTER(ctypes.c_int64)
 SIGNATURES = {
     "kvp_abi_version": (ctypes.c_int, []),
     "kvp_status_string": (ctypes.c_char_p, [ctypes.c_int]),
@@ -72,6 +75,9 @@ SIGNATURES = {
     "kvp_scores_select": (ctypes.c_int, [_PP, _P, ctypes.POINTER(ctypes.c_int64), _P, _P, _SZ, _P]),
     "kvp_scores_compress_rerotate": (
         ctypes.c_int, [_PP, _P, ctypes.POINTER(ctypes.c_int64), _P, _P, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_criticalkv_score": (ctypes.c_int, [_PP, _P, _P, _PI64, _P, _I, _I64, ctypes.c_float, _I, _P, _P, _SZ, _P]),
+    "kvp_criticalkv_compress": (
+        ctypes.c_int, [_PP, _P, _P, _P, _PI64, _P, _I, _I64, ctypes.c_float, _I, _P, _P, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -509,3 +515,43 @@ def scores_compress_rerotate(scores: torch.Tensor, keys, values, n_kept: int, in
     inv_freq = inv_freq.to(device=keys.device, dtype=torch.float32).contiguous()
     return _compress("kvp_scores_compress_rerotate", SCORER_GENERIC, keys, values, n_kept,
                      (scores, sstride, keys, values, inv_freq), return_indices)
+
+
+# --------------------------------------------------------------------------------------------------
+# CriticalKV (on the scores of the press it wraps)
+# --------------------------------------------------------------------------------------------------
+def _check_wo(wo: torch.Tensor, values: torch.Tensor):
+    """o_proj.weight [hidden, Hq*D] in the cache dtype with unit-stride rows: (wo, Hq, row stride). Sliced rows are
+    consumed in place; a layout the kernel cannot address is copied."""
+    D = values.shape[3]
+    if wo.dim() != 2 or wo.shape[1] % D or wo.device != values.device:
+        raise RuntimeError(f"wo must be o_proj.weight [hidden, Hq*{D}] on the cache device, got {tuple(wo.shape)}")
+    wo = wo.to(values.dtype)
+    if wo.stride(1) != 1 or wo.data_ptr() % 16 or (wo.shape[0] > 1 and wo.stride(0) % 8):
+        wo = wo.contiguous()
+    return wo, wo.shape[1] // D, int(wo.stride(0) if wo.shape[0] > 1 else wo.shape[1])
+
+
+def criticalkv_score(base_scores: torch.Tensor, values: torch.Tensor, wo: torch.Tensor, epsilon: float,
+                     n_first: int) -> torch.Tensor:
+    """CriticalKV scores [B, Hkv, S] from the wrapped press's scores: (base + epsilon) * the mean over the group of
+    ||v_s Wo_h^T||_1, then finfo.max on the n_first best base scores of every row."""
+    _require_cuda_kv(values, values)
+    values = _normalise(values)
+    wo, Hq, wo_stride = _check_wo(wo, values)
+    base, sstride = _caller_scores(base_scores, values)
+    p = make_problem(values, values, 0, Hq)
+    return _score("kvp_criticalkv_score", SCORER_CRITICALKV, values, p, values, base, sstride, wo, wo.shape[0],
+                  wo_stride, float(epsilon), int(n_first))
+
+
+def criticalkv_compress(base_scores: torch.Tensor, keys, values, wo: torch.Tensor, epsilon: float, n_first: int,
+                        n_kept: int, return_indices: bool = False, return_scores: bool = False):
+    """criticalkv_score, then top-n_kept + compaction on the final scores."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    wo, Hq, wo_stride = _check_wo(wo, values)
+    base, sstride = _caller_scores(base_scores, keys)
+    return _compress("kvp_criticalkv_compress", SCORER_CRITICALKV, keys, values, n_kept,
+                     (keys, values, base, sstride, wo, wo.shape[0], wo_stride, float(epsilon), int(n_first)),
+                     return_indices, return_scores, Hq)

@@ -1,4 +1,4 @@
-"""Scores for cache shapes the two tensor-core scorers do not instantiate (GPU, torch / cuBLAS GEMMs).
+"""Scores for cache shapes the tensor-core scorers do not instantiate (GPU, torch / cuBLAS GEMMs).
 
 The tensor-core (wgmma) SnapKV and ExpectedAttention kernels keep their query block / covariance resident in shared memory
 and exist for head_dim 64 and 128, at most 8 query heads per kv head and (for SnapKV) at most 512 window-query rows
@@ -9,7 +9,8 @@ result goes through the sm_90a selection + compaction kernels like any caller-su
 (`native.scores_compress`). Nothing here runs on the CPU; CPU tensors are refused like everywhere else.
 
 Formulas: SnapKV `kvpress/presses/snapkv_press.py:41-105`, ExpectedAttention
-`kvpress/presses/expected_attention_press.py:136-165`.
+`kvpress/presses/expected_attention_press.py:136-165`, CriticalKV `kvpress/presses/criticalkv_press.py:57-92` (head_dim
+other than 64 / 128).
 """
 from __future__ import annotations
 
@@ -36,6 +37,11 @@ def expected_attention_on_tensor_cores(head_dim: int, group: int, has_cov: bool)
     """Shapes `kvp_expected_attention_*` instantiates (csrc/expected_attention.cu launch_ea_t): the covariance-free
     scan takes any head_dim, the covariance path head_dim 64 / 128; both at most 8 query heads per kv head."""
     return group <= MAX_GROUP and (not has_cov or head_dim in TENSOR_CORE_HEAD_DIMS)
+
+
+def criticalkv_on_tensor_cores(head_dim: int) -> bool:
+    """Shapes `kvp_criticalkv_*` instantiates (csrc/criticalkv.cu): head_dim 64 / 128, any group size and hidden size."""
+    return head_dim in TENSOR_CORE_HEAD_DIMS
 
 
 def _note(what: str, keys: torch.Tensor, group: int) -> None:
@@ -115,3 +121,31 @@ def expected_attention_scores(keys: torch.Tensor, values: torch.Tensor, mu: torc
             vn[..., s0:s1] = values[:, :, n_sink + s0:n_sink + s1].float().norm(dim=-1)
         score = (score + epsilon) * vn
     return _pad_forced(score.to(keys.dtype), n_sink, 0)
+
+
+def criticalkv_scores(base_scores: torch.Tensor, values: torch.Tensor, wo: torch.Tensor, epsilon: float, n_first: int,
+                      chunk: int = 4096) -> torch.Tensor:
+    """CriticalKV scores [B,Hkv,S] in the cache dtype from the wrapped press's scores, values [B,Hkv,S,D] and
+    o_proj.weight [hidden, Hq*D]: one query head and one slab of positions at a time in fp32, rounded once; the
+    n_first best base scores of every row get finfo.max through the sm_90a selection."""
+    from kvpress_b200 import native
+
+    _require_cuda(values)
+    B, Hkv, S, D = values.shape
+    Hq = wo.shape[1] // D
+    G = Hq // Hkv
+    _note("CriticalKV", values, G)
+    base = base_scores.to(values.dtype)
+    w = wo.to(values.dtype).float()
+    norm = torch.zeros((B, Hkv, S), dtype=torch.float32, device=values.device)
+    for h in range(Hq):
+        w_h = w[:, h * D:(h + 1) * D]                                   # [hidden, D]
+        for s0 in range(0, S, chunk):
+            s1 = min(S, s0 + chunk)
+            v = values[:, h // G, s0:s1].float()                        # [B, c, D]
+            norm[:, h // G, s0:s1] += torch.matmul(v, w_h.T).abs().sum(dim=-1)
+    scores = ((base.float() + epsilon) * (norm / G)).to(values.dtype)
+    if n_first > 0:
+        first = native.scores_select(base, n_first).long()
+        scores.scatter_(-1, first, torch.finfo(scores.dtype).max)
+    return scores
