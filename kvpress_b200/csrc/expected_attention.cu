@@ -122,9 +122,9 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                  int n_split) {
     using L = EaSmem<D, GR>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    // dynamic shared memory is only guaranteed 16-B aligned: round up to 1024 B for the swizzle
-    unsigned char* smem = reinterpret_cast<unsigned char*>(
-        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    // dynamic shared memory is only guaranteed 16-B aligned: round up to 1024 B for the swizzle. The pointer is
+    // offset from smem_raw (not rebuilt from an integer) so that the compiler still sees shared memory and emits LDS.
+    unsigned char* smem = smem_raw + ((1024u - (umma::smem_u32(smem_raw) & 1023u)) & 1023u);
     unsigned char* s_cov = smem + L::kCovOff;
     unsigned char* s_stage = smem + L::kStageOff;
     float* s_bias = reinterpret_cast<float*>(smem + L::kBiasOff);
@@ -221,10 +221,33 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                 // the k rows are in registers: hand the stage back to the producer before the MMAs
                 __syncwarp();
                 if (lane == 0) umma::mbar_arrive(&k_empty[stage]);
-                float lg[GR][2];
+                // Head g's logits are finished (quad sum, scale, store, online max / sum-exp) while the tensor cores
+                // work on head g + 1: the MMAs are issued first, then the previous head's finish runs before the wait.
+                // Only the last head's finish is exposed. Both rows' shuffles come before the store branch, since a
+                // shuffle cannot be scheduled across a divergent branch.
+                auto finish = [&](const int g, const float l0, const float l1) {
+                    float l[2] = {l0, l1};
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) l[hh] += __shfl_xor_sync(0xFFFFFFFFu, l[hh], 1);
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        l[hh] += __shfl_xor_sync(0xFFFFFFFFu, l[hh], 2);
+                        l[hh] *= inv_2d;
+                    }
+#pragma unroll
+                    for (int hh = 0; hh < 2; ++hh) {
+                        const int s = t * kEaTile + r0 + 8 * hh;
+                        if (qd == 0 && s >= n_sink && s < S) {
+                            sc.logits[((size_t)row * g_total + g_off + g) * S_pad + s] = l[hh];
+                            const float m_new = fmaxf(run_m[g], l[hh]);
+                            run_z[g] = run_z[g] * __expf(run_m[g] - m_new) + __expf(l[hh] - m_new);
+                            run_m[g] = m_new;
+                        }
+                    }
+                };
+                float p0 = 0.f, p1 = 0.f;  // head g - 1's partial dot products of rows r0, r0 + 8
 #pragma unroll
                 for (int g = 0; g < GR; ++g) {
-                    lg[g][0] = lg[g][1] = 0.f;
                     if (g >= n_real) continue;  // warpgroup-uniform
                     float acc[D / 2];
                     umma::wgmma_fence();
@@ -237,6 +260,7 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                             kk > 0);
                     }
                     umma::wgmma_commit();
+                    if (g > 0) finish(g - 1, p0, p1);
                     umma::wgmma_wait_all();
                     float l0 = 0.f, l1 = 0.f;
 #pragma unroll
@@ -250,25 +274,9 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                         l1 = fmaf(k1.x, acc[4 * j + 2] + bb.x, l1);
                         l1 = fmaf(k1.y, acc[4 * j + 3] + bb.y, l1);
                     }
-                    lg[g][0] = l0;
-                    lg[g][1] = l1;
-                }
-#pragma unroll
-                for (int g = 0; g < GR; ++g) {
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        float l = lg[g][hh];
-                        l += __shfl_xor_sync(0xFFFFFFFFu, l, 1);
-                        l += __shfl_xor_sync(0xFFFFFFFFu, l, 2);
-                        l *= inv_2d;
-                        const int s = t * kEaTile + r0 + 8 * hh;
-                        if (g < n_real && qd == 0 && s >= n_sink && s < S) {
-                            sc.logits[((size_t)row * g_total + g_off + g) * S_pad + s] = l;
-                            const float m_new = fmaxf(run_m[g], l);
-                            run_z[g] = run_z[g] * __expf(run_m[g] - m_new) + __expf(l - m_new);
-                            run_m[g] = m_new;
-                        }
-                    }
+                    p0 = l0;
+                    p1 = l1;
+                    if (g + 1 == n_real) finish(g, l0, l1);
                 }
             }
             // ---- warp-level (max, sum-exp) per head -> shared ---------------------------------------------------
