@@ -14,6 +14,7 @@
  *     kvp_expected_attention_* <- kvpress/presses/expected_attention_press.py:126-165
  *     kvp_keydiff_*            <- kvpress/presses/keydiff_press.py:36-46
  *     kvp_criticalkv_*         <- kvpress/presses/criticalkv_press.py:57-92 (on the wrapped press's scores)
+ *     kvp_observed_attention_* <- kvpress/presses/observed_attention_press.py (H2O; from Q and K, no eager weights)
  *     kvp_scores_compress      <- scorer_press.py:93-100 for an arbitrary score tensor
  *                                 (what wrapper presses / user ScorerPress subclasses need)
  *
@@ -71,7 +72,8 @@ typedef enum kvp_scorer {
     KVP_SCORER_SNAPKV = 3,
     KVP_SCORER_EXPECTED_ATTENTION = 4,
     KVP_SCORER_KEYDIFF = 5,
-    KVP_SCORER_CRITICALKV = 6
+    KVP_SCORER_CRITICALKV = 6,
+    KVP_SCORER_OBSERVED_ATTENTION = 7
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -182,6 +184,27 @@ int kvp_criticalkv_compress(const kvp_problem* p, const void* K, const void* V, 
                             const int64_t* score_stride, const void* wo, int32_t hidden, int64_t wo_stride,
                             float epsilon, int32_t n_first, void* K_out, void* V_out, int32_t* idx_out,
                             void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+
+/* ---- ObservedAttentionPress (kvpress/presses/observed_attention_press.py, the H2O score) -------------------------------
+ * q: the RoPE'd queries of the current forward, contiguous [B, Hq, n_q, D], 16-byte aligned; row i is at position
+ * p_i = S - n_q + i (1 <= n_q <= S: n_q = S in prefill, the current step's rows under DecodingPress). With G = Hq / Hkv
+ * and the query heads h = j G + g of kv head j:
+ *   y[b,h,i,s]   = scaling * q[b,h,i] . K[b,j,s] for s <= p_i, else -inf     (scaling: the attention's module.scaling)
+ *   P[b,h,i,s]   = softmax over s of y                                      (exact normaliser over the whole row)
+ *   score[b,j,s] = (1/G) sum_g sum_i P[b,h,i,s] / c(S - s)                  (fp32, one rounding to the K dtype)
+ * where c(n) is n rounded to the K dtype, as the reference divides by torch.arange(S, 0, -1) in the attention dtype:
+ * counts above 256 round in bf16, and in fp16 counts of 65520 and above are inf, so those first positions score
+ * exactly 0. No position is forced. head_dim 64 or 128 and 1 <= G <= 8, else KVP_ERR_UNSUPPORTED_SHAPE.
+ * Check order (the first failure is returned): validate the problem -> n_kept == 0 returns KVP_OK (compress) ->
+ * K / V / K_out / V_out null and alignment (compress) -> q null / alignment (and K, scores_out for the score call) ->
+ * 1 <= n_q <= S, else KVP_ERR_BAD_ARGUMENT -> scaling finite and > 0, else KVP_ERR_BAD_ARGUMENT -> workspace.
+ * kvp_workspace_bytes sizes the workspace for n_q = S. The compress call keeps the n_kept best scores (scores_out
+ * nullable). Memory beyond the workspace: none; the [B, Hq, n_q, S] weights are never formed. */
+int kvp_observed_attention_score(const kvp_problem* p, const void* K, const void* q, int32_t n_q, float scaling,
+                                 void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+int kvp_observed_attention_compress(const kvp_problem* p, const void* K, const void* V, const void* q, int32_t n_q,
+                                    float scaling, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
+                                    void* workspace, size_t workspace_bytes, kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

@@ -1,6 +1,7 @@
 // api.cu — the extern "C" surface declared in include/kvpress_b200.h.
 // Validates the problem, carves the caller's workspace and enqueues the kernels on the caller's
 // stream. Never allocates, never synchronises (except kvp_workspace_check), never throws.
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -10,12 +11,13 @@ namespace kvp {
 
 static thread_local char g_last_cuda_error[256] = "";
 
-// kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention and CriticalKV score launchers report a shape they
-// have no kernel for as cudaErrorNotSupported.
+// kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention, CriticalKV and ObservedAttention score launchers
+// report a shape they have no kernel for as cudaErrorNotSupported.
 static int status(cudaError_t e, int scorer = KVP_SCORER_GENERIC) {
     if (e == cudaSuccess) return KVP_OK;
-    if (e == cudaErrorNotSupported && (scorer == KVP_SCORER_KEYDIFF || scorer == KVP_SCORER_SNAPKV ||
-                                       scorer == KVP_SCORER_EXPECTED_ATTENTION || scorer == KVP_SCORER_CRITICALKV))
+    if (e == cudaErrorNotSupported &&
+        (scorer == KVP_SCORER_KEYDIFF || scorer == KVP_SCORER_SNAPKV || scorer == KVP_SCORER_EXPECTED_ATTENTION ||
+         scorer == KVP_SCORER_CRITICALKV || scorer == KVP_SCORER_OBSERVED_ATTENTION))
         return KVP_ERR_UNSUPPORTED_SHAPE;
     snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
     // launch-configuration errors are not sticky: clear them, or the cudaPeekAtLastError() of every later call
@@ -54,7 +56,12 @@ static int validate(const kvp_problem* p, Dims* d, bool need_kv_strides = true) 
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-// The workspace of a call: sized when `base` is null, carved otherwise. Returns the total bytes and, in *zeroed, the
+// The window kvp_workspace_bytes / kvp_workspace_check size a scorer's scratch for: the largest a call may pass (SnapKV's
+// supported windows, ObservedAttention's n_q = S).
+static int largest_window(const Dims& d, int scorer) { return scorer == KVP_SCORER_OBSERVED_ATTENTION ? d.S : 256; }
+
+// The workspace of a call: sized when `base` is null, carved otherwise. `window` is SnapKV's window, or the query rows
+// n_q of ObservedAttention. Returns the total bytes and, in *zeroed, the
 // leading bytes every call clears with one memset: the histograms, the counters and the tile prefixes. The
 // histograms are whole KiB per row, so hist_lo and the counters follow hist_hi without padding.
 static size_t layout(const Dims& d, int scorer, int window, void* base, Workspace* ws, size_t* zeroed) {
@@ -74,6 +81,7 @@ static size_t layout(const Dims& d, int scorer, int window, void* base, Workspac
                        : scorer == KVP_SCORER_EXPECTED_ATTENTION ? ea_scratch_bytes(d)
                        : scorer == KVP_SCORER_KEYDIFF            ? keydiff_scratch_bytes(d)
                        : scorer == KVP_SCORER_CRITICALKV         ? criticalkv_scratch_bytes(d)
+                       : scorer == KVP_SCORER_OBSERVED_ATTENTION ? observed_attention_scratch_bytes(d, window)
                                                                  : 0;
     ws->scorer = c.take<char>(ws->scorer_bytes);
     return c.bytes;
@@ -199,10 +207,10 @@ int kvp_workspace_bytes(const kvp_problem* p, int scorer, size_t* bytes_out) {
     int rc = validate(p, &d, false);
     if (rc) return rc;
     if (!bytes_out) return KVP_ERR_NULL_POINTER;
-    // window only changes the SnapKV scratch; size for the largest supported window
+    // window only changes the SnapKV and ObservedAttention scratch; size for the largest supported window
     Workspace ws;
     size_t zeroed;
-    *bytes_out = layout(d, scorer, 256, nullptr, &ws, &zeroed);
+    *bytes_out = layout(d, scorer, largest_window(d, scorer), nullptr, &ws, &zeroed);
     return KVP_OK;
 }
 
@@ -210,7 +218,8 @@ int kvp_workspace_check(const kvp_problem* p, int scorer, const void* workspace,
                         kvp_stream_t stream) {
     Call c;
     int rc = validate(p, &c.d, false);
-    if (rc || (rc = c.carve(scorer, 256, const_cast<void*>(workspace), workspace_bytes))) return rc;
+    if (rc || (rc = c.carve(scorer, largest_window(c.d, scorer), const_cast<void*>(workspace), workspace_bytes)))
+        return rc;
     uint32_t flag = 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     cudaError_t e = cudaMemcpyAsync(&flag, c.ws.counters + kCounterErrSlot(c.d.R), sizeof(flag),
@@ -239,6 +248,7 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         // press defaults (first_stage_ratio > 0): memset, keys of the base scores, select n_first, score, force
         // n_first, memset, keys of the final scores, select+compact
         case KVP_SCORER_CRITICALKV: *launches_out = 8; break;
+        case KVP_SCORER_OBSERVED_ATTENTION: *launches_out = 5; break;  // memset, stats, colsum, finalize, select+compact
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -440,6 +450,43 @@ int kvp_criticalkv_compress(const kvp_problem* p, const void* K, const void* V, 
     };
     return run(Kind::compress, p, KVP_SCORER_CRITICALKV, 0, {K, V, K_out, V_out, idx_out, nullptr}, operands, score,
                workspace, workspace_bytes, stream);
+}
+
+// ---- ObservedAttention ---------------------------------------------------------------------------
+// The operand checks both entry points share, after their null / alignment checks.
+static int observed_attention_args(const Dims& d, int32_t n_q, float scaling) {
+    if (n_q < 1 || n_q > d.S) return KVP_ERR_BAD_ARGUMENT;
+    return (isfinite(scaling) && scaling > 0.f) ? KVP_OK : KVP_ERR_BAD_ARGUMENT;
+}
+
+static auto observed_attention_stage(const kvp_problem* p, const void* K, const void* q, int32_t n_q, float scaling,
+                                     void* scores_out) {
+    return [=](const Call& c) {
+        return launch_observed_attention_score(c.d, p->dtype, K, q, n_q, scaling, c.ws, scores_out, c.st);
+    };
+}
+
+int kvp_observed_attention_score(const kvp_problem* p, const void* K, const void* q, int32_t n_q, float scaling,
+                                 void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!K || !q || !scores_out) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(K) || !aligned16(q)) return KVP_ERR_BAD_STRIDE;
+        return observed_attention_args(d, n_q, scaling);
+    };
+    return run(Kind::score, p, KVP_SCORER_OBSERVED_ATTENTION, n_q, {}, operands,
+               observed_attention_stage(p, K, q, n_q, scaling, scores_out), workspace, workspace_bytes, stream);
+}
+
+int kvp_observed_attention_compress(const kvp_problem* p, const void* K, const void* V, const void* q, int32_t n_q,
+                                    float scaling, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
+                                    void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!q) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(q)) return KVP_ERR_BAD_STRIDE;
+        return observed_attention_args(d, n_q, scaling);
+    };
+    return run(Kind::compress, p, KVP_SCORER_OBSERVED_ATTENTION, n_q, {K, V, K_out, V_out, idx_out, nullptr}, operands,
+               observed_attention_stage(p, K, q, n_q, scaling, scores_out), workspace, workspace_bytes, stream);
 }
 
 // ---- generic scores ------------------------------------------------------------------------------

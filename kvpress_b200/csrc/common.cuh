@@ -43,7 +43,8 @@ struct Workspace {
     uint2* tile_prefix;  // [R][n_tiles] {kept (> T) + 1, tied (== T) + 1} positions in the tiles before;
                          // zero = row not scanned yet
     int R;
-    void* scorer;        // scorer-specific scratch (SnapKV / ExpectedAttention / KeyDiff / CriticalKV)
+    void* scorer;        // scorer-specific scratch (SnapKV / ExpectedAttention / KeyDiff / CriticalKV /
+                         // ObservedAttention)
     size_t scorer_bytes;
     int S_pad;
     int n_tiles;
@@ -348,5 +349,8 @@ void* criticalkv_scratch_scores(const Dims& d, const Workspace& ws);
 cudaError_t launch_criticalkv_score(const Dims& d, int dtype, const void* V, const void* base, int64_t sb,
                                     int64_t sh, const void* wo, int hidden, int64_t wo_stride, float eps, int n_first,
                                     const Workspace& ws, void* scores_out, cudaStream_t st);
+size_t observed_attention_scratch_bytes(const Dims& d, int n_q);
+cudaError_t launch_observed_attention_score(const Dims& d, int dtype, const void* K, const void* q, int n_q,
+                                            float scaling, const Workspace& ws, void* scores_out, cudaStream_t st);
 
 }  // namespace kvp

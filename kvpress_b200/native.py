@@ -19,7 +19,7 @@ _LIB_NAME = "libkvpress_b200.so"
 _LIB_PATH = Path(__file__).resolve().parent / _LIB_NAME
 
 (SCORER_GENERIC, SCORER_KNORM, SCORER_STREAMING, SCORER_SNAPKV, SCORER_EXPECTED_ATTENTION, SCORER_KEYDIFF,
- SCORER_CRITICALKV) = range(7)
+ SCORER_CRITICALKV, SCORER_OBSERVED_ATTENTION) = range(8)
 _DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
 
@@ -78,6 +78,9 @@ SIGNATURES = {
     "kvp_criticalkv_score": (ctypes.c_int, [_PP, _P, _P, _PI64, _P, _I, _I64, ctypes.c_float, _I, _P, _P, _SZ, _P]),
     "kvp_criticalkv_compress": (
         ctypes.c_int, [_PP, _P, _P, _P, _PI64, _P, _I, _I64, ctypes.c_float, _I, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_observed_attention_score": (ctypes.c_int, [_PP, _P, _P, _I, ctypes.c_float, _P, _P, _SZ, _P]),
+    "kvp_observed_attention_compress": (
+        ctypes.c_int, [_PP, _P, _P, _P, _I, ctypes.c_float, _P, _P, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -555,3 +558,37 @@ def criticalkv_compress(base_scores: torch.Tensor, keys, values, wo: torch.Tenso
     return _compress("kvp_criticalkv_compress", SCORER_CRITICALKV, keys, values, n_kept,
                      (keys, values, base, sstride, wo, wo.shape[0], wo_stride, float(epsilon), int(n_first)),
                      return_indices, return_scores, Hq)
+
+
+# --------------------------------------------------------------------------------------------------
+# ObservedAttention (H2O)
+# --------------------------------------------------------------------------------------------------
+def _check_queries(q: torch.Tensor, keys: torch.Tensor) -> torch.Tensor:
+    """RoPE'd queries [B, Hq, n_q, D] with 1 <= n_q <= S, in the cache dtype and on its device, made contiguous."""
+    B, _, S, D = keys.shape
+    if q.dim() != 4 or q.shape[0] != B or q.shape[3] != D or not 1 <= q.shape[2] <= S:
+        raise RuntimeError(f"q must be [B, Hq, n_q, {D}] with 1 <= n_q <= {S}, got {tuple(q.shape)}")
+    if q.dtype != keys.dtype or q.device != keys.device:
+        raise RuntimeError("q must share dtype and device with the keys")
+    return q.contiguous()
+
+
+def observed_attention_score(keys, q, scaling: float) -> torch.Tensor:
+    """H2O scores [B, Hkv, S]: the causal softmax(scaling q.k) of the n_q queries q [B, Hq, n_q, D] (the last n_q
+    positions), summed over the queries, divided by S - s in the cache dtype, averaged over the group."""
+    _require_cuda_kv(keys, keys)
+    keys = _normalise(keys)
+    q = _check_queries(q, keys)
+    p = make_problem(keys, keys, 0, q.shape[1])
+    return _score("kvp_observed_attention_score", SCORER_OBSERVED_ATTENTION, keys, p, keys, q, q.shape[2],
+                  float(scaling))
+
+
+def observed_attention_compress(keys, values, q, scaling: float, n_kept: int, return_indices: bool = False,
+                                return_scores: bool = False):
+    """observed_attention_score, then top-n_kept + compaction."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    q = _check_queries(q, keys)
+    return _compress("kvp_observed_attention_compress", SCORER_OBSERVED_ATTENTION, keys, values, n_kept,
+                     (keys, values, q, q.shape[2], float(scaling)), return_indices, return_scores, q.shape[1])

@@ -10,7 +10,8 @@ result goes through the sm_90a selection + compaction kernels like any caller-su
 
 Formulas: SnapKV `kvpress/presses/snapkv_press.py:41-105`, ExpectedAttention
 `kvpress/presses/expected_attention_press.py:136-165`, CriticalKV `kvpress/presses/criticalkv_press.py:57-92` (head_dim
-other than 64 / 128).
+other than 64 / 128), ObservedAttention `kvpress/presses/observed_attention_press.py` (head_dim other than 64 / 128, more
+than 8 query heads per kv head).
 """
 from __future__ import annotations
 
@@ -42,6 +43,12 @@ def expected_attention_on_tensor_cores(head_dim: int, group: int, has_cov: bool)
 def criticalkv_on_tensor_cores(head_dim: int) -> bool:
     """Shapes `kvp_criticalkv_*` instantiates (csrc/criticalkv.cu): head_dim 64 / 128, any group size and hidden size."""
     return head_dim in TENSOR_CORE_HEAD_DIMS
+
+
+def observed_attention_on_tensor_cores(head_dim: int, group: int) -> bool:
+    """Shapes `kvp_observed_attention_*` instantiates (csrc/observed_attention.cu launch_obs_d): head_dim 64 / 128, at
+    most 8 query heads per kv head."""
+    return head_dim in TENSOR_CORE_HEAD_DIMS and 1 <= group <= MAX_GROUP
 
 
 def _note(what: str, keys: torch.Tensor, group: int) -> None:
@@ -149,3 +156,36 @@ def criticalkv_scores(base_scores: torch.Tensor, values: torch.Tensor, wo: torch
         first = native.scores_select(base, n_first).long()
         scores.scatter_(-1, first, torch.finfo(scores.dtype).max)
     return scores
+
+
+def observed_attention_scores(keys: torch.Tensor, q: torch.Tensor, scaling: float,
+                              max_logits: int = 1 << 27) -> torch.Tensor:
+    """keys [B,Hkv,S,D], RoPE'd queries [B,Hq,n_q,D] of positions S - n_q .. S - 1 -> H2O scores [B,Hkv,S] in the cache
+    dtype: (1/G) sum over the group's query rows of the causal softmax(scaling q.k), / (S - s) rounded to the cache
+    dtype. Two passes over blocks of query rows in fp32: the row log-sum-exp, then the column sums; at most one block
+    of logits ([B, Hq, rows, S], at most `max_logits` elements) exists at a time."""
+    _require_cuda(keys)
+    B, Hkv, S, D = keys.shape
+    Hq, n_q = q.shape[1], q.shape[2]
+    G, off = Hq // Hkv, S - n_q
+    _note("ObservedAttention", keys, G)
+    block = max(1, max_logits // (B * Hq * S))
+    k = keys.float().unsqueeze(2)                                      # [B,Hkv,1,S,D]
+    qf = q.to(keys.dtype).float().reshape(B, Hkv, G, n_q, D) * scaling
+    pos = torch.arange(S, device=keys.device)
+
+    def logits(i0: int, i1: int) -> torch.Tensor:                      # [B,Hkv,G,i1-i0,S], causal
+        y = torch.matmul(qf[:, :, :, i0:i1], k.transpose(-1, -2))
+        rows = torch.arange(off + i0, off + i1, device=keys.device)
+        return y.masked_fill_(pos[None, :] > rows[:, None], float("-inf"))
+
+    lse = torch.empty((B, Hkv, G, n_q, 1), dtype=torch.float32, device=keys.device)
+    for i0 in range(0, n_q, block):
+        i1 = min(n_q, i0 + block)
+        lse[:, :, :, i0:i1] = torch.logsumexp(logits(i0, i1), dim=-1, keepdim=True)
+    col = torch.zeros((B, Hkv, S), dtype=torch.float32, device=keys.device)
+    for i0 in range(0, n_q, block):
+        i1 = min(n_q, i0 + block)
+        col += torch.exp(logits(i0, i1) - lse[:, :, :, i0:i1]).sum(dim=(2, 3))
+    div = torch.arange(S, 0, -1, device=keys.device).to(keys.dtype).float()
+    return (col / (G * div)).to(keys.dtype)
