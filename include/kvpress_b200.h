@@ -15,6 +15,7 @@
  *     kvp_keydiff_*            <- kvpress/presses/keydiff_press.py:36-46
  *     kvp_criticalkv_*         <- kvpress/presses/criticalkv_press.py:57-92 (on the wrapped press's scores)
  *     kvp_observed_attention_* <- kvpress/presses/observed_attention_press.py (H2O; from Q and K, no eager weights)
+ *     kvp_non_causal_attention_* <- kvpress/presses/non_causal_attention_press.py (Compactor's attention half)
  *     kvp_scores_compress      <- scorer_press.py:93-100 for an arbitrary score tensor
  *                                 (what wrapper presses / user ScorerPress subclasses need)
  *
@@ -73,7 +74,8 @@ typedef enum kvp_scorer {
     KVP_SCORER_EXPECTED_ATTENTION = 4,
     KVP_SCORER_KEYDIFF = 5,
     KVP_SCORER_CRITICALKV = 6,
-    KVP_SCORER_OBSERVED_ATTENTION = 7
+    KVP_SCORER_OBSERVED_ATTENTION = 7,
+    KVP_SCORER_NON_CAUSAL_ATTENTION = 8
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -205,6 +207,35 @@ int kvp_observed_attention_score(const kvp_problem* p, const void* K, const void
 int kvp_observed_attention_compress(const kvp_problem* p, const void* K, const void* V, const void* q, int32_t n_q,
                                     float scaling, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
                                     void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+
+/* ---- NonCausalAttnPress (kvpress/presses/non_causal_attention_press.py, the attention half of Compactor) -------------
+ * Prefill only. q: the RoPE'd queries of all S positions, contiguous [B, Hq, S, D], 16-byte aligned. With G = Hq / Hkv,
+ * the query heads h = j G + g of kv head j, cs = chunk_size and the chunks [c cs, (c+1) cs) of positions:
+ *   y[b,h,i,s]   = q[b,h,i] . K[b,j,s]  for i, s in the same chunk        (NO 1/sqrt(D) scaling)
+ *   A[b,h,s]     = sum_i softmax over the chunk's keys of y[b,h,i,:] at s   (non-causal)
+ *   x[b,j,s]     = (1/G) sum_g A[b,h,s] * ||V[b,j,s]||_2
+ *   pooled       = avg_pool1d(x, 3, padding 1, stride 1)                     (zeros outside [0, S), always / 3)
+ *   score        = (pooled - mean) / max(std, 1e-6)                          (fp32 evaluation, ONE rounding to the K dtype)
+ * mean and the unbiased std run over ALL B*Hkv*S entries, so the rows of a batch are coupled, and B*Hkv*S = 1 gives
+ * NaN, as torch's std. Padding of the last chunk (S not a multiple of cs; pad = ceil(S/cs) cs - S), as the reference:
+ * the pad padded keys are NOT masked, every valid query row of the last chunk sees them at logit 0 (the reference's
+ * -1e-9, to fp32 resolution); each of the pad padded query rows adds a uniform 1/cs to every valid key of that chunk.
+ * The reference rounds the logits and ||v|| to the cache dtype and returns fp32 z; here the formula is evaluated in fp32
+ * from the 16-bit inputs and z is rounded once. Selection keeps the n_kept largest rounded z (ties to the lowest
+ * positions), exactly what scores_out holds. head_dim 64 or 128, chunk_size 128 or 256 and 1 <= G <= 8, else
+ * KVP_ERR_UNSUPPORTED_SHAPE.
+ * Check order (the first failure is returned): validate the problem -> n_kept == 0 returns KVP_OK (compress) ->
+ * K / V / K_out / V_out null and alignment (compress) -> q null / alignment (and K, V, scores_out for the score call) ->
+ * chunk_size >= 1, else KVP_ERR_BAD_ARGUMENT -> shape instantiated, else KVP_ERR_UNSUPPORTED_SHAPE -> workspace.
+ * The compress call keeps the n_kept best scores (scores_out nullable). Memory beyond the workspace: none; no cs x cs
+ * tensor is formed. */
+int kvp_non_causal_attention_score(const kvp_problem* p, const void* K, const void* V, const void* q,
+                                   int32_t chunk_size, void* scores_out, void* workspace, size_t workspace_bytes,
+                                   kvp_stream_t stream);
+int kvp_non_causal_attention_compress(const kvp_problem* p, const void* K, const void* V, const void* q,
+                                      int32_t chunk_size, void* K_out, void* V_out, int32_t* idx_out,
+                                      void* scores_out, void* workspace, size_t workspace_bytes,
+                                      kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

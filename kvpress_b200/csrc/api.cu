@@ -11,13 +11,14 @@ namespace kvp {
 
 static thread_local char g_last_cuda_error[256] = "";
 
-// kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention, CriticalKV and ObservedAttention score launchers
-// report a shape they have no kernel for as cudaErrorNotSupported.
+// kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention, CriticalKV, ObservedAttention and
+// NonCausalAttention score launchers report a shape they have no kernel for as cudaErrorNotSupported.
 static int status(cudaError_t e, int scorer = KVP_SCORER_GENERIC) {
     if (e == cudaSuccess) return KVP_OK;
     if (e == cudaErrorNotSupported &&
         (scorer == KVP_SCORER_KEYDIFF || scorer == KVP_SCORER_SNAPKV || scorer == KVP_SCORER_EXPECTED_ATTENTION ||
-         scorer == KVP_SCORER_CRITICALKV || scorer == KVP_SCORER_OBSERVED_ATTENTION))
+         scorer == KVP_SCORER_CRITICALKV || scorer == KVP_SCORER_OBSERVED_ATTENTION ||
+         scorer == KVP_SCORER_NON_CAUSAL_ATTENTION))
         return KVP_ERR_UNSUPPORTED_SHAPE;
     snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
     // launch-configuration errors are not sticky: clear them, or the cudaPeekAtLastError() of every later call
@@ -82,7 +83,8 @@ static size_t layout(const Dims& d, int scorer, int window, void* base, Workspac
                        : scorer == KVP_SCORER_KEYDIFF            ? keydiff_scratch_bytes(d)
                        : scorer == KVP_SCORER_CRITICALKV         ? criticalkv_scratch_bytes(d)
                        : scorer == KVP_SCORER_OBSERVED_ATTENTION ? observed_attention_scratch_bytes(d, window)
-                                                                 : 0;
+                       : scorer == KVP_SCORER_NON_CAUSAL_ATTENTION ? non_causal_attention_scratch_bytes(d)
+                                                                   : 0;
     ws->scorer = c.take<char>(ws->scorer_bytes);
     return c.bytes;
 }
@@ -249,6 +251,8 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         // n_first, memset, keys of the final scores, select+compact
         case KVP_SCORER_CRITICALKV: *launches_out = 8; break;
         case KVP_SCORER_OBSERVED_ATTENTION: *launches_out = 5; break;  // memset, stats, colsum, finalize, select+compact
+        // memset, column sums, pooled partials, mean / std, z, select+compact
+        case KVP_SCORER_NON_CAUSAL_ATTENTION: *launches_out = 6; break;
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -487,6 +491,46 @@ int kvp_observed_attention_compress(const kvp_problem* p, const void* K, const v
     };
     return run(Kind::compress, p, KVP_SCORER_OBSERVED_ATTENTION, n_q, {K, V, K_out, V_out, idx_out, nullptr}, operands,
                observed_attention_stage(p, K, q, n_q, scaling, scores_out), workspace, workspace_bytes, stream);
+}
+
+// ---- NonCausalAttention --------------------------------------------------------------------------
+// The operand checks both entry points share, after their null / alignment checks.
+static int non_causal_attention_args(const Dims& d, int32_t chunk_size) {
+    if (chunk_size < 1) return KVP_ERR_BAD_ARGUMENT;
+    return non_causal_attention_supported(d, chunk_size) ? KVP_OK : KVP_ERR_UNSUPPORTED_SHAPE;
+}
+
+static auto non_causal_attention_stage(const kvp_problem* p, const void* K, const void* V, const void* q,
+                                       int32_t chunk_size, void* scores_out) {
+    return [=](const Call& c) {
+        return launch_non_causal_attention_score(c.d, p->dtype, K, V, q, chunk_size, c.ws, scores_out, c.st);
+    };
+}
+
+int kvp_non_causal_attention_score(const kvp_problem* p, const void* K, const void* V, const void* q,
+                                   int32_t chunk_size, void* scores_out, void* workspace, size_t workspace_bytes,
+                                   kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!K || !V || !q || !scores_out) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(K) || !aligned16(V) || !aligned16(q)) return KVP_ERR_BAD_STRIDE;
+        return non_causal_attention_args(d, chunk_size);
+    };
+    return run(Kind::score, p, KVP_SCORER_NON_CAUSAL_ATTENTION, 0, {}, operands,
+               non_causal_attention_stage(p, K, V, q, chunk_size, scores_out), workspace, workspace_bytes, stream);
+}
+
+int kvp_non_causal_attention_compress(const kvp_problem* p, const void* K, const void* V, const void* q,
+                                      int32_t chunk_size, void* K_out, void* V_out, int32_t* idx_out,
+                                      void* scores_out, void* workspace, size_t workspace_bytes,
+                                      kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!q) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(q)) return KVP_ERR_BAD_STRIDE;
+        return non_causal_attention_args(d, chunk_size);
+    };
+    return run(Kind::compress, p, KVP_SCORER_NON_CAUSAL_ATTENTION, 0, {K, V, K_out, V_out, idx_out, nullptr},
+               operands, non_causal_attention_stage(p, K, V, q, chunk_size, scores_out), workspace, workspace_bytes,
+               stream);
 }
 
 // ---- generic scores ------------------------------------------------------------------------------

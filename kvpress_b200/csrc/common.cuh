@@ -44,7 +44,7 @@ struct Workspace {
                          // zero = row not scanned yet
     int R;
     void* scorer;        // scorer-specific scratch (SnapKV / ExpectedAttention / KeyDiff / CriticalKV /
-                         // ObservedAttention)
+                         // ObservedAttention / NonCausalAttention)
     size_t scorer_bytes;
     int S_pad;
     int n_tiles;
@@ -352,5 +352,9 @@ cudaError_t launch_criticalkv_score(const Dims& d, int dtype, const void* V, con
 size_t observed_attention_scratch_bytes(const Dims& d, int n_q);
 cudaError_t launch_observed_attention_score(const Dims& d, int dtype, const void* K, const void* q, int n_q,
                                             float scaling, const Workspace& ws, void* scores_out, cudaStream_t st);
+size_t non_causal_attention_scratch_bytes(const Dims& d);
+bool non_causal_attention_supported(const Dims& d, int chunk_size);
+cudaError_t launch_non_causal_attention_score(const Dims& d, int dtype, const void* K, const void* V, const void* q,
+                                              int chunk_size, const Workspace& ws, void* scores_out, cudaStream_t st);
 
 }  // namespace kvp

@@ -19,7 +19,7 @@ _LIB_NAME = "libkvpress_b200.so"
 _LIB_PATH = Path(__file__).resolve().parent / _LIB_NAME
 
 (SCORER_GENERIC, SCORER_KNORM, SCORER_STREAMING, SCORER_SNAPKV, SCORER_EXPECTED_ATTENTION, SCORER_KEYDIFF,
- SCORER_CRITICALKV, SCORER_OBSERVED_ATTENTION) = range(8)
+ SCORER_CRITICALKV, SCORER_OBSERVED_ATTENTION, SCORER_NON_CAUSAL_ATTENTION) = range(9)
 _DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
 
@@ -81,6 +81,8 @@ SIGNATURES = {
     "kvp_observed_attention_score": (ctypes.c_int, [_PP, _P, _P, _I, ctypes.c_float, _P, _P, _SZ, _P]),
     "kvp_observed_attention_compress": (
         ctypes.c_int, [_PP, _P, _P, _P, _I, ctypes.c_float, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_non_causal_attention_score": (ctypes.c_int, [_PP, _P, _P, _P, _I, _P, _P, _SZ, _P]),
+    "kvp_non_causal_attention_compress": (ctypes.c_int, [_PP, _P, _P, _P, _I, _P, _P, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -592,3 +594,37 @@ def observed_attention_compress(keys, values, q, scaling: float, n_kept: int, re
     q = _check_queries(q, keys)
     return _compress("kvp_observed_attention_compress", SCORER_OBSERVED_ATTENTION, keys, values, n_kept,
                      (keys, values, q, q.shape[2], float(scaling)), return_indices, return_scores, q.shape[1])
+
+
+# --------------------------------------------------------------------------------------------------
+# NonCausalAttention (the attention half of Compactor)
+# --------------------------------------------------------------------------------------------------
+def _check_prefill_queries(q: torch.Tensor, keys: torch.Tensor) -> torch.Tensor:
+    """RoPE'd queries [B, Hq, S, D] of every cached position, in the cache dtype and on its device, made contiguous."""
+    B, _, S, D = keys.shape
+    if q.dim() != 4 or q.shape[0] != B or q.shape[2] != S or q.shape[3] != D:
+        raise RuntimeError(f"q must be [B, Hq, {S}, {D}] (prefill: one query per cached position), got {tuple(q.shape)}")
+    if q.dtype != keys.dtype or q.device != keys.device:
+        raise RuntimeError("q must share dtype and device with the keys")
+    return q.contiguous()
+
+
+def non_causal_attention_score(keys, values, q, chunk_size: int) -> torch.Tensor:
+    """NonCausalAttnPress scores [B, Hkv, S]: the chunked non-causal softmax(q.k) (no scaling) summed over each chunk's
+    queries, averaged over the group, times ||v||, pooled over 3 positions and z-normalised over the whole tensor."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    q = _check_prefill_queries(q, keys)
+    p = make_problem(keys, values, 0, q.shape[1])
+    return _score("kvp_non_causal_attention_score", SCORER_NON_CAUSAL_ATTENTION, keys, p, keys, values, q,
+                  int(chunk_size))
+
+
+def non_causal_attention_compress(keys, values, q, chunk_size: int, n_kept: int, return_indices: bool = False,
+                                  return_scores: bool = False):
+    """non_causal_attention_score, then top-n_kept + compaction."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    q = _check_prefill_queries(q, keys)
+    return _compress("kvp_non_causal_attention_compress", SCORER_NON_CAUSAL_ATTENTION, keys, values, n_kept,
+                     (keys, values, q, int(chunk_size)), return_indices, return_scores, q.shape[1])

@@ -11,7 +11,8 @@ result goes through the sm_90a selection + compaction kernels like any caller-su
 Formulas: SnapKV `kvpress/presses/snapkv_press.py:41-105`, ExpectedAttention
 `kvpress/presses/expected_attention_press.py:136-165`, CriticalKV `kvpress/presses/criticalkv_press.py:57-92` (head_dim
 other than 64 / 128), ObservedAttention `kvpress/presses/observed_attention_press.py` (head_dim other than 64 / 128, more
-than 8 query heads per kv head).
+than 8 query heads per kv head), NonCausalAttention `kvpress/presses/non_causal_attention_press.py` (head_dim other than
+64 / 128, more than 8 query heads per kv head, chunk sizes other than 128 / 256).
 """
 from __future__ import annotations
 
@@ -49,6 +50,12 @@ def observed_attention_on_tensor_cores(head_dim: int, group: int) -> bool:
     """Shapes `kvp_observed_attention_*` instantiates (csrc/observed_attention.cu launch_obs_d): head_dim 64 / 128, at
     most 8 query heads per kv head."""
     return head_dim in TENSOR_CORE_HEAD_DIMS and 1 <= group <= MAX_GROUP
+
+
+def non_causal_attention_on_tensor_cores(head_dim: int, group: int, chunk_size: int) -> bool:
+    """Shapes `kvp_non_causal_attention_*` instantiates (csrc/non_causal_attention.cu launch_nca_d): head_dim 64 / 128,
+    chunk_size 128 / 256, at most 8 query heads per kv head."""
+    return head_dim in TENSOR_CORE_HEAD_DIMS and chunk_size in (128, 256) and 1 <= group <= MAX_GROUP
 
 
 def _note(what: str, keys: torch.Tensor, group: int) -> None:
@@ -189,3 +196,30 @@ def observed_attention_scores(keys: torch.Tensor, q: torch.Tensor, scaling: floa
         col += torch.exp(logits(i0, i1) - lse[:, :, :, i0:i1]).sum(dim=(2, 3))
     div = torch.arange(S, 0, -1, device=keys.device).to(keys.dtype).float()
     return (col / (G * div)).to(keys.dtype)
+
+
+def non_causal_attention_scores(keys: torch.Tensor, values: torch.Tensor, q: torch.Tensor, chunk_size: int,
+                                max_logits: int = 1 << 27) -> torch.Tensor:
+    """keys / values [B,Hkv,S,D], RoPE'd queries [B,Hq,S,D] -> NonCausalAttnPress z-scores [B,Hkv,S] in the cache
+    dtype, by the definition of include/kvpress_b200.h (kvp_non_causal_attention_score): fp32 over blocks of chunks (at
+    most `max_logits` logits at a time), the padded last chunk as the reference pads it, one rounding."""
+    _require_cuda(keys)
+    B, Hkv, S, D = keys.shape
+    G, cs = q.shape[1] // Hkv, int(chunk_size)
+    _note("NonCausalAttention", keys, G)
+    n_chunks = -(-S // cs)
+    pad = n_chunks * cs - S
+    kf = F.pad(keys.float(), (0, 0, 0, pad)).view(B, Hkv, 1, n_chunks, cs, D)
+    qf = F.pad(q.to(keys.dtype).float(), (0, 0, 0, pad)).view(B, Hkv, G, n_chunks, cs, D)
+    colsum = torch.empty((B, Hkv, n_chunks, cs), dtype=torch.float32, device=keys.device)
+    block = max(1, max_logits // (B * Hkv * G * cs * cs))
+    for c0 in range(0, n_chunks, block):
+        c1 = min(n_chunks, c0 + block)
+        y = torch.matmul(qf[:, :, :, c0:c1], kf[:, :, :, c0:c1].transpose(-1, -2))   # [B,Hkv,G,c,cs,cs]
+        if pad and c1 == n_chunks:   # padded query rows: uniform over the chunk; padded keys stay at logit 0
+            y[:, :, :, -1, cs - pad:] = 0
+        colsum[:, :, c0:c1] = torch.softmax(y, dim=-1).sum(dim=-2).mean(dim=2)
+        del y
+    x = colsum.view(B, Hkv, n_chunks * cs)[..., :S] * values.float().norm(dim=-1)
+    pooled = F.avg_pool1d(x, kernel_size=3, padding=1, stride=1)
+    return ((pooled - pooled.mean()) / pooled.std().clamp_min(1e-6)).to(keys.dtype)
