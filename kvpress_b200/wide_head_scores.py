@@ -8,6 +8,14 @@ definition the kernels implement ("fp32 evaluation of the reference formula, rou
 result goes through the sm_90a selection + compaction kernels like any caller-supplied score tensor
 (`native.scores_compress`). Nothing here runs on the CPU; CPU tensors are refused like everywhere else.
 
+Every GEMM operand is a 16-bit value (the cache's, or the model's queries) widened to fp32, and the scales (1/sqrt(d), 1/(2d), the attention
+`scaling`) multiply the fp32 GEMM results, never an operand. fp32 matmuls follow the process-wide
+`torch.backends.cuda.matmul.fp32_precision`: under "tf32" (what `torch.set_float32_matmul_precision("high")` selects)
+cuBLAS rounds its operands to 10 mantissa bits. A scaled operand would lose up to 2^-11 of itself there, which the
+softmax turns into several fp16 ulps of error at logits near 20. A 16-bit value fits TF32 exactly, and its products are
+exact and summed in fp32, so the result keeps the contract whatever the caller has set. The setting itself is never
+touched here: it is global to the process, shared between threads, and the caller's to choose.
+
 Formulas: SnapKV `kvpress/presses/snapkv_press.py:41-105`, ExpectedAttention
 `kvpress/presses/expected_attention_press.py:136-165`, CriticalKV `kvpress/presses/criticalkv_press.py:57-92` (head_dim
 other than 64 / 128), ObservedAttention `kvpress/presses/observed_attention_press.py` (head_dim other than 64 / 128, more
@@ -93,11 +101,12 @@ def snapkv_scores(keys: torch.Tensor, q_window: torch.Tensor, window: int, kerne
     B, Hkv, S, D = keys.shape
     G, w = q_window.shape[1] // Hkv, window
     _note("SnapKV", keys, G)
-    q = q_window.float().reshape(B, Hkv, G * w, D) * (1.0 / math.sqrt(D))
+    q = q_window.float().reshape(B, Hkv, G * w, D)
     logits = torch.empty((B, Hkv, G * w, S), dtype=torch.float32, device=keys.device)
     for s0 in range(0, S, chunk):  # fp32 copies of K one slab at a time
         s1 = min(S, s0 + chunk)
         torch.matmul(q, keys[:, :, s0:s1].float().transpose(-1, -2), out=logits[..., s0:s1])
+    logits.mul_(1.0 / math.sqrt(D))
     # inside the window query i (position S - w + i) does not see key S - w + j for j > i
     future = torch.ones((w, w), dtype=torch.bool, device=keys.device).triu(1)
     logits.view(B, Hkv, G, w, S)[..., S - w:].masked_fill_(future, float("-inf"))
@@ -116,16 +125,16 @@ def expected_attention_scores(keys: torch.Tensor, values: torch.Tensor, mu: torc
     G = mu.shape[1] // Hkv
     _note("ExpectedAttention", keys, G)
     L = S - n_sink
-    mu_f = mu.to(keys.dtype).float().reshape(B, Hkv, G, D) * (1.0 / math.sqrt(D))   # operands in the cache dtype,
-    cov_f = None if cov is None else cov.to(keys.dtype).float().reshape(B, Hkv, G, D, D) * (0.5 / D)  # like the C ABI
+    mu_f = mu.to(keys.dtype).float().reshape(B, Hkv, G, D)                    # operands in the cache dtype,
+    cov_f = None if cov is None else cov.to(keys.dtype).float().reshape(B, Hkv, G, D, D)  # like the C ABI
     logits = torch.empty((B, Hkv, G, L), dtype=torch.float32, device=keys.device)
     for s0 in range(0, L, chunk):
         s1 = min(L, s0 + chunk)
         k = keys[:, :, n_sink + s0:n_sink + s1].float()               # [B,Hkv,c,D]
-        part = torch.matmul(mu_f, k.transpose(-1, -2))                 # mu.k / sqrt(d)
+        part = torch.matmul(mu_f, k.transpose(-1, -2)) * (1.0 / math.sqrt(D))    # mu.k / sqrt(d)
         if cov_f is not None:                                          # + k^T Sigma k / 2d
             y = torch.matmul(k.unsqueeze(2), cov_f)                    # [B,Hkv,G,c,D]
-            part = part + (y * k.unsqueeze(2)).sum(dim=-1)
+            part = part + (y * k.unsqueeze(2)).sum(dim=-1) * (0.5 / D)
         logits[..., s0:s1] = part
     score = torch.softmax(logits, dim=-1).mean(dim=2)                  # [B,Hkv,L]
     if use_vnorm:
@@ -178,11 +187,11 @@ def observed_attention_scores(keys: torch.Tensor, q: torch.Tensor, scaling: floa
     _note("ObservedAttention", keys, G)
     block = max(1, max_logits // (B * Hq * S))
     k = keys.float().unsqueeze(2)                                      # [B,Hkv,1,S,D]
-    qf = q.to(keys.dtype).float().reshape(B, Hkv, G, n_q, D) * scaling
+    qf = q.to(keys.dtype).float().reshape(B, Hkv, G, n_q, D)
     pos = torch.arange(S, device=keys.device)
 
     def logits(i0: int, i1: int) -> torch.Tensor:                      # [B,Hkv,G,i1-i0,S], causal
-        y = torch.matmul(qf[:, :, :, i0:i1], k.transpose(-1, -2))
+        y = torch.matmul(qf[:, :, :, i0:i1], k.transpose(-1, -2)).mul_(scaling)
         rows = torch.arange(off + i0, off + i1, device=keys.device)
         return y.masked_fill_(pos[None, :] > rows[:, None], float("-inf"))
 

@@ -245,19 +245,6 @@ def test_no_intermediate_at_32k():
     assert grown < B * S * hidden * 2  # one head's [S, hidden] product alone would exceed this
 
 
-@gpu
-@pytest.mark.parametrize("D", [96, 256])
-def test_wide_head_fallback_vs_fp64(D):
-    from kvpress_b200 import wide_head_scores
-
-    assert not wide_head_scores.criticalkv_on_tensor_cores(D)
-    v, wo, base = inputs(1, 2, 3, 700, D, 600, torch.bfloat16, seed=D)
-    got = wide_head_scores.criticalkv_scores(base, v, wo, 1e-4, 70)
-    assert_scores(got, base, v, wo, 1e-4, 70, f"ckv fallback d{D}")
-    with pytest.raises(RuntimeError, match="unsupported shape"):
-        _native().criticalkv_score(base, v, wo, 1e-4, 70)
-
-
 # --------------------------------------------------------------------------------------------------
 # the reference's evaluation registry on a GPU tiny Llama, against the same presses over the oracle stand-ins
 # --------------------------------------------------------------------------------------------------

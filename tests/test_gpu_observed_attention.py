@@ -152,7 +152,7 @@ def test_unsupported_shapes():
 
 
 # --------------------------------------------------------------------------------------------------
-# graph replay, memory, the cuBLAS fallback
+# graph replay, memory (the torch GEMM fallback: tests/test_gpu_wide_head_sweep.py)
 # --------------------------------------------------------------------------------------------------
 @gpu
 def test_replays_under_capture():
@@ -190,17 +190,6 @@ def test_no_intermediate_at_32k():
     q_bytes = q.numel() * q.element_size()
     assert grown <= max(ws, 1 << 20) + outputs + q_bytes + (1 << 16), (grown, ws, outputs)
     assert grown < B * Hkv * G * S * S // 64  # a 64th of one layer's [B, Hq, S, S] bf16 weights
-
-
-@gpu
-@pytest.mark.parametrize("D,G", [(96, 4), (256, 2), (128, 16)])
-def test_fallback_vs_fp64(D, G):
-    from kvpress_b200 import wide_head_scores
-
-    assert not wide_head_scores.observed_attention_on_tensor_cores(D, G)
-    k, _, q = inputs(1, 2, G, 900, 700, D, torch.bfloat16, seed=D + G)
-    got = wide_head_scores.observed_attention_scores(k, q, D ** -0.5, max_logits=1 << 20)  # several query blocks
-    assert_vs_ref64(got, ref64(k, q, D ** -0.5), torch.zeros(900, dtype=torch.bool), f"obs fallback d{D} g{G}")
 
 
 # --------------------------------------------------------------------------------------------------

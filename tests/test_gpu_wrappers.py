@@ -375,12 +375,22 @@ def test_tensor_core_scorers_state_their_shape_limits():
     assert nat.knorm_score(k).shape == (1, 2, 600)
 
 
+@pytest.fixture(params=["ieee", "tf32"])
+def fp32_precision(request):
+    """torch's fp32 matmul precision for one test; the caller's setting is restored afterwards."""
+    matmul = torch.backends.cuda.matmul
+    saved = matmul.fp32_precision
+    request.addfinalizer(lambda: setattr(matmul, "fp32_precision", saved))
+    matmul.fp32_precision = request.param
+    return request.param
+
+
 @pytest.mark.parametrize("D,Hq,Hkv", [(96, 4, 2), (256, 4, 1), (128, 16, 1)])
-def test_presses_on_head_dims_outside_the_tensor_core_set(D, Hq, Hkv):
+def test_presses_on_head_dims_outside_the_tensor_core_set(D, Hq, Hkv, fp32_precision):
     """Phi-3 (head_dim 96), Gemma-3 (256), 16 query heads per kv head: the C ABI states the limit (test above), the
     presses score those shapes with cuBLAS GEMMs on the GPU (kvpress_b200/wide_head_scores.py: fp32, one rounding) and
     select + compact on the sm_90a kernels. Scores <= 1 ulp from the oracle's fp32 evaluation, kept rows == the
-    canonical selection of the press's own scores."""
+    canonical selection of the press's own scores, under either fp32 matmul precision (TF32 must not change them)."""
     from kvpress_b200 import ExpectedAttentionPress, SnapKVPress
 
     torch.manual_seed(D + Hq)
