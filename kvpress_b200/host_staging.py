@@ -12,7 +12,7 @@ and the three stages run on three streams,
 so the host link is busy in both directions at once and the kernels hide under the copies: the step costs
 max(H2D, D2H) + one chunk of latency instead of H2D + compute + D2H.
 
-`values_zero_copy=True` (scorers that never read V to score: Knorm, SnapKV, StreamingLLM): V is not staged at
+`values_zero_copy=True` (scorers that never read V to score: Knorm, KeyDiff, SnapKV, StreamingLLM): V is not staged at
 all — the compaction kernel reads the KEPT rows of V straight from the pinned host buffer over PCIe (UVA), so
 only n_kept/S of V crosses the link.
 
@@ -90,7 +90,8 @@ def compress_host(scorer: str, keys_host: torch.Tensor, values_host: torch.Tenso
     if values_zero_copy is None:
         values_zero_copy = False
     if values_zero_copy and scorer == "expected_attention":
-        raise RuntimeError("values_zero_copy needs a scorer that does not read V to score (Knorm, SnapKV, StreamingLLM)")
+        raise RuntimeError("values_zero_copy needs a scorer that does not read V to score (Knorm, KeyDiff, SnapKV, "
+                           "StreamingLLM)")
     Hq = num_q_heads or {"snapkv": lambda: params["q_window"].shape[1],
                          "expected_attention": lambda: params["mu"].shape[1]}.get(scorer, lambda: H)()
     G = Hq // H
