@@ -16,6 +16,7 @@
  *     kvp_criticalkv_*         <- kvpress/presses/criticalkv_press.py:57-92 (on the wrapped press's scores)
  *     kvp_observed_attention_* <- kvpress/presses/observed_attention_press.py (H2O; from Q and K, no eager weights)
  *     kvp_non_causal_attention_* <- kvpress/presses/non_causal_attention_press.py (Compactor's attention half)
+ *     kvp_lagkv_*              <- kvpress/presses/lagkv_press.py (lag-relative K / V statistics, from K and V only)
  *     kvp_scores_compress      <- scorer_press.py:93-100 for an arbitrary score tensor
  *                                 (what wrapper presses / user ScorerPress subclasses need)
  *
@@ -75,7 +76,8 @@ typedef enum kvp_scorer {
     KVP_SCORER_KEYDIFF = 5,
     KVP_SCORER_CRITICALKV = 6,
     KVP_SCORER_OBSERVED_ATTENTION = 7,
-    KVP_SCORER_NON_CAUSAL_ATTENTION = 8
+    KVP_SCORER_NON_CAUSAL_ATTENTION = 8,
+    KVP_SCORER_LAGKV = 9
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -236,6 +238,38 @@ int kvp_non_causal_attention_compress(const kvp_problem* p, const void* K, const
                                       int32_t chunk_size, void* K_out, void* V_out, int32_t* idx_out,
                                       void* scores_out, void* workspace, size_t workspace_bytes,
                                       kvp_stream_t stream);
+
+/* ---- LagKVPress (kvpress/presses/lagkv_press.py, https://arxiv.org/abs/2504.04704) ----------------------------------
+ * Reads K and V only. Per row (b, kv head j), with S positions and L = lag_size:
+ *   - Short cache, S < n_sink + 2L. Position s < n_sink scores 1. Position s >= n_sink scores
+ *     fp32(s - n_sink) / fp32(S - n_sink), rounded once to the cache dtype (the reference's float32 arange / n).
+ *   - Otherwise P = (S - n_sink) // L, partition c covers [n_sink + cL, n_sink + (c+1)L), and partitions
+ *     c = 0 ... P-2 are scored, each against partition c+1. The sinks, partition P-1 and the remainder score 1.
+ *   - Within a scored partition, per channel d: lo_d / hi_d = min / max over the reference partition's L rows,
+ *     x = (k - lo) / (hi - lo) with IEEE rules (x/0 = +-inf, 0/0 = NaN), sigma_k = unbiased std of x over d
+ *     (divisor D - 1), a_k = softmax of sigma_k over the L rows; sigma_v and a_v likewise from V;
+ *     c = (a_k + a_v) / 2.
+ *   - cross_scoring != 0: the score is c rounded once. Otherwise it is fp32(r) / fp32(L) rounded once, with the rank
+ *     r(s) = #{t : c(t) < c(s)} + #{t < s : c(t) = c(s)} over the partition; NaN compares above every number and equal
+ *     to NaN (torch.sort(stable=True)).
+ * A constant channel of a reference partition, in K or V (a zeroed channel, or any partition when L = 1), makes every c
+ * of the partition it scores NaN: NaN cross scores and ranks in position order, as in the reference. So does a NaN in
+ * the reference partition's K or V (torch.min / max propagate it). Where an fp32 intermediate overflows, which only bf16
+ * inputs can cause (a reference range hi - lo beyond the fp32 range, or one so small that x or its square overflows),
+ * the scores depart from the definition, and an overflowing sigma makes the whole partition NaN.
+ * The reference evaluates the chain in the cache dtype; here it is fp32, rounded once. Ties in the rank go to the earlier
+ * position. 1 <= lag_size <= 1024 (kLagMax), every head_dim the problem validates. V must be device memory.
+ * Check order (the first failure is returned): validate the problem -> n_kept == 0 returns KVP_OK (compress) ->
+ * K / V / K_out / V_out null and alignment (compress) -> K, V, scores_out null and K / V alignment (score call) ->
+ * n_sink < 0 or lag_size < 1 gives KVP_ERR_BAD_ARGUMENT -> lag_size > 1024 gives KVP_ERR_UNSUPPORTED_SHAPE ->
+ * workspace. One kernel writes the scores and the selection keys; a compress takes 3 launches (memset, score,
+ * select+compact) and keeps the n_kept best scores (scores_out nullable). Memory beyond the workspace: none. */
+int kvp_lagkv_score(const kvp_problem* p, const void* K, const void* V, int32_t n_sink, int32_t lag_size,
+                    int32_t cross_scoring, void* scores_out, void* workspace, size_t workspace_bytes,
+                    kvp_stream_t stream);
+int kvp_lagkv_compress(const kvp_problem* p, const void* K, const void* V, int32_t n_sink, int32_t lag_size,
+                       int32_t cross_scoring, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
+                       void* workspace, size_t workspace_bytes, kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

@@ -18,6 +18,7 @@ from kvpress_b200.presses.expected_attention_with_stats import ExpectedAttention
 from kvpress_b200.presses.key_rerotation_press import KeyRerotationPress
 from kvpress_b200.presses.keydiff_press import KeyDiffPress
 from kvpress_b200.presses.knorm_press import KnormPress
+from kvpress_b200.presses.lagkv_press import LagKVPress
 from kvpress_b200.presses.non_causal_attention_press import NonCausalAttnPress
 from kvpress_b200.presses.observed_attention_press import ObservedAttentionPress
 from kvpress_b200.presses.per_layer_compression_press import PerLayerCompressionPress
@@ -50,6 +51,7 @@ __all__ = [
     "CriticalAdaKVPress",
     "ObservedAttentionPress",
     "NonCausalAttnPress",
+    "LagKVPress",
     "BlockPress",
     "ChunkPress",
     "ChunkKVPress",

@@ -11,14 +11,14 @@ namespace kvp {
 
 static thread_local char g_last_cuda_error[256] = "";
 
-// kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention, CriticalKV, ObservedAttention and
-// NonCausalAttention score launchers report a shape they have no kernel for as cudaErrorNotSupported.
+// kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention, CriticalKV, ObservedAttention, NonCausalAttention
+// and LagKV score launchers report a shape they have no kernel for as cudaErrorNotSupported.
 static int status(cudaError_t e, int scorer = KVP_SCORER_GENERIC) {
     if (e == cudaSuccess) return KVP_OK;
     if (e == cudaErrorNotSupported &&
         (scorer == KVP_SCORER_KEYDIFF || scorer == KVP_SCORER_SNAPKV || scorer == KVP_SCORER_EXPECTED_ATTENTION ||
          scorer == KVP_SCORER_CRITICALKV || scorer == KVP_SCORER_OBSERVED_ATTENTION ||
-         scorer == KVP_SCORER_NON_CAUSAL_ATTENTION))
+         scorer == KVP_SCORER_NON_CAUSAL_ATTENTION || scorer == KVP_SCORER_LAGKV))
         return KVP_ERR_UNSUPPORTED_SHAPE;
     snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
     // launch-configuration errors are not sticky: clear them, or the cudaPeekAtLastError() of every later call
@@ -253,6 +253,7 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         case KVP_SCORER_OBSERVED_ATTENTION: *launches_out = 5; break;  // memset, stats, colsum, finalize, select+compact
         // memset, column sums, pooled partials, mean / std, z, select+compact
         case KVP_SCORER_NON_CAUSAL_ATTENTION: *launches_out = 6; break;
+        case KVP_SCORER_LAGKV: *launches_out = 3; break;  // memset, scores + keys, select+compact
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -531,6 +532,39 @@ int kvp_non_causal_attention_compress(const kvp_problem* p, const void* K, const
     return run(Kind::compress, p, KVP_SCORER_NON_CAUSAL_ATTENTION, 0, {K, V, K_out, V_out, idx_out, nullptr},
                operands, non_causal_attention_stage(p, K, V, q, chunk_size, scores_out), workspace, workspace_bytes,
                stream);
+}
+
+// ---- LagKV ---------------------------------------------------------------------------------------
+// The operand checks both entry points share, after their null / alignment checks.
+static int lagkv_args(int32_t n_sink, int32_t lag_size) {
+    if (n_sink < 0 || lag_size < 1) return KVP_ERR_BAD_ARGUMENT;
+    return lag_size > kLagMax ? KVP_ERR_UNSUPPORTED_SHAPE : KVP_OK;
+}
+
+int kvp_lagkv_score(const kvp_problem* p, const void* K, const void* V, int32_t n_sink, int32_t lag_size,
+                    int32_t cross_scoring, void* scores_out, void* workspace, size_t workspace_bytes,
+                    kvp_stream_t stream) {
+    auto operands = [&](const Dims&) -> int {
+        if (!K || !V || !scores_out) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(K) || !aligned16(V)) return KVP_ERR_BAD_STRIDE;
+        return lagkv_args(n_sink, lag_size);
+    };
+    auto score = [&](const Call& c) {
+        return launch_lagkv_score(c.d, p->dtype, K, V, n_sink, lag_size, cross_scoring, c.ws, scores_out, false, c.st);
+    };
+    // the kernel writes no keys and no histogram when the selection is skipped: nothing to clear
+    return run(Kind::score, p, KVP_SCORER_LAGKV, 0, {}, operands, score, workspace, workspace_bytes, stream, false);
+}
+
+int kvp_lagkv_compress(const kvp_problem* p, const void* K, const void* V, int32_t n_sink, int32_t lag_size,
+                       int32_t cross_scoring, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
+                       void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims&) { return lagkv_args(n_sink, lag_size); };
+    auto score = [&](const Call& c) {
+        return launch_lagkv_score(c.d, p->dtype, K, V, n_sink, lag_size, cross_scoring, c.ws, scores_out, true, c.st);
+    };
+    return run(Kind::compress, p, KVP_SCORER_LAGKV, 0, {K, V, K_out, V_out, idx_out, nullptr}, operands, score,
+               workspace, workspace_bytes, stream);
 }
 
 // ---- generic scores ------------------------------------------------------------------------------

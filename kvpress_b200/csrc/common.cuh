@@ -17,6 +17,7 @@ constexpr int kSfxStride = 264;     // u16 per tile record: sfx[0..256], gt_hi a
 constexpr uint16_t kForcedKey = 0xFFFFu;  // ordered key of a forced-keep position
 constexpr int kFinalizeTiles = 1;          // 256-position tiles per CTA of the finalize kernels (1: >5 waves at 128k, no tail)
 constexpr int kScoreChunkGeneric = 256;   // positions per CTA of the plain streaming score kernels
+constexpr int kLagMax = 1024;              // largest LagKV lag_size (partition length) the kernel scores
 // counters[] layout: [0] ticket, [1, 1+R) refine done, [1+R, 1+2R) row ready, then the slot below:
 // order-preserving uint image of the largest valid score (for the reference's max+1 sentinel);
 // [2+2R, 2+3R) score items done per row (fused Knorm kernel)
@@ -44,7 +45,7 @@ struct Workspace {
                          // zero = row not scanned yet
     int R;
     void* scorer;        // scorer-specific scratch (SnapKV / ExpectedAttention / KeyDiff / CriticalKV /
-                         // ObservedAttention / NonCausalAttention)
+                         // ObservedAttention / NonCausalAttention; LagKV needs none)
     size_t scorer_bytes;
     int S_pad;
     int n_tiles;
@@ -356,5 +357,7 @@ size_t non_causal_attention_scratch_bytes(const Dims& d);
 bool non_causal_attention_supported(const Dims& d, int chunk_size);
 cudaError_t launch_non_causal_attention_score(const Dims& d, int dtype, const void* K, const void* V, const void* q,
                                               int chunk_size, const Workspace& ws, void* scores_out, cudaStream_t st);
+cudaError_t launch_lagkv_score(const Dims& d, int dtype, const void* K, const void* V, int n_sink, int lag_size,
+                               int cross, const Workspace& ws, void* scores_out, bool want_keys, cudaStream_t st);
 
 }  // namespace kvp

@@ -19,7 +19,8 @@ _LIB_NAME = "libkvpress_b200.so"
 _LIB_PATH = Path(__file__).resolve().parent / _LIB_NAME
 
 (SCORER_GENERIC, SCORER_KNORM, SCORER_STREAMING, SCORER_SNAPKV, SCORER_EXPECTED_ATTENTION, SCORER_KEYDIFF,
- SCORER_CRITICALKV, SCORER_OBSERVED_ATTENTION, SCORER_NON_CAUSAL_ATTENTION) = range(9)
+ SCORER_CRITICALKV, SCORER_OBSERVED_ATTENTION, SCORER_NON_CAUSAL_ATTENTION, SCORER_LAGKV) = range(10)
+LAG_MAX = 1024  # the largest lag_size the LagKV kernel scores (kLagMax in csrc/common.cuh)
 _DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
 
@@ -83,6 +84,8 @@ SIGNATURES = {
         ctypes.c_int, [_PP, _P, _P, _P, _I, ctypes.c_float, _P, _P, _P, _P, _P, _SZ, _P]),
     "kvp_non_causal_attention_score": (ctypes.c_int, [_PP, _P, _P, _P, _I, _P, _P, _SZ, _P]),
     "kvp_non_causal_attention_compress": (ctypes.c_int, [_PP, _P, _P, _P, _I, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_lagkv_score": (ctypes.c_int, [_PP, _P, _P, _I, _I, _I, _P, _P, _SZ, _P]),
+    "kvp_lagkv_compress": (ctypes.c_int, [_PP, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -628,3 +631,26 @@ def non_causal_attention_compress(keys, values, q, chunk_size: int, n_kept: int,
     q = _check_prefill_queries(q, keys)
     return _compress("kvp_non_causal_attention_compress", SCORER_NON_CAUSAL_ATTENTION, keys, values, n_kept,
                      (keys, values, q, int(chunk_size)), return_indices, return_scores, q.shape[1])
+
+
+# --------------------------------------------------------------------------------------------------
+# LagKV
+# --------------------------------------------------------------------------------------------------
+def lagkv_score(keys, values, n_sink: int, lag_size: int, cross_scoring: bool) -> torch.Tensor:
+    """LagKVPress scores [B, Hkv, S] (include/kvpress_b200.h, kvp_lagkv_score): per partition of lag_size positions, the
+    softmax of the std of the keys and values scaled by the next partition's min / max, as ranks / lag_size, or the
+    averaged softmax itself with cross_scoring; the sinks and the tail score 1."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    return _score("kvp_lagkv_score", SCORER_LAGKV, keys, make_problem(keys, values, 0), keys, values, int(n_sink),
+                  int(lag_size), int(bool(cross_scoring)))
+
+
+def lagkv_compress(keys, values, n_sink: int, lag_size: int, cross_scoring: bool, n_kept: int,
+                   return_indices: bool = False, return_scores: bool = False):
+    """lagkv_score, then top-n_kept + compaction."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    return _compress("kvp_lagkv_compress", SCORER_LAGKV, keys, values, n_kept,
+                     (keys, values, int(n_sink), int(lag_size), int(bool(cross_scoring))), return_indices,
+                     return_scores)
