@@ -17,6 +17,7 @@
  *     kvp_observed_attention_* <- kvpress/presses/observed_attention_press.py (H2O; from Q and K, no eager weights)
  *     kvp_non_causal_attention_* <- kvpress/presses/non_causal_attention_press.py (Compactor's attention half)
  *     kvp_lagkv_*              <- kvpress/presses/lagkv_press.py (lag-relative K / V statistics, from K and V only)
+ *     kvp_cur_*                <- kvpress/presses/cur_press.py (approximate K / V leverage scores, from K and V only)
  *     kvp_scores_compress      <- scorer_press.py:93-100 for an arbitrary score tensor
  *                                 (what wrapper presses / user ScorerPress subclasses need)
  *
@@ -77,7 +78,9 @@ typedef enum kvp_scorer {
     KVP_SCORER_CRITICALKV = 6,
     KVP_SCORER_OBSERVED_ATTENTION = 7,
     KVP_SCORER_NON_CAUSAL_ATTENTION = 8,
-    KVP_SCORER_LAGKV = 9
+    KVP_SCORER_LAGKV = 9,
+    /* 10 is not assigned: kvp_launches_per_compress answers KVP_ERR_BAD_ARGUMENT for it, as for any unknown id */
+    KVP_SCORER_CUR = 11
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -270,6 +273,43 @@ int kvp_lagkv_score(const kvp_problem* p, const void* K, const void* V, int32_t 
 int kvp_lagkv_compress(const kvp_problem* p, const void* K, const void* V, int32_t n_sink, int32_t lag_size,
                        int32_t cross_scoring, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
                        void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+
+/* ---- CURPress (kvpress/presses/cur_press.py, CurDKV, https://arxiv.org/abs/2509.15038) ------------------------------
+ * Reads K and V only. Per row (b, kv head j) with S positions and w = local_window_size, evaluated in fp32 from the
+ * 16-bit inputs and rounded once to the cache dtype:
+ *   - a_k(s) = sum_d k_d^2, or with a projection G [D, r] (float32, row-major, device memory):
+ *     a_k(s) = sum_c (sum_d k_d G_dc)^2. a_v(s) likewise from V. G == NULL and r == 0: no projection.
+ *   - w >= 1: window c covers [cw, (c+1)w) within [0, S), and p_k(s) = a_k(s) / sum_{t in window} a_k(t) with IEEE
+ *     rules (0/0 = NaN). The last, short window sums its real positions only (the reference pads with zeros).
+ *     w == 0: no local approximation, p_k = a_k. p_v likewise.
+ *   - u(s) = p_k, p_v, (p_k + p_v) / 2 or p_k p_v for leverage_type 0, 1, 2, 3 (the reference's "key", "value",
+ *     "kv_avg", "kv_product"). Type 0 does not read V and type 1 does not read K.
+ *   - T = sum_s u(s) over all S positions, the sinks included; score(s) = u(s) / T; then positions s < num_sinks score
+ *     exactly 1 (num_sinks >= S: all of them; 0: none).
+ * NaN and inf propagate as in torch: one NaN u makes T, and so every non-sink score of the row, NaN. A window whose a_k
+ * (or a_v) is all zero is 0/0 = NaN, as in the reference; a zero row inside a non-zero window scores 0. An inf u makes T
+ * inf, its own score NaN and the other scores 0. The evaluation is fp32: where a sum of squares, or the product of two
+ * of them without local approximation, leaves the fp32 range, which only bf16 inputs near the top of their range can
+ * cause, the scores depart from the definition. The shared selection ranks a NaN score above every number, the sinks' 1
+ * included, and breaks ties by position: a NaN row keeps its first non-sink positions, and its sinks only once every
+ * other position is kept. The windows are relative to the first row of the K / V view, so a slice of a cache gets its
+ * own windows. The reference evaluates the chain in the cache dtype
+ * and raises on 16-bit caches with a projection (a 16-bit matrix times a float32 one); here the projection is fp32.
+ * 0 <= local_window_size <= 1024, 0 <= r <= 32, every head_dim the problem validates. G needs only float alignment.
+ * Check order (the first failure is returned): validate the problem -> n_kept == 0 returns KVP_OK (compress) ->
+ * K / V / K_out / V_out null and alignment (compress) -> K, V, scores_out null and K / V alignment (score call) ->
+ * num_sinks < 0, leverage_type outside 0..3, local_window_size < 0, r < 0 or (G == NULL) != (r == 0) give
+ * KVP_ERR_BAD_ARGUMENT -> local_window_size > 1024 or r > 32 gives KVP_ERR_UNSUPPORTED_SHAPE -> workspace.
+ * The workspace holds u as fp32 [B, Hkv, S] and one fp64 partial sum per 256 or more positions, summed in a fixed
+ * order, so scores are bitwise independent of the schedule and of the batch. A compress takes 4 launches (memset, unit
+ * sums, finalize, select+compact) and keeps the n_kept best scores (scores_out nullable). Memory beyond the workspace:
+ * none. */
+int kvp_cur_score(const kvp_problem* p, const void* K, const void* V, int32_t num_sinks, int32_t leverage_type,
+                  int32_t local_window_size, const float* G, int32_t r, void* scores_out, void* workspace,
+                  size_t workspace_bytes, kvp_stream_t stream);
+int kvp_cur_compress(const kvp_problem* p, const void* K, const void* V, int32_t num_sinks, int32_t leverage_type,
+                     int32_t local_window_size, const float* G, int32_t r, void* K_out, void* V_out, int32_t* idx_out,
+                     void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

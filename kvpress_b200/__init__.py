@@ -12,6 +12,7 @@ from kvpress_b200.presses.chunkkv_press import ChunkKVPress
 from kvpress_b200.presses.composed_press import ComposedPress
 from kvpress_b200.presses.compression_ratio_decoding_press import CompressionRatioDecodingPress
 from kvpress_b200.presses.criticalkv_press import CriticalAdaKVPress, CriticalKVPress
+from kvpress_b200.presses.cur_press import CURPress
 from kvpress_b200.presses.decoding_press import DecodingPress
 from kvpress_b200.presses.expected_attention_press import ExpectedAttentionPress
 from kvpress_b200.presses.expected_attention_with_stats import ExpectedAttentionStatsPress
@@ -52,6 +53,7 @@ __all__ = [
     "ObservedAttentionPress",
     "NonCausalAttnPress",
     "LagKVPress",
+    "CURPress",
     "BlockPress",
     "ChunkPress",
     "ChunkKVPress",

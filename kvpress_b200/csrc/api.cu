@@ -11,14 +11,14 @@ namespace kvp {
 
 static thread_local char g_last_cuda_error[256] = "";
 
-// kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention, CriticalKV, ObservedAttention, NonCausalAttention
-// and LagKV score launchers report a shape they have no kernel for as cudaErrorNotSupported.
+// kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention, CriticalKV, ObservedAttention, NonCausalAttention,
+// LagKV and CUR score launchers report a shape they have no kernel for as cudaErrorNotSupported.
 static int status(cudaError_t e, int scorer = KVP_SCORER_GENERIC) {
     if (e == cudaSuccess) return KVP_OK;
     if (e == cudaErrorNotSupported &&
         (scorer == KVP_SCORER_KEYDIFF || scorer == KVP_SCORER_SNAPKV || scorer == KVP_SCORER_EXPECTED_ATTENTION ||
          scorer == KVP_SCORER_CRITICALKV || scorer == KVP_SCORER_OBSERVED_ATTENTION ||
-         scorer == KVP_SCORER_NON_CAUSAL_ATTENTION || scorer == KVP_SCORER_LAGKV))
+         scorer == KVP_SCORER_NON_CAUSAL_ATTENTION || scorer == KVP_SCORER_LAGKV || scorer == KVP_SCORER_CUR))
         return KVP_ERR_UNSUPPORTED_SHAPE;
     snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
     // launch-configuration errors are not sticky: clear them, or the cudaPeekAtLastError() of every later call
@@ -84,6 +84,7 @@ static size_t layout(const Dims& d, int scorer, int window, void* base, Workspac
                        : scorer == KVP_SCORER_CRITICALKV         ? criticalkv_scratch_bytes(d)
                        : scorer == KVP_SCORER_OBSERVED_ATTENTION ? observed_attention_scratch_bytes(d, window)
                        : scorer == KVP_SCORER_NON_CAUSAL_ATTENTION ? non_causal_attention_scratch_bytes(d)
+                       : scorer == KVP_SCORER_CUR                  ? cur_scratch_bytes(d)
                                                                    : 0;
     ws->scorer = c.take<char>(ws->scorer_bytes);
     return c.bytes;
@@ -254,6 +255,7 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         // memset, column sums, pooled partials, mean / std, z, select+compact
         case KVP_SCORER_NON_CAUSAL_ATTENTION: *launches_out = 6; break;
         case KVP_SCORER_LAGKV: *launches_out = 3; break;  // memset, scores + keys, select+compact
+        case KVP_SCORER_CUR: *launches_out = 4; break;  // memset, unit sums, finalize, select+compact
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -565,6 +567,43 @@ int kvp_lagkv_compress(const kvp_problem* p, const void* K, const void* V, int32
     };
     return run(Kind::compress, p, KVP_SCORER_LAGKV, 0, {K, V, K_out, V_out, idx_out, nullptr}, operands, score,
                workspace, workspace_bytes, stream);
+}
+
+// ---- CUR -----------------------------------------------------------------------------------------
+// The operand checks both entry points share, after their null / alignment checks.
+static int cur_args(int32_t num_sinks, int32_t leverage_type, int32_t window, const float* G, int32_t r) {
+    if (num_sinks < 0 || leverage_type < 0 || leverage_type > 3 || window < 0 || r < 0 || (G == nullptr) != (r == 0))
+        return KVP_ERR_BAD_ARGUMENT;
+    return (window > kCurWindowMax || r > kCurRankMax) ? KVP_ERR_UNSUPPORTED_SHAPE : KVP_OK;
+}
+
+static auto cur_stage(const kvp_problem* p, const void* K, const void* V, int32_t num_sinks, int32_t leverage_type,
+                      int32_t window, const float* G, int32_t r, void* scores_out) {
+    return [=](const Call& c) {
+        return launch_cur_score(c.d, p->dtype, K, V, num_sinks, leverage_type, window, G, r, c.ws, scores_out, c.st);
+    };
+}
+
+int kvp_cur_score(const kvp_problem* p, const void* K, const void* V, int32_t num_sinks, int32_t leverage_type,
+                  int32_t local_window_size, const float* G, int32_t r, void* scores_out, void* workspace,
+                  size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims&) -> int {
+        if (!K || !V || !scores_out) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(K) || !aligned16(V)) return KVP_ERR_BAD_STRIDE;
+        return cur_args(num_sinks, leverage_type, local_window_size, G, r);
+    };
+    return run(Kind::score, p, KVP_SCORER_CUR, 0, {}, operands,
+               cur_stage(p, K, V, num_sinks, leverage_type, local_window_size, G, r, scores_out), workspace,
+               workspace_bytes, stream);
+}
+
+int kvp_cur_compress(const kvp_problem* p, const void* K, const void* V, int32_t num_sinks, int32_t leverage_type,
+                     int32_t local_window_size, const float* G, int32_t r, void* K_out, void* V_out, int32_t* idx_out,
+                     void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims&) { return cur_args(num_sinks, leverage_type, local_window_size, G, r); };
+    return run(Kind::compress, p, KVP_SCORER_CUR, 0, {K, V, K_out, V_out, idx_out, nullptr}, operands,
+               cur_stage(p, K, V, num_sinks, leverage_type, local_window_size, G, r, scores_out), workspace,
+               workspace_bytes, stream);
 }
 
 // ---- generic scores ------------------------------------------------------------------------------

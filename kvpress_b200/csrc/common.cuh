@@ -18,6 +18,8 @@ constexpr uint16_t kForcedKey = 0xFFFFu;  // ordered key of a forced-keep positi
 constexpr int kFinalizeTiles = 1;          // 256-position tiles per CTA of the finalize kernels (1: >5 waves at 128k, no tail)
 constexpr int kScoreChunkGeneric = 256;   // positions per CTA of the plain streaming score kernels
 constexpr int kLagMax = 1024;              // largest LagKV lag_size (partition length) the kernel scores
+constexpr int kCurWindowMax = 1024;        // largest CUR local_window_size the kernel scores
+constexpr int kCurRankMax = 32;            // most columns of a CUR projection G the kernel scores
 // counters[] layout: [0] ticket, [1, 1+R) refine done, [1+R, 1+2R) row ready, then the slot below:
 // order-preserving uint image of the largest valid score (for the reference's max+1 sentinel);
 // [2+2R, 2+3R) score items done per row (fused Knorm kernel)
@@ -45,7 +47,7 @@ struct Workspace {
                          // zero = row not scanned yet
     int R;
     void* scorer;        // scorer-specific scratch (SnapKV / ExpectedAttention / KeyDiff / CriticalKV /
-                         // ObservedAttention / NonCausalAttention; LagKV needs none)
+                         // ObservedAttention / NonCausalAttention / CUR; LagKV needs none)
     size_t scorer_bytes;
     int S_pad;
     int n_tiles;
@@ -359,5 +361,9 @@ cudaError_t launch_non_causal_attention_score(const Dims& d, int dtype, const vo
                                               int chunk_size, const Workspace& ws, void* scores_out, cudaStream_t st);
 cudaError_t launch_lagkv_score(const Dims& d, int dtype, const void* K, const void* V, int n_sink, int lag_size,
                                int cross, const Workspace& ws, void* scores_out, bool want_keys, cudaStream_t st);
+size_t cur_scratch_bytes(const Dims& d);
+cudaError_t launch_cur_score(const Dims& d, int dtype, const void* K, const void* V, int num_sinks, int leverage_type,
+                             int window, const float* G, int r, const Workspace& ws, void* scores_out,
+                             cudaStream_t st);
 
 }  // namespace kvp

@@ -117,8 +117,8 @@ __device__ __forceinline__ void knorm_score_chunk(const T* __restrict__ K, Strid
 // (this is warp `wi` of them) in batches of U loads per lane; a sub-warp of LPR lanes covers a 2*D-byte row. Loads are
 // L2-evict-first: the rows are read exactly once. Each row's sum of squares is formed as in knorm_score_chunk (per lane
 // an even/odd FMA pair over its 8 elements, then the lane tree over xor LPR/2 .. 1 of RowSums), so the norms do not
-// depend on U, on the span or on how many warps share it.
-template <typename T, int LPR, int U>
+// depend on U, on the span or on how many warps share it. kSqrt = false writes the sum of squares itself (CUR).
+template <typename T, int LPR, int U, bool kSqrt = true>
 __device__ __forceinline__ void row_norm_span(const T* __restrict__ X, Strides3 xs, int b, int h, int s_begin,
                                               int s_end, int D, float* __restrict__ out, int wi, int n_warps) {
     const int lane = threadIdx.x & 31;
@@ -156,7 +156,7 @@ __device__ __forceinline__ void row_norm_span(const T* __restrict__ X, Strides3 
 #pragma unroll
             for (int i = 0; i < RS::kSlots; ++i) {
                 const int s = s0 + (RS::row_of(sub) + i) * RPW + rsel;
-                if (s < s_end) out[s] = sqrtf(ssu[i]);
+                if (s < s_end) out[s] = kSqrt ? sqrtf(ssu[i]) : ssu[i];
             }
         }
     }

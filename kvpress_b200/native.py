@@ -20,7 +20,11 @@ _LIB_PATH = Path(__file__).resolve().parent / _LIB_NAME
 
 (SCORER_GENERIC, SCORER_KNORM, SCORER_STREAMING, SCORER_SNAPKV, SCORER_EXPECTED_ATTENTION, SCORER_KEYDIFF,
  SCORER_CRITICALKV, SCORER_OBSERVED_ATTENTION, SCORER_NON_CAUSAL_ATTENTION, SCORER_LAGKV) = range(10)
+SCORER_CUR = 11  # KVP_SCORER_CUR; id 10 is not assigned
 LAG_MAX = 1024  # the largest lag_size the LagKV kernel scores (kLagMax in csrc/common.cuh)
+CUR_WINDOW_MAX = 1024  # the largest local_window_size the CUR kernel scores (kCurWindowMax in csrc/common.cuh)
+CUR_RANK_MAX = 32  # the most projection columns the CUR kernel scores (kCurRankMax)
+CUR_LEVERAGE_TYPES = ("key", "value", "kv_avg", "kv_product")  # leverage_type 0 ... 3 of kvp_cur_score
 _DTYPES = {torch.bfloat16: 0, torch.float16: 1}
 
 
@@ -86,6 +90,8 @@ SIGNATURES = {
     "kvp_non_causal_attention_compress": (ctypes.c_int, [_PP, _P, _P, _P, _I, _P, _P, _P, _P, _P, _SZ, _P]),
     "kvp_lagkv_score": (ctypes.c_int, [_PP, _P, _P, _I, _I, _I, _P, _P, _SZ, _P]),
     "kvp_lagkv_compress": (ctypes.c_int, [_PP, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_cur_score": (ctypes.c_int, [_PP, _P, _P, _I, _I, _I, _P, _I, _P, _P, _SZ, _P]),
+    "kvp_cur_compress": (ctypes.c_int, [_PP, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -654,3 +660,39 @@ def lagkv_compress(keys, values, n_sink: int, lag_size: int, cross_scoring: bool
     return _compress("kvp_lagkv_compress", SCORER_LAGKV, keys, values, n_kept,
                      (keys, values, int(n_sink), int(lag_size), int(bool(cross_scoring))), return_indices,
                      return_scores)
+
+
+# --------------------------------------------------------------------------------------------------
+# CUR
+# --------------------------------------------------------------------------------------------------
+def _cur_inputs(keys, values, num_sinks: int, leverage_type: str, local_window_size: int, G) -> tuple:
+    """The arguments of kvp_cur_score / kvp_cur_compress between the kvp_problem and the outputs."""
+    if leverage_type not in CUR_LEVERAGE_TYPES:
+        raise ValueError("Unknown leverage type: choose from 'kv_avg', 'key', 'value' or 'kv_product'")
+    r = 0
+    if G is not None:
+        if G.dtype != torch.float32 or G.dim() != 2 or G.shape[0] != keys.shape[-1] or G.device != keys.device:
+            raise RuntimeError(f"expected a float32 projection [head_dim, r] on {keys.device}, got "
+                               f"{G.dtype} {tuple(G.shape)} on {G.device}")
+        G, r = G.contiguous(), G.shape[1]
+    return keys, values, int(num_sinks), CUR_LEVERAGE_TYPES.index(leverage_type), int(local_window_size), G, int(r)
+
+
+def cur_score(keys, values, num_sinks: int, leverage_type: str, local_window_size: int, G=None) -> torch.Tensor:
+    """CURPress scores [B, Hkv, S] (include/kvpress_b200.h, kvp_cur_score): the squared norms of the keys and of the
+    values (of their projections by G [D, r], float32, when given), each divided by its sum over its window of
+    local_window_size positions (0: not divided), combined by leverage_type, divided by the row's sum; the first
+    num_sinks positions score 1."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    inputs = _cur_inputs(keys, values, num_sinks, leverage_type, local_window_size, G)
+    return _score("kvp_cur_score", SCORER_CUR, keys, make_problem(keys, values, 0), *inputs)
+
+
+def cur_compress(keys, values, num_sinks: int, leverage_type: str, local_window_size: int, G, n_kept: int,
+                 return_indices: bool = False, return_scores: bool = False):
+    """cur_score, then top-n_kept + compaction."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    inputs = _cur_inputs(keys, values, num_sinks, leverage_type, local_window_size, G)
+    return _compress("kvp_cur_compress", SCORER_CUR, keys, values, n_kept, inputs, return_indices, return_scores)
