@@ -10,7 +10,8 @@ import torch
 from oracle import press_oracle as O
 
 
-def _select(scores, keys, values, n_kept, want_idx=True, want_scores=False):
+def select_gather(scores, keys, values, n_kept, want_idx=True, want_scores=False):
+    """The shared selection and compaction of a compress call: (K', V', idx or None, scores or None)."""
     idx = O.select_lowest_index_ties(scores, n_kept)
     k_out, v_out = O.gather_rows(keys, idx), O.gather_rows(values, idx)
     return k_out, v_out, (idx.to(torch.int32) if want_idx else None), (scores if want_scores else None)
@@ -21,7 +22,7 @@ def knorm_score(keys):
 
 
 def knorm_compress(keys, values, n_kept, return_indices=False, return_scores=False):
-    return _select(O.knorm_scores(keys), keys, values, n_kept, return_indices, return_scores)
+    return select_gather(O.knorm_scores(keys), keys, values, n_kept, return_indices, return_scores)
 
 
 def streaming_score(keys, n_kept, n_sink):
@@ -42,7 +43,7 @@ def snapkv_score(keys, q_window, window, kernel_size):
 
 
 def snapkv_compress(keys, values, q_window, window, kernel_size, n_kept, return_indices=False, return_scores=False):
-    return _select(O.snapkv_scores(q_window, keys, window, kernel_size), keys, values, n_kept, return_indices,
+    return select_gather(O.snapkv_scores(q_window, keys, window, kernel_size), keys, values, n_kept, return_indices,
                    return_scores)
 
 
@@ -53,11 +54,11 @@ def expected_attention_score(keys, values, mu, cov, epsilon, n_sink, use_vnorm):
 def expected_attention_compress(keys, values, mu, cov, epsilon, n_sink, use_vnorm, n_kept, return_indices=False,
                                 return_scores=False):
     scores = O.expected_attention_scores(keys, values, mu, cov, epsilon, n_sink, use_vnorm)
-    return _select(scores, keys, values, n_kept, return_indices, return_scores)
+    return select_gather(scores, keys, values, n_kept, return_indices, return_scores)
 
 
 def scores_compress(scores, keys, values, n_kept, return_indices=False):
-    k_out, v_out, idx, _ = _select(scores, keys, values, n_kept, return_indices, False)
+    k_out, v_out, idx, _ = select_gather(scores, keys, values, n_kept, return_indices, False)
     return k_out, v_out, idx
 
 
@@ -72,7 +73,7 @@ def keydiff_score(keys):
 
 
 def keydiff_compress(keys, values, n_kept, return_indices=False, return_scores=False):
-    return _select(O.keydiff_scores(keys), keys, values, n_kept, return_indices, return_scores)
+    return select_gather(O.keydiff_scores(keys), keys, values, n_kept, return_indices, return_scores)
 
 
 def scores_select(scores, n_kept):

@@ -5,6 +5,7 @@ torch: they run on CPU or CUDA tensors."""
 import torch
 
 from oracle import press_oracle as O
+from tests.cpu_backend import select_gather
 
 
 def criticalkv_scores(base: torch.Tensor, values: torch.Tensor, wo: torch.Tensor, epsilon: float,
@@ -34,9 +35,7 @@ def criticalkv_score(base_scores, values, wo, epsilon, n_first):
 def criticalkv_compress(base_scores, keys, values, wo, epsilon, n_first, n_kept, return_indices=False,
                         return_scores=False):
     scores = criticalkv_score(base_scores, values, wo, epsilon, n_first)
-    idx = O.select_lowest_index_ties(scores, n_kept)
-    return (O.gather_rows(keys, idx), O.gather_rows(values, idx), idx.to(torch.int32) if return_indices else None,
-            scores if return_scores else None)
+    return select_gather(scores, keys, values, n_kept, return_indices, return_scores)
 
 
 def install(monkeypatch):

@@ -3,7 +3,7 @@ by the CUR tests next to tests/cpu_backend.py: the same contract (float64 evalua
 lowest-position ties). Pure torch: they run on CPU or CUDA tensors."""
 import torch
 
-from oracle import press_oracle as O
+from tests.cpu_backend import select_gather
 
 LEVERAGE_TYPES = ("key", "value", "kv_avg", "kv_product")
 
@@ -52,9 +52,7 @@ def cur_score(keys, values, num_sinks, leverage_type, local_window_size, G=None)
 def cur_compress(keys, values, num_sinks, leverage_type, local_window_size, G, n_kept, return_indices=False,
                  return_scores=False):
     scores = cur_score(keys, values, num_sinks, leverage_type, local_window_size, G)
-    idx = O.select_lowest_index_ties(scores, n_kept)
-    return (O.gather_rows(keys, idx), O.gather_rows(values, idx), idx.to(torch.int32) if return_indices else None,
-            scores if return_scores else None)
+    return select_gather(scores, keys, values, n_kept, return_indices, return_scores)
 
 
 def install(monkeypatch):

@@ -3,7 +3,7 @@ used by the LagKV tests next to tests/cpu_backend.py: the same contract (float64
 positions, lowest-position ties). Pure torch: they run on CPU or CUDA tensors."""
 import torch
 
-from oracle import press_oracle as O
+from tests.cpu_backend import select_gather
 
 
 def is_short(S: int, n_sink: int, lag_size: int) -> bool:
@@ -59,9 +59,7 @@ def lagkv_score(keys, values, n_sink, lag_size, cross_scoring):
 
 def lagkv_compress(keys, values, n_sink, lag_size, cross_scoring, n_kept, return_indices=False, return_scores=False):
     scores = lagkv_score(keys, values, n_sink, lag_size, cross_scoring)
-    idx = O.select_lowest_index_ties(scores, n_kept)
-    return (O.gather_rows(keys, idx), O.gather_rows(values, idx), idx.to(torch.int32) if return_indices else None,
-            scores if return_scores else None)
+    return select_gather(scores, keys, values, n_kept, return_indices, return_scores)
 
 
 def install(monkeypatch):

@@ -5,7 +5,7 @@ Pure torch: they run on CPU or CUDA tensors."""
 import torch
 import torch.nn.functional as F
 
-from oracle import press_oracle as O
+from tests.cpu_backend import select_gather
 
 
 def non_causal_attention_parts64(keys: torch.Tensor, values: torch.Tensor, q: torch.Tensor, chunk_size: int,
@@ -54,9 +54,7 @@ def non_causal_attention_score(keys, values, q, chunk_size):
 
 def non_causal_attention_compress(keys, values, q, chunk_size, n_kept, return_indices=False, return_scores=False):
     scores = non_causal_attention_score(keys, values, q, chunk_size)
-    idx = O.select_lowest_index_ties(scores, n_kept)
-    return (O.gather_rows(keys, idx), O.gather_rows(values, idx), idx.to(torch.int32) if return_indices else None,
-            scores if return_scores else None)
+    return select_gather(scores, keys, values, n_kept, return_indices, return_scores)
 
 
 def install(monkeypatch):

@@ -4,7 +4,7 @@ tests/cpu_backend.py: the same contract (float64 evaluation rounded once, the di
 dtype, ascending positions, lowest-position ties). Pure torch: they run on CPU or CUDA tensors."""
 import torch
 
-from oracle import press_oracle as O
+from tests.cpu_backend import select_gather
 
 
 def observed_attention_scores64(keys: torch.Tensor, q: torch.Tensor, scaling: float, block: int = 4096) -> torch.Tensor:
@@ -40,9 +40,7 @@ def observed_attention_score(keys, q, scaling):
 
 def observed_attention_compress(keys, values, q, scaling, n_kept, return_indices=False, return_scores=False):
     scores = observed_attention_scores(keys, q, scaling)
-    idx = O.select_lowest_index_ties(scores, n_kept)
-    return (O.gather_rows(keys, idx), O.gather_rows(values, idx), idx.to(torch.int32) if return_indices else None,
-            scores if return_scores else None)
+    return select_gather(scores, keys, values, n_kept, return_indices, return_scores)
 
 
 def install(monkeypatch):

@@ -13,20 +13,17 @@ validation". To re-record from the library as built:  KVP_RECORD_ABI_STATUS=1 py
 """
 import ctypes
 import hashlib
-import itertools
 import json
 import os
-import subprocess
-import sys
 from pathlib import Path
 
-ROOT = Path(__file__).resolve().parent.parent
-STORE = ROOT / "tests" / "golden" / "abi_status_matrix.json"
+from tests.abi_cases import FIELDS, GOOD, ODD16 as ODD, arg, case_matrix, in_child, load_native, problem, \
+    workspace_bytes
+
+STORE = Path(__file__).resolve().parent / "golden" / "abi_status_matrix.json"
 RECORD = os.environ.get("KVP_RECORD_ABI_STATUS") == "1"
 
-GOOD, ODD, BIG = 0x10000, 0x1000C, 1 << 40  # aligned / misaligned pointer; more workspace than any case needs
-FIELDS = dict(B=1, Hkv=2, Hq=4, S=1000, D=128, n_kept=500, dtype=0)
-STRIDES = (256000, 128000, 128)
+BIG = 1 << 40  # more workspace than any case needs
 BAD_STRIDES = {"s100": (256000, 128000, 100), "s120": (256000, 128000, 120), "b-8": (-8, 128000, 128)}
 PROBLEM_CHANGES = {  # slot -> {label: value}
     "p": {"null": None},
@@ -81,34 +78,18 @@ SWEEP += [(1, 1, 1, 131072, 128), (1, 1, 1, 131073, 128), (2, 8, 1, 8192, 128), 
           (2, 1, 1, 131072, 64), (2, 1, 1, 131073, 64)]
 
 
-def _problem(native, changes=None, **fields):
-    changes = changes or {}
-    p = native.KvpProblem()
-    for k, v in {**FIELDS, **fields, **{k: v for k, v in changes.items() if k in FIELDS}}.items():
-        setattr(p, k, v)
-    p.k_stride = (ctypes.c_int64 * 3)(*changes.get("k_stride", STRIDES))
-    p.v_stride = (ctypes.c_int64 * 3)(*changes.get("v_stride", STRIDES))
-    return p
-
-
 def _call(native, lib, name, changes):
     """`name` with the valid arguments and `changes` ({slot: value}): its status, and for the two query calls the value
     written through the output pointer."""
     scorer, slots = ENTRIES[name]
-    args, out = [None if changes.get("p", 0) is None else ctypes.byref(_problem(native, changes))], None
+    args, out = [None if changes.get("p", 0) is None else ctypes.byref(problem(native, changes, FIELDS))], None
     for slot in slots.split():
         v = changes.get(slot, ARGS[slot][0] if slot in ARGS else GOOD)
         if v == "out":
             out = (ctypes.c_size_t if name == "kvp_workspace_bytes" else ctypes.c_int)(0)
             v = ctypes.byref(out)
-        elif v == "sstride":
-            v = (ctypes.c_int64 * 2)(2000, 1000)
-        elif v == "short":  # one byte less than the library asks for the valid problem
-            need = ctypes.c_size_t(0)
-            assert lib.kvp_workspace_bytes(ctypes.byref(_problem(native)), scorer, ctypes.byref(need)) == 0
-            v = need.value - 1
-        elif slot in ("idx", "inv_freq") and v is not None:
-            v = ctypes.cast(ctypes.c_void_p(v), ctypes.POINTER(ctypes.c_int32 if slot == "idx" else ctypes.c_float))
+        else:  # "short": one byte less than the library asks for the valid problem
+            v = arg(slot, v, lambda: workspace_bytes(lib, problem(native, {}, FIELDS), scorer))
         args.append(v)
     rc = getattr(lib, name)(*args)
     return str(-rc) if out is None else f"{-rc}:{out.value}"
@@ -117,28 +98,15 @@ def _call(native, lib, name, changes):
 def matrix() -> dict:
     """Every case, per entry point: a digest of the case names and the results in case order. Run only in a process
     that sees no GPU."""
-    import importlib.util
-
-    import torch
-
-    assert torch.cuda.device_count() == 0, "the status matrix passes fake device pointers: it must not see a GPU"
-    # the binding alone: importing the package would also import the presses and transformers, for nothing
-    spec = importlib.util.spec_from_file_location("kvp_native", ROOT / "kvpress_b200" / "native.py")
-    native = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(native)
-    lib = native.load()
+    native, lib = load_native()
     got = {}
     for name, (_, slots) in ENTRIES.items():
-        changes = {**PROBLEM_CHANGES, **{s: ARGS[s][1] if s in ARGS else PTR for s in slots.split()}}
-        singles = [(s, label, v) for s, c in changes.items() for label, v in c.items()]
-        cases = {"valid": {}, **{f"{s}={label}": {s: v} for s, label, v in singles}}
-        cases.update({f"{s1}={l1},{s2}={l2}": {s1: v1, s2: v2}
-                      for (s1, l1, v1), (s2, l2, v2) in itertools.combinations(singles, 2) if s1 != s2})
+        cases = case_matrix({**PROBLEM_CHANGES, **{s: ARGS[s][1] if s in ARGS else PTR for s in slots.split()}})
         results = [_call(native, lib, name, c) for c in cases.values()]
         got[name] = {"cases": hashlib.sha256("|".join(cases).encode()).hexdigest()[:16], "names": list(cases),
                      "results": "".join(results) if all(len(r) == 1 for r in results) else " ".join(results)}
     for B, H, G, S, D in SWEEP:
-        p = ctypes.byref(_problem(native, B=B, Hkv=H, Hq=G * H, S=S, D=D, n_kept=S // 2))
+        p = ctypes.byref(problem(native, {}, dict(FIELDS, B=B, Hkv=H, Hq=G * H, S=S, D=D, n_kept=S // 2)))
         row = []
         for scorer in range(6):
             n, launches = ctypes.c_size_t(0), ctypes.c_int(0)
@@ -150,13 +118,7 @@ def matrix() -> dict:
 
 
 def test_every_status_workspace_size_and_launch_count_matches_the_recording():
-    env = {k: v for k, v in os.environ.items() if not k.startswith("KVP_")}  # the library's knobs at their defaults
-    env["CUDA_VISIBLE_DEVICES"] = ""
-    code = "import json, tests.test_abi_status_matrix as m; print(json.dumps(m.matrix()))"
-    r = subprocess.run([sys.executable, *(["-s"] if sys.flags.no_user_site else []), "-c", code], cwd=ROOT, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    got = json.loads(r.stdout.strip().splitlines()[-1])
+    got = in_child(f"{__name__}:matrix")  # the library's knobs at their defaults
     names = {k: v.pop("names") for k, v in got.items() if "names" in v}
     if RECORD:
         STORE.write_text("{\n" + ",\n".join(f"{json.dumps(k)}: {json.dumps(v)}" for k, v in got.items()) + "\n}\n")

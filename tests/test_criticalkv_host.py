@@ -11,11 +11,6 @@ tests/golden/criticalkv_reference.npz. To re-record it from a checkout of the re
 oracle/build_ref.py):  KVP_RECORD_CRITICALKV=1 python -m pytest tests/test_criticalkv_host.py
 """
 import ctypes
-import itertools
-import json
-import os
-import subprocess
-import sys
 from pathlib import Path
 
 import numpy as np
@@ -25,157 +20,67 @@ from transformers import DynamicCache
 
 from kvpress_b200 import (CriticalAdaKVPress, CriticalKVPress, DecodingPress, ExpectedAttentionPress, KnormPress,
                           PrefillDecodingPress, SnapKVPress, native)
-from tests import cpu_backend, criticalkv_backend
-from tests.test_native_marshalling import _kv, rec  # noqa: F401  (fixture)
-from tests.test_reference_differential import _import_reference, _rows_signature, close
-from tests.tiny_models import tiny_llama, tiny_qwen3
+from tests import abi_cases, cpu_backend, criticalkv_backend
+from tests.abi_cases import GOOD, ODD16
+from tests.support import TO_32BIT, close, kv, rec, reference_store, rows_signature  # noqa: F401  (rec: fixture)
+from tests.tiny_models import distinct_ids, tiny_model
 
-ROOT = Path(__file__).resolve().parent.parent
-STORE = ROOT / "tests" / "golden" / "criticalkv_reference.npz"
-RECORD = os.environ.get("KVP_RECORD_CRITICALKV") == "1"
+STORE = Path(__file__).resolve().parent / "golden" / "criticalkv_reference.npz"
 
 # --------------------------------------------------------------------------------------------------
 # C ABI statuses
 # --------------------------------------------------------------------------------------------------
-GOOD, ODD16, ODD2 = 0x10000, 0x1000C, 0x10001  # aligned; 4-byte but not 16-byte aligned; odd
-FIELDS = dict(B=1, Hkv=2, Hq=4, S=1000, D=128, n_kept=500, dtype=0)  # Hq * D = 512
-STRIDES = (256000, 128000, 128)
-VALID = dict(K=GOOD, V=GOOD, base=GOOD, sstride="sstride", wo=GOOD, hidden=4096, wo_stride=512, eps=1e-4,
-             n_first=100, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD, ws=GOOD, ws_bytes=1 << 40, stream=0)
-SLOTS = {
-    "kvp_criticalkv_score": "V base sstride wo hidden wo_stride eps n_first scores ws ws_bytes stream",
-    "kvp_criticalkv_compress": "K V base sstride wo hidden wo_stride eps n_first K_out V_out idx scores ws ws_bytes "
-                               "stream",
-}
-CHANGES = {  # slot -> {label: value}
-    "p": {"null": None},
-    "dtype": {"3": 3},
-    "S": {"0": 0},
-    "D": {"12": 12, "64": 64},
-    "Hq": {"5": 5},
-    "n_kept": {"-1": -1, "0": 0, "1000": 1000},
-    "v_stride": {"s100": (256000, 128000, 100)},
-    "K": {"null": None, "odd": ODD16},
-    "V": {"null": None, "odd": ODD16},
-    "base": {"null": None, "odd": ODD2, "4-aligned": ODD16},
-    "sstride": {"null": None},
-    "wo": {"null": None, "odd": ODD16},
-    "hidden": {"0": 0, "-1": -1, "1": 1},
-    "wo_stride": {"100": 100, "504": 504, "520": 520},
-    "n_first": {"-1": -1, "0": 0, "500": 500, "501": 501, "1000": 1000, "1001": 1001},
-    "K_out": {"null": None},
-    "V_out": {"null": None, "odd": ODD16},
-    "idx": {"null": None},
-    "scores": {"null": None},
-    "ws": {"null": None, "odd": ODD16},
-    "ws_bytes": {"short": "short"},
-}
-PROBLEM = ("dtype", "S", "D", "Hq", "n_kept", "v_stride")
+ODD2 = 0x10001
 
 
-def expected(name: str, c: dict) -> int:
-    """The documented check order: validate -> n_kept == 0 short cut (compress) -> K / V / outputs (compress) ->
-    null / alignment of the operands -> hidden -> wo_stride -> n_first -> workspace."""
-    f = {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}
-    a = {**VALID, **{k: v for k, v in c.items() if k not in FIELDS}}
-    compress = name.endswith("compress")
-    if c.get("p", 0) is None:
-        return -1
-    if f["dtype"] not in (0, 1):
-        return -3
-    if f["S"] <= 0 or f["D"] % 8 or f["Hq"] % FIELDS["Hkv"]:
-        return -2
-    if not 0 <= f["n_kept"] <= f["S"]:
-        return -7
-    if "v_stride" in c:
-        return -4
-    if compress:
-        if f["n_kept"] == 0:
-            return 0
-        io = [a["K"], a["V"], a["K_out"], a["V_out"]]
-        if None in io:
-            return -1
-        if any(x % 16 for x in io):
-            return -4
-        nulls, aligned = [a["base"], a["sstride"], a["wo"]], [a["wo"]]
-    else:
-        nulls, aligned = [a["V"], a["base"], a["sstride"], a["wo"], a["scores"]], [a["V"], a["wo"]]
-    if None in nulls:
-        return -1
-    if any(x % 16 for x in aligned) or a["base"] % 2:
+def _checks(f, a, compress):
+    """base_scores 2-byte aligned -> hidden -> wo_stride -> n_first."""
+    if a["base"] % 2:
         return -4
     if a["hidden"] <= 0:
         return -7
     if a["wo_stride"] % 8 or a["wo_stride"] < f["Hq"] * f["D"]:
         return -4
-    if not 0 <= a["n_first"] <= (f["n_kept"] if compress else f["S"]):
-        return -7
-    if a["ws"] is None:
-        return -1
-    if a["ws"] % 16:
-        return -4
-    return -5 if a["ws_bytes"] == "short" else -6
+    return -7 if not 0 <= a["n_first"] <= (f["n_kept"] if compress else f["S"]) else 0
 
 
-def _cases(name: str) -> dict:
-    slots = ["p", *PROBLEM, *SLOTS[name].split()]
-    singles = [(s, label, v) for s in slots for label, v in CHANGES.get(s, {}).items()]
-    cases = {"valid": {}, **{f"{s}={label}": {s: v} for s, label, v in singles}}
-    cases.update({f"{s1}={l1},{s2}={l2}": {s1: v1, s2: v2}
-                  for (s1, l1, v1), (s2, l2, v2) in itertools.combinations(singles, 2) if s1 != s2})
-    return cases
-
-
-def statuses() -> dict:
-    """Every case's status. Run only in a process that sees no GPU."""
-    import importlib.util
-
-    assert torch.cuda.device_count() == 0, "the status cases pass fake device pointers: they must not see a GPU"
-    spec = importlib.util.spec_from_file_location("kvp_native", ROOT / "kvpress_b200" / "native.py")
-    nat = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(nat)
-    lib = nat.load()
-
-    def problem(c):
-        p = nat.KvpProblem()
-        for k, v in {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}.items():
-            setattr(p, k, v)
-        p.k_stride = (ctypes.c_int64 * 3)(*STRIDES)
-        p.v_stride = (ctypes.c_int64 * 3)(*c.get("v_stride", STRIDES))
-        return p
-
-    out = {}
-    for name in SLOTS:
-        for label, c in _cases(name).items():
-            args = [None if c.get("p", 0) is None else ctypes.byref(problem(c))]
-            for slot in SLOTS[name].split():
-                v = c.get(slot, VALID[slot])
-                if v == "sstride":
-                    v = (ctypes.c_int64 * 2)(2000, 1000)
-                elif v == "short":
-                    need = ctypes.c_size_t(0)
-                    assert lib.kvp_workspace_bytes(ctypes.byref(problem({})), native.SCORER_CRITICALKV,
-                                                   ctypes.byref(need)) == 0
-                    v = need.value - 1
-                elif slot == "idx" and v is not None:
-                    v = ctypes.cast(ctypes.c_void_p(v), ctypes.POINTER(ctypes.c_int32))
-                args.append(v)
-            out[f"{name}({label})"] = getattr(lib, name)(*args)
-    return out
+ABI = abi_cases.Spec(
+    scorer=native.SCORER_CRITICALKV,  # Hq * D = 512
+    slots={"kvp_criticalkv_score": "V base sstride wo hidden wo_stride eps n_first scores ws ws_bytes stream",
+           "kvp_criticalkv_compress": "K V base sstride wo hidden wo_stride eps n_first K_out V_out idx scores ws "
+                                      "ws_bytes stream"},
+    valid=dict(K=GOOD, V=GOOD, base=GOOD, sstride="sstride", wo=GOOD, hidden=4096, wo_stride=512, eps=1e-4,
+               n_first=100, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD, ws=GOOD, ws_bytes="enough", stream=0),
+    changes={
+        "p": {"null": None},
+        "dtype": {"3": 3},
+        "S": {"0": 0},
+        "D": {"12": 12, "64": 64},
+        "Hq": {"5": 5},
+        "n_kept": {"-1": -1, "0": 0, "1000": 1000},
+        "v_stride": {"s100": (256000, 128000, 100)},
+        "K": {"null": None, "odd": ODD16},
+        "V": {"null": None, "odd": ODD16},
+        "base": {"null": None, "odd": ODD2, "4-aligned": ODD16},
+        "sstride": {"null": None},
+        "wo": {"null": None, "odd": ODD16},
+        "hidden": {"0": 0, "-1": -1, "1": 1},
+        "wo_stride": {"100": 100, "504": 504, "520": 520},
+        "n_first": {"-1": -1, "0": 0, "500": 500, "501": 501, "1000": 1000, "1001": 1001},
+        "K_out": {"null": None},
+        "V_out": {"null": None, "odd": ODD16},
+        "idx": {"null": None},
+        "scores": {"null": None},
+        "ws": {"null": None, "odd": ODD16},
+        "ws_bytes": {"short": "short"},
+    },
+    operands={"score": (["V", "base", "sstride", "wo", "scores"], ["V", "wo"]),
+              "compress": (["base", "sstride", "wo"], ["wo"])},
+    checks=_checks)
 
 
 def test_every_status_of_the_criticalkv_entry_points_follows_the_check_order():
-    env = {k: v for k, v in os.environ.items() if not k.startswith("KVP_")}
-    env["CUDA_VISIBLE_DEVICES"] = ""
-    code = "import json, tests.test_criticalkv_host as m; print(json.dumps(m.statuses()))"
-    r = subprocess.run([sys.executable, *(["-s"] if sys.flags.no_user_site else []), "-c", code], cwd=ROOT, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    got = json.loads(r.stdout.strip().splitlines()[-1])
-    want = {f"{name}({label})": expected(name, c) for name in SLOTS for label, c in _cases(name).items()}
-    assert sorted(got) == sorted(want) and len(got) > 1000
-    diffs = [f"{k}: {got[k]} != {want[k]}" for k in want if got[k] != want[k]]
-    assert not diffs, f"{len(diffs)} differences, first ones:\n" + "\n".join(diffs[:30])
+    abi_cases.assert_statuses(__name__, 1000)
 
 
 def test_workspace_and_launch_count_of_the_new_scorer_id():
@@ -203,7 +108,7 @@ def test_criticalkv_wrappers_pass_their_full_argument_list(rec, monkeypatch):  #
 
     monkeypatch.setattr(native, "_workspace", spy)
     P = lambda t: t.data_ptr()  # noqa: E731
-    k, v = _kv(B=2, H=2, S=64, D=64)
+    k, v = kv(B=2, H=2, S=64, D=64)
     wo = torch.randn(96, 8 * 64 + 16).to(torch.bfloat16)[:, 8:8 + 8 * 64]  # sliced rows: consumed in place
     base = torch.rand(2, 2, 64).to(torch.bfloat16)
 
@@ -233,39 +138,7 @@ def test_criticalkv_wrappers_pass_their_full_argument_list(rec, monkeypatch):  #
 # --------------------------------------------------------------------------------------------------
 # presses against the unmodified reference (CPU stand-ins)
 # --------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def ref():
-    stored = {} if RECORD or not STORE.exists() else dict(np.load(STORE))
-    recorded = {}
-
-    def result(key: str, compute) -> dict:
-        if RECORD:
-            out = {k: np.asarray(x.detach().numpy() if torch.is_tensor(x) else x)
-                   for k, x in compute(_import_reference()).items()}
-            out = {k: x.astype(np.float32) if x.dtype == np.float64 else x.astype(np.int32) if x.dtype == np.int64
-                   else x for k, x in out.items()}
-            recorded.update({f"{key}|{k}": x for k, x in out.items()})
-            return out
-        out = {k.split("|", 1)[1]: x for k, x in stored.items() if k.split("|", 1)[0] == key}
-        assert out, f"no stored reference result for {key}"
-        return out
-
-    yield result
-    if RECORD:
-        np.savez_compressed(STORE, **recorded)
-
-
-def _ids(n=160, seed=5):
-    # distinct tokens per sequence: a repeated token gives exactly tied layer-0 key norms (see
-    # tests/test_reference_differential.py)
-    g = torch.Generator().manual_seed(seed)
-    return torch.stack([torch.randperm(250, generator=g)[:n] + 2 for _ in range(2)])
-
-
-def _model(family):
-    m = tiny_llama() if family == "llama" else tiny_qwen3()
-    m.config._attn_implementation = "sdpa"
-    return m
+ref = reference_store(STORE, "KVP_RECORD_CRITICALKV", TO_32BIT)
 
 
 INNER = {
@@ -286,14 +159,14 @@ def test_criticalkv_keeps_the_reference_rows(monkeypatch, ref, inner, ratio, fam
                     "torch.topk and the lowest-position rule break differently")
     cpu_backend.install(monkeypatch)
     criticalkv_backend.install(monkeypatch)
-    model, ids = _model(family), _ids()
+    model, ids = tiny_model(family), distinct_ids(160, seed=5)
     ref_inner, our_inner = INNER[inner]
 
     def reference(kvpress):
         cache = DynamicCache()
         with kvpress.CriticalKVPress(ref_inner(kvpress, ratio))(model):
             model.model(input_ids=ids, past_key_values=cache, cache_position=torch.arange(ids.shape[1]))
-        return {"len": cache.get_seq_length(), **{f"sig{i}": _rows_signature(la.keys, la.values)
+        return {"len": cache.get_seq_length(), **{f"sig{i}": rows_signature(la.keys, la.values)
                                                    for i, la in enumerate(cache.layers)}}
 
     want = ref(f"critical/{inner}/{ratio}/{family}", reference)
@@ -302,7 +175,7 @@ def test_criticalkv_keeps_the_reference_rows(monkeypatch, ref, inner, ratio, fam
         model.model(input_ids=ids, past_key_values=ours)
     assert ours.get_seq_length() == int(want["len"]) == int(ids.shape[1] * (1 - ratio))
     for i, la in enumerate(ours.layers):
-        close(_rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
+        close(rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
 
 
 def _masks(model, clear=True):
@@ -324,7 +197,7 @@ def test_critical_adakv_masks_and_decoding_step_match_the_reference(monkeypatch,
     criticalkv_backend.install(monkeypatch)
     # one sequence: the reference sums the head budgets over the batch and asks torch.topk for more than S positions
     # once a head's budget exceeds S (criticalkv_press.py:163-176)
-    model, ids = _model(family), _ids()[:1]
+    model, ids = tiny_model(family), distinct_ids(160, seed=5)[:1]
     ref_inner, our_inner = INNER[inner]
     nxt = torch.tensor([[7]])
 
@@ -354,7 +227,7 @@ def test_prefill_decoding_press_of_the_reference_readme(monkeypatch, ref):
     """PrefillDecodingPress(CriticalKVPress(KnormPress(0.5)), DecodingPress(KnormPress(), 5, 64)) at tiny size."""
     cpu_backend.install(monkeypatch)
     criticalkv_backend.install(monkeypatch)
-    model, ids = _model("llama"), _ids(120)
+    model, ids = tiny_model("llama"), distinct_ids(120, seed=5)
     steps = [torch.tensor([[10 + t], [40 + t]]) for t in range(12)]
 
     def drive(cache, **fw):
@@ -370,7 +243,7 @@ def test_prefill_decoding_press_of_the_reference_readme(monkeypatch, ref):
             decoding_press=kvpress.DecodingPress(kvpress.KnormPress(), compression_interval=5, target_size=64))
         with press(model):
             drive(cache, cache_position=torch.arange(ids.shape[1]))
-        return {"len": cache.get_seq_length(), **{f"sig{i}": _rows_signature(la.keys, la.values)
+        return {"len": cache.get_seq_length(), **{f"sig{i}": rows_signature(la.keys, la.values)
                                                    for i, la in enumerate(cache.layers)}}
 
     want = ref("prefill_decoding/critical_knorm", reference)
@@ -381,4 +254,4 @@ def test_prefill_decoding_press_of_the_reference_readme(monkeypatch, ref):
         drive(cache)
     assert cache.get_seq_length() == int(want["len"])
     for i, la in enumerate(cache.layers):
-        close(_rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
+        close(rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")

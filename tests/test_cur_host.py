@@ -15,14 +15,9 @@ float32 tiny Llamas, are stored in tests/golden/cur_reference.npz. To re-record 
 """
 import ctypes
 import itertools
-import json
 import math
-import os
-import subprocess
-import sys
 from pathlib import Path
 
-import numpy as np
 import pytest
 import torch
 from transformers import DynamicCache
@@ -31,158 +26,62 @@ from kvpress_b200 import (AdaKVPress, ChunkPress, ComposedPress, CriticalKVPress
                           KeyRerotationPress, KnormPress, native)
 from kvpress_b200.presses.cur_press import _cur_scores_fp32
 from oracle import press_oracle as O
-from tests import cpu_backend, criticalkv_backend, cur_backend as CB
-from tests.test_native_marshalling import _kv, rec  # noqa: F401  (fixture)
-from tests.test_reference_differential import _import_reference, _rows_signature, close
-from tests.tiny_models import tiny_llama
+from tests import abi_cases, cpu_backend, criticalkv_backend, cur_backend as CB
+from tests.abi_cases import GOOD, ODD16
+from tests.support import close, kv, rec, reference_store, rows_signature  # noqa: F401  (rec: fixture)
+from tests.tiny_models import distinct_ids, tiny_model
 
-ROOT = Path(__file__).resolve().parent.parent
-STORE = ROOT / "tests" / "golden" / "cur_reference.npz"
-RECORD = os.environ.get("KVP_RECORD_CUR") == "1"
+STORE = Path(__file__).resolve().parent / "golden" / "cur_reference.npz"
 WINDOW_MAX, RANK_MAX = 1024, 32
 TYPES = CB.LEVERAGE_TYPES
 
 # --------------------------------------------------------------------------------------------------
 # C ABI statuses
 # --------------------------------------------------------------------------------------------------
-GOOD, ODD16 = 0x10000, 0x1000C  # aligned; 4-byte but not 16-byte aligned
-FIELDS = dict(B=1, Hkv=2, Hq=2, S=1000, D=128, n_kept=500, dtype=0)
-STRIDES = (256000, 128000, 128)
-VALID = dict(K=GOOD, V=GOOD, sinks=4, type=3, w=16, G=None, r=0, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD, ws=GOOD,
-             ws_bytes="enough", stream=0)
-SLOTS = {
-    "kvp_cur_score": "K V sinks type w G r scores ws ws_bytes stream",
-    "kvp_cur_compress": "K V sinks type w G r K_out V_out idx scores ws ws_bytes stream",
-}
-CHANGES = {  # slot -> {label: value}
-    "p": {"null": None},
-    "dtype": {"1": 1, "3": 3},
-    "S": {"0": 0, "1": 1},
-    "D": {"8": 8, "12": 12, "264": 264},
-    "Hq": {"5": 5, "8": 8},
-    "n_kept": {"-1": -1, "0": 0, "1000": 1000, "1001": 1001},
-    "v_stride": {"s100": (256000, 128000, 100)},
-    "K": {"null": None, "odd": ODD16},
-    "V": {"null": None, "odd": ODD16},
-    "sinks": {"-1": -1, "0": 0, "1000": 1000, "max": 2 ** 31 - 1},
-    "type": {"-1": -1, "0": 0, "2": 2, "4": 4},
-    "w": {"-3": -3, "0": 0, "1": 1, str(WINDOW_MAX): WINDOW_MAX, str(WINDOW_MAX + 1): WINDOW_MAX + 1},
-    "G": {"set": GOOD, "odd": ODD16},
-    "r": {"-1": -1, "20": 20, str(RANK_MAX): RANK_MAX, str(RANK_MAX + 1): RANK_MAX + 1},
-    "K_out": {"null": None, "odd": ODD16},
-    "V_out": {"null": None},
-    "idx": {"null": None},
-    "scores": {"null": None, "odd": ODD16},
-    "ws": {"null": None, "odd": ODD16},
-    "ws_bytes": {"short": "short"},
-}
-PROBLEM = ("dtype", "S", "D", "Hq", "n_kept", "v_stride")
-
-
-def expected(name: str, c: dict) -> int:
-    """The documented check order: validate -> n_kept == 0 short cut (compress) -> K / V / outputs (compress) ->
-    K, V, scores null and K / V alignment (score call) -> num_sinks, leverage_type, local_window_size, r and G / r
-    together -> the kernel's window and r limits -> workspace."""
-    f = {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}
-    a = {**VALID, **{k: v for k, v in c.items() if k not in FIELDS}}
-    compress = name.endswith("compress")
-    if c.get("p", 0) is None:
-        return -1
-    if f["dtype"] not in (0, 1):
-        return -3
-    if f["S"] <= 0 or f["D"] % 8 or f["D"] > 256 or f["Hq"] % FIELDS["Hkv"]:
-        return -2
-    if not 0 <= f["n_kept"] <= f["S"]:
-        return -7
-    if "v_stride" in c:
-        return -4
-    if compress:
-        if f["n_kept"] == 0:
-            return 0
-        io = [a["K"], a["V"], a["K_out"], a["V_out"]]
-        if None in io:
-            return -1
-        if any(x % 16 for x in io):
-            return -4
-    else:
-        if None in (a["K"], a["V"], a["scores"]):
-            return -1
-        if a["K"] % 16 or a["V"] % 16:
-            return -4
+def _checks(f, a, compress):
+    """num_sinks, leverage_type, local_window_size, r and G / r together -> the kernel's window and r limits."""
     if a["sinks"] < 0 or not 0 <= a["type"] <= 3 or a["w"] < 0 or a["r"] < 0 or (a["G"] is None) != (a["r"] == 0):
         return -7
-    if a["w"] > WINDOW_MAX or a["r"] > RANK_MAX:
-        return -2
-    if a["ws"] is None:
-        return -1
-    if a["ws"] % 16:
-        return -4
-    if a["ws_bytes"] == "short":
-        return -5
-    return -6
+    return -2 if a["w"] > WINDOW_MAX or a["r"] > RANK_MAX else 0
 
 
-def _cases(name: str) -> dict:
-    slots = ["p", *PROBLEM, *SLOTS[name].split()]
-    singles = [(s, label, v) for s in slots for label, v in CHANGES.get(s, {}).items()]
-    cases = {"valid": {}, **{f"{s}={label}": {s: v} for s, label, v in singles}}
-    cases.update({f"{s1}={l1},{s2}={l2}": {s1: v1, s2: v2}
-                  for (s1, l1, v1), (s2, l2, v2) in itertools.combinations(singles, 2) if s1 != s2})
-    return cases
-
-
-def statuses() -> dict:
-    """Every case's status. Run only in a process that sees no GPU."""
-    import importlib.util
-
-    assert torch.cuda.device_count() == 0, "the status cases pass fake device pointers: they must not see a GPU"
-    spec = importlib.util.spec_from_file_location("kvp_native", ROOT / "kvpress_b200" / "native.py")
-    nat = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(nat)
-    lib = nat.load()
-
-    def problem(c):
-        p = nat.KvpProblem()
-        for k, v in {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}.items():
-            setattr(p, k, v)
-        p.k_stride = (ctypes.c_int64 * 3)(*STRIDES)
-        p.v_stride = (ctypes.c_int64 * 3)(*c.get("v_stride", STRIDES))
-        return p
-
-    out = {}
-    for name in SLOTS:
-        for label, c in _cases(name).items():
-            pr = None if c.get("p", 0) is None else problem(c)
-            need = ctypes.c_size_t(1 << 20)
-            if pr is not None:
-                lib.kvp_workspace_bytes(ctypes.byref(pr), nat.SCORER_CUR, ctypes.byref(need))
-            args = [None if pr is None else ctypes.byref(pr)]
-            for slot in SLOTS[name].split():
-                v = c.get(slot, VALID[slot])
-                if slot == "ws_bytes":
-                    v = need.value - 1 if v == "short" else need.value
-                elif slot == "idx" and v is not None:
-                    v = ctypes.cast(ctypes.c_void_p(v), ctypes.POINTER(ctypes.c_int32))
-                args.append(v)
-            out[f"{name}({label})"] = getattr(lib, name)(*args)
-    return out
+ABI = abi_cases.Spec(
+    scorer=native.SCORER_CUR, fields=dict(Hq=2),
+    slots={"kvp_cur_score": "K V sinks type w G r scores ws ws_bytes stream",
+           "kvp_cur_compress": "K V sinks type w G r K_out V_out idx scores ws ws_bytes stream"},
+    valid=dict(K=GOOD, V=GOOD, sinks=4, type=3, w=16, G=None, r=0, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD,
+               ws=GOOD, ws_bytes="enough", stream=0),
+    changes={
+        "p": {"null": None},
+        "dtype": {"1": 1, "3": 3},
+        "S": {"0": 0, "1": 1},
+        "D": {"8": 8, "12": 12, "264": 264},
+        "Hq": {"5": 5, "8": 8},
+        "n_kept": {"-1": -1, "0": 0, "1000": 1000, "1001": 1001},
+        "v_stride": {"s100": (256000, 128000, 100)},
+        "K": {"null": None, "odd": ODD16},
+        "V": {"null": None, "odd": ODD16},
+        "sinks": {"-1": -1, "0": 0, "1000": 1000, "max": 2 ** 31 - 1},
+        "type": {"-1": -1, "0": 0, "2": 2, "4": 4},
+        "w": {"-3": -3, "0": 0, "1": 1, str(WINDOW_MAX): WINDOW_MAX, str(WINDOW_MAX + 1): WINDOW_MAX + 1},
+        "G": {"set": GOOD, "odd": ODD16},
+        "r": {"-1": -1, "20": 20, str(RANK_MAX): RANK_MAX, str(RANK_MAX + 1): RANK_MAX + 1},
+        "K_out": {"null": None, "odd": ODD16},
+        "V_out": {"null": None},
+        "idx": {"null": None},
+        "scores": {"null": None, "odd": ODD16},
+        "ws": {"null": None, "odd": ODD16},
+        "ws_bytes": {"short": "short"},
+    },
+    operands={"score": (["K", "V", "scores"], ["K", "V"]), "compress": ([], [])},
+    checks=_checks)
 
 
 def test_every_status_of_the_cur_entry_points_follows_the_check_order():
-    env = {k: v for k, v in os.environ.items() if not k.startswith("KVP_")}
-    env["CUDA_VISIBLE_DEVICES"] = ""
-    code = "import json, tests.test_cur_host as m; print(json.dumps(m.statuses()))"
-    r = subprocess.run([sys.executable, *(["-s"] if sys.flags.no_user_site else []), "-c", code], cwd=ROOT, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    got = json.loads(r.stdout.strip().splitlines()[-1])
-    want = {f"{name}({label})": expected(name, c) for name in SLOTS for label, c in _cases(name).items()}
-    assert sorted(got) == sorted(want) and len(got) > 1900
+    want = abi_cases.assert_statuses(__name__, 1900)
     # a projection and its column count are one operand: both given is valid, and the limits are the kernel's
     assert want["kvp_cur_score(G=set,r=20)"] == -6 and want["kvp_cur_score(G=set,r=33)"] == -2
     assert want["kvp_cur_score(G=set)"] == want["kvp_cur_score(r=20)"] == -7
-    diffs = [f"{k}: {got[k]} != {want[k]}" for k in want if got[k] != want[k]]
-    assert not diffs, f"{len(diffs)} differences, first ones:\n" + "\n".join(diffs[:30])
 
 
 def test_workspace_and_launch_count_of_the_new_scorer_id():
@@ -212,7 +111,7 @@ def test_workspace_and_launch_count_of_the_new_scorer_id():
 # --------------------------------------------------------------------------------------------------
 def test_cur_wrappers_pass_their_full_argument_list(rec):  # noqa: F811
     P = lambda t: t.data_ptr()  # noqa: E731
-    k, v = _kv(B=2, H=2, S=300, D=64)
+    k, v = kv(B=2, H=2, S=300, D=64)
     G = torch.randn(64, 20)
 
     def last(name, n_kept):
@@ -257,24 +156,7 @@ def test_cur_wrappers_pass_their_full_argument_list(rec):  # noqa: F811
 # --------------------------------------------------------------------------------------------------
 # the float64 definition against the unmodified reference
 # --------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def ref():
-    stored = {} if RECORD or not STORE.exists() else dict(np.load(STORE))
-    recorded = {}
-
-    def result(key: str, compute) -> dict:
-        if RECORD:
-            out = {k: np.asarray(x.detach().numpy() if torch.is_tensor(x) else x)
-                   for k, x in compute(_import_reference()).items()}
-            recorded.update({f"{key}|{k}": x for k, x in out.items()})
-            return out
-        out = {k.split("|", 1)[1]: x for k, x in stored.items() if k.split("|", 1)[0] == key}
-        assert out, f"no stored reference result for {key}"
-        return out
-
-    yield result
-    if RECORD:
-        np.savez_compressed(STORE, **recorded)
+ref = reference_store(STORE, "KVP_RECORD_CUR")
 
 
 # (S, local_window_size): S a multiple of w, one more, one less, S below w, w = 1
@@ -413,17 +295,6 @@ def test_press_arguments_and_the_projection_draw(monkeypatch):
 # --------------------------------------------------------------------------------------------------
 # the press on tiny Llamas, with the float64 stand-ins in place of the kernels
 # --------------------------------------------------------------------------------------------------
-def _ids(n=150, seed=5):
-    g = torch.Generator().manual_seed(seed)
-    return torch.stack([torch.randperm(250, generator=g)[:n] + 2 for _ in range(2)])
-
-
-def _model():
-    m = tiny_llama()
-    m.config._attn_implementation = "sdpa"
-    return m
-
-
 @pytest.fixture
 def standins(monkeypatch):
     """The float64 stand-ins, with every CUR call recorded as (entry point, S, window, leverage type)."""
@@ -451,25 +322,25 @@ ALONE = [("kv_product", True, 16), ("kv_avg", True, 7), ("key", False, 16), ("va
 def test_press_keeps_the_reference_rows(standins, ref, leverage_type, local, w):
     """The press on a float32 tiny Llama keeps the rows the reference's CURPress keeps (150 positions: the last window
     is short)."""
-    ids = _ids()
+    ids = distinct_ids(150, seed=5)
     options = dict(compression_ratio=0.4, leverage_type=leverage_type, use_local_approximation=local,
                    local_window_size=w)
 
     def reference(kvpress):
-        model, cache = _model(), DynamicCache()
+        model, cache = tiny_model(), DynamicCache()
         with kvpress.CURPress(**options)(model):
             model.model(input_ids=ids, past_key_values=cache, cache_position=torch.arange(ids.shape[1]))
         return {"len": cache.get_seq_length(),
-                **{f"sig{i}": _rows_signature(la.keys, la.values) for i, la in enumerate(cache.layers)}}
+                **{f"sig{i}": rows_signature(la.keys, la.values) for i, la in enumerate(cache.layers)}}
 
     want = ref(f"press/{leverage_type}/{int(local)}/{w}", reference)
-    model, cache = _model(), DynamicCache()
+    model, cache = tiny_model(), DynamicCache()
     with CURPress(**options)(model):
         model.model(input_ids=ids, past_key_values=cache)
     assert cache.get_seq_length() == int(want["len"]) == 90
     assert standins == [("compress", 150, w if local else 0, leverage_type)] * 2
     for i, la in enumerate(cache.layers):
-        close(_rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
+        close(rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
 
 
 WRAPPED = {
@@ -490,29 +361,29 @@ class _Ours:
 def test_wrapped_press_keeps_the_reference_rows(standins, ref, wrapper):
     """ChunkPress (chunks of 40: not a multiple of the window, so each chunk has its own windows and a short last one),
     KeyRerotationPress, ComposedPress and CriticalKVPress over CURPress against the same wrappers of the reference."""
-    ids = _ids()
+    ids = distinct_ids(150, seed=5)
 
     def reference(kvpress):
-        model, cache = _model(), DynamicCache()
+        model, cache = tiny_model(), DynamicCache()
         with WRAPPED[wrapper](kvpress)(model):
             model.model(input_ids=ids, past_key_values=cache, cache_position=torch.arange(ids.shape[1]))
         return {"len": cache.get_seq_length(),
-                **{f"sig{i}": _rows_signature(la.keys, la.values) for i, la in enumerate(cache.layers)}}
+                **{f"sig{i}": rows_signature(la.keys, la.values) for i, la in enumerate(cache.layers)}}
 
     want = ref(f"wrapped/{wrapper}", reference)
-    model, cache = _model(), DynamicCache()
+    model, cache = tiny_model(), DynamicCache()
     with WRAPPED[wrapper](_Ours)(model):
         model.model(input_ids=ids, past_key_values=cache)
     assert cache.get_seq_length() == int(want["len"])
     if wrapper == "chunk":
         assert standins == ([("score", 40, 16, "kv_product")] * 3 + [("score", 30, 16, "kv_product")]) * 2
     for i, la in enumerate(cache.layers):
-        close(_rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
+        close(rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
 
 
 def test_adakv_decoding_and_a_user_subclass(standins):
-    ids = _ids()
-    model, cache = _model(), DynamicCache()
+    ids = distinct_ids(150, seed=5)
+    model, cache = tiny_model(), DynamicCache()
     with AdaKVPress(CURPress(compression_ratio=0.4))(model):
         model.model(input_ids=ids, past_key_values=cache)
     attn = [layer.self_attn for layer in model.model.layers]
@@ -526,7 +397,7 @@ def test_adakv_decoding_and_a_user_subclass(standins):
         a.masked_key_indices = None
 
     del standins[:]
-    model, cache = _model(), DynamicCache()
+    model, cache = tiny_model(), DynamicCache()
     with DecodingPress(CURPress(), compression_interval=4, target_size=100)(model):
         model.model(input_ids=ids[:, :120], past_key_values=cache)
         for t in range(8):
@@ -539,7 +410,7 @@ def test_adakv_decoding_and_a_user_subclass(standins):
             return -super().score(module, hidden_states, keys, values, attentions, kwargs)
 
     del standins[:]
-    model, cache = _model(), DynamicCache()
+    model, cache = tiny_model(), DynamicCache()
     with Reversed(compression_ratio=0.4)(model):
         model.model(input_ids=ids, past_key_values=cache)
     # the overriding score() is used: the generic selection, and the sinks (score -1, the lowest) are dropped

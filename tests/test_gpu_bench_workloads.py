@@ -34,11 +34,9 @@ import pytest
 import torch
 
 from oracle import press_oracle as O
-from tests.test_gpu_keydiff_rerotation_sweep import (assert_e_small, assert_keydiff_vs_ref, assert_rerotated, kd_chain,
-                                                     keydiff_error_bound, keydiff_ref64)
-from tests.test_gpu_knorm_sweep import _same, knorm_ref64
-from tests.test_gpu_scorer_sweep import (_forced_head, _forced_tail, _gather, assert_vs_ref64, ea_ref64,
-                                         snap_ref64)
+from tests.gpu_support import (assert_e_small, assert_keydiff_vs_ref, assert_rerotated, assert_vs_ref64, ea_ref64,
+                               _forced_head, _forced_tail, _gather, kd_chain, keydiff_error_bound, keydiff_ref64,
+                               knorm_ref64, _name, _native, _same, snap_ref64)
 
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
@@ -48,16 +46,6 @@ import bench  # noqa: E402
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 DTYPES = [torch.bfloat16, torch.float16]
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
-
-
-def _name(dtype) -> str:
-    return "bf16" if dtype == torch.bfloat16 else "fp16"
 
 
 def _n_kept(w: dict) -> int:

@@ -6,7 +6,6 @@ row bias (|mean relative error| <= 8 u / sqrt(12 n) over rows of >= 500 normal-r
 are exactly the lowest-index-ties top-n_first of the base scores and hold finfo(dtype).max. Compress keeps the
 top-n_kept of its own scores and returns exact gathers.
 """
-import math
 
 import pytest
 import torch
@@ -14,8 +13,8 @@ from transformers import DynamicCache
 
 from oracle import press_oracle as O
 from tests import criticalkv_backend
-from tests.conftest import ulp16_diff
 from tests.tiny_models import tiny_llama
+from tests.gpu_support import ckv_assert_scores, ckv_inputs, _name, _native
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
@@ -24,71 +23,11 @@ UNIT_ROUNDOFF = {torch.bfloat16: 2.0 ** -7, torch.float16: 2.0 ** -10}
 BIAS_MIN_N = 500
 
 
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
-
-
-def _name(dtype) -> str:
-    return "bf16" if dtype == torch.bfloat16 else "fp16"
-
-
-def inputs(B, Hkv, G, S, D, hidden, dtype, seed, base_scale=1.0):
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    v = torch.randn((B, Hkv, S, D), generator=g, device=DEV).to(dtype)
-    wo = (torch.randn((hidden, Hkv * G * D), generator=g, device=DEV) / math.sqrt(D)).to(dtype)
-    base = (torch.rand((B, Hkv, S), generator=g, device=DEV) * base_scale).to(dtype)
-    return v, wo, base
-
-
-def ref64(base, v, wo, eps: float) -> torch.Tensor:
-    """(base + eps) * mean_g sum_n |v . wo[n, h D:(h+1) D]| in float64 on the device, one query head at a time."""
-    B, Hkv, S, D = v.shape
-    Hq = wo.shape[1] // D
-    G = Hq // Hkv
-    w = wo.double()
-    norm = torch.zeros((B, Hkv, S), dtype=torch.float64, device=v.device)
-    for h in range(Hq):
-        for s0 in range(0, S, 4096):
-            s1 = min(S, s0 + 4096)
-            norm[:, h // G, s0:s1] += (v[:, h // G, s0:s1].double() @ w[:, h * D:(h + 1) * D].T).abs().sum(-1)
-    return (base.double() + eps) * (norm / G)
-
-
-def assert_scores(got, base, v, wo, eps, n_first, what, bias=True):
-    dtype = got.dtype
-    ref = ref64(base, v, wo, eps)
-    forced = torch.zeros(got.shape, dtype=torch.bool, device=got.device)
-    if n_first > 0:
-        forced.scatter_(-1, O.select_lowest_index_ties(base, n_first), True)
-    assert (got[forced] == torch.finfo(dtype).max).all(), f"{what}: forced positions do not hold finfo.max"
-    if n_first > 0:  # no other position holds it (the fp64 scores of these inputs stay far below)
-        assert int((got == torch.finfo(dtype).max).sum()) == int(forced.sum()), what
-    g, r = got[~forced], ref[~forced]
-    d = ulp16_diff(g, r.to(dtype))
-    assert (d <= 1).all(), f"{what}: {int((d > 1).sum())} positions beyond 1 ulp of the fp64 score (max {int(d.max())})"
-    worst = 0.0
-    if bias:
-        normal = (ref.abs() >= torch.finfo(dtype).tiny) & ~forced & torch.isfinite(ref.to(dtype))
-        n = normal.sum(-1)
-        rel = torch.where(normal, (got.double() - ref) / ref, torch.zeros_like(ref))
-        mean = rel.sum(-1) / n.clamp_min(1)
-        bound = 8 * UNIT_ROUNDOFF[dtype] / torch.sqrt(12.0 * n.clamp_min(1).double())
-        rows = n >= BIAS_MIN_N
-        ratio = (mean.abs() / bound)[rows]
-        if ratio.numel():
-            worst = float(ratio.max())
-            assert (ratio <= 1).all(), f"{what}: row bias {worst:.2f}x its bound"
-    print(f"[measured] {what}: max ulp {int(d.max()) if d.numel() else 0}, "
-          f"1-ulp fraction {float((d == 1).float().mean()) if d.numel() else 0.0:.4f}, worst row bias {worst:.3f}")
-
-
 def run_score(v, wo, base, eps, n_first, what, bias=True):
     native = _native()
     got = native.criticalkv_score(base, v, wo, eps, n_first)
     torch.cuda.synchronize()
-    assert_scores(got, base, v, wo, eps, n_first, what, bias)
+    ckv_assert_scores(got, base, v, wo, eps, n_first, what, bias)
     return got
 
 
@@ -101,7 +40,7 @@ def run_score(v, wo, base, eps, n_first, what, bias=True):
 @pytest.mark.parametrize("dtype", DTYPES, ids=_name)
 def test_instantiations(dtype, D, G):
     S = 1000
-    v, wo, base = inputs(1, 2, G, S, D, 1000, dtype, seed=G * 10 + D)
+    v, wo, base = ckv_inputs(1, 2, G, S, D, 1000, dtype, seed=G * 10 + D)
     run_score(v, wo, base, 1e-4, 200, f"ckv {_name(dtype)} d{D} g{G}")
 
 
@@ -110,21 +49,21 @@ def test_instantiations(dtype, D, G):
 @pytest.mark.parametrize("dtype", DTYPES, ids=_name)
 def test_hidden_sizes(dtype, hidden):
     """hidden a multiple of the 128-row Wo chunk, not one, and below one chunk: rows past hidden read as zero."""
-    v, wo, base = inputs(1, 2, 4, 700, 128, hidden, dtype, seed=hidden)
+    v, wo, base = ckv_inputs(1, 2, 4, 700, 128, hidden, dtype, seed=hidden)
     run_score(v, wo, base, 1e-4, 100, f"ckv {_name(dtype)} hidden {hidden}")
 
 
 @gpu
 @pytest.mark.parametrize("S", [1, 127, 128, 129, 255, 256, 257, 4097])
 def test_sequence_lengths_and_batch(S):
-    v, wo, base = inputs(3, 2, 2, S, 64, 512, torch.bfloat16, seed=S)
+    v, wo, base = ckv_inputs(3, 2, 2, S, 64, 512, torch.bfloat16, seed=S)
     run_score(v, wo, base, 1e-4, S // 3, f"ckv S {S} B 3")
 
 
 @gpu
 def test_llama8b_layer_rows_spread_over_every_sm():
     """The 8B layer shape at 8k: 256 items, so every CTA owns items of several rows."""
-    v, wo, base = inputs(1, 8, 4, 8192, 128, 4096, torch.bfloat16, seed=8)
+    v, wo, base = ckv_inputs(1, 8, 4, 8192, 128, 4096, torch.bfloat16, seed=8)
     run_score(v, wo, base, 1e-4, 2048, "ckv llama8b 8k")
 
 
@@ -133,7 +72,7 @@ def test_llama8b_layer_rows_spread_over_every_sm():
 def test_strided_operands_are_consumed_in_place(layout):
     native = _native()
     B, Hkv, G, S, D, hidden = 2, 4, 2, 600, 128, 700
-    v, wo, base = inputs(B, Hkv, G, S, D, hidden, torch.bfloat16, seed=3)
+    v, wo, base = ckv_inputs(B, Hkv, G, S, D, hidden, torch.bfloat16, seed=3)
     if layout == "s_slice":
         big = torch.randn((B, Hkv, S + 40, D), device=DEV).to(v.dtype)
         big[:, :, 17:17 + S] = v
@@ -148,13 +87,13 @@ def test_strided_operands_are_consumed_in_place(layout):
     assert not vv.is_contiguous() or not ww.is_contiguous()
     got = native.criticalkv_score(base, vv, ww, 1e-4, 50)
     assert torch.equal(got, native.criticalkv_score(base, v, wo, 1e-4, 50))
-    assert_scores(got, base, v, wo, 1e-4, 50, f"ckv {layout}")
+    ckv_assert_scores(got, base, v, wo, 1e-4, 50, f"ckv {layout}")
 
 
 @gpu
 def test_base_scores_with_sentinels_and_strided_base():
     """Base scores of a wrapped press carry max + 1 on its forced positions; a broadcast-free strided base view."""
-    v, wo, base = inputs(2, 2, 4, 900, 64, 512, torch.bfloat16, seed=4)
+    v, wo, base = ckv_inputs(2, 2, 4, 900, 64, 512, torch.bfloat16, seed=4)
     base[..., :4] = (base.float().max() + 1).to(base.dtype)
     base[..., -64:] = (base.float().max() + 1).to(base.dtype)
     run_score(v, wo, base, 1e-4, 100, "ckv sentinels")
@@ -166,7 +105,7 @@ def test_base_scores_with_sentinels_and_strided_base():
 
 @gpu
 def test_fp16_overflow_goes_to_inf():
-    v, wo, base = inputs(1, 2, 2, 600, 128, 2048, torch.float16, seed=5, base_scale=60000.0)
+    v, wo, base = ckv_inputs(1, 2, 2, 600, 128, 2048, torch.float16, seed=5, base_scale=60000.0)
     got = run_score(v, wo, base, 1e-4, 10, "ckv fp16 overflow", bias=False)
     assert torch.isinf(got).sum() > 100
 
@@ -174,7 +113,7 @@ def test_fp16_overflow_goes_to_inf():
 @gpu
 @pytest.mark.parametrize("n_first", [0, 1, 333, 600, 1000])
 def test_forced_positions_are_the_top_n_first_of_base(n_first):
-    v, wo, base = inputs(2, 2, 2, 1000, 64, 256, torch.float16, seed=6)
+    v, wo, base = ckv_inputs(2, 2, 2, 1000, 64, 256, torch.float16, seed=6)
     base[0, 0, 100:300] = base[0, 0, 100]  # a long run of ties across the n_first threshold
     got = run_score(v, wo, base, 1e-4, n_first, f"ckv n_first {n_first}")
     assert int((got == torch.finfo(got.dtype).max).sum()) == 4 * n_first
@@ -183,7 +122,7 @@ def test_forced_positions_are_the_top_n_first_of_base(n_first):
 @gpu
 def test_two_calls_are_bitwise_equal():
     native = _native()
-    v, wo, base = inputs(1, 8, 4, 20000, 128, 2048, torch.bfloat16, seed=7)
+    v, wo, base = ckv_inputs(1, 8, 4, 20000, 128, 2048, torch.bfloat16, seed=7)
     a = native.criticalkv_score(base, v, wo, 1e-4, 5000)
     b = native.criticalkv_score(base, v, wo, 1e-4, 5000)
     assert torch.equal(a.view(torch.int16), b.view(torch.int16))
@@ -195,12 +134,12 @@ def test_two_calls_are_bitwise_equal():
 def test_compress_keeps_the_top_of_its_own_scores(dtype, n_first):
     native = _native()
     B, Hkv, G, S, D, hidden = 2, 2, 4, 1000, 128, 1000
-    v, wo, base = inputs(B, Hkv, G, S, D, hidden, dtype, seed=8)
+    v, wo, base = ckv_inputs(B, Hkv, G, S, D, hidden, dtype, seed=8)
     k = torch.randn_like(v)
     n_kept = 400
     k_out, v_out, idx, scores = native.criticalkv_compress(base, k, v, wo, 1e-4, n_first, n_kept, True, True)
     assert torch.equal(scores, native.criticalkv_score(base, v, wo, 1e-4, n_first))
-    assert_scores(scores, base, v, wo, 1e-4, n_first, f"ckv compress {_name(dtype)} n_first {n_first}")
+    ckv_assert_scores(scores, base, v, wo, 1e-4, n_first, f"ckv compress {_name(dtype)} n_first {n_first}")
     want = O.select_lowest_index_ties(scores, n_kept)
     assert torch.equal(idx.long(), want)
     assert torch.equal(k_out, O.gather_rows(k, want)) and torch.equal(v_out, O.gather_rows(v, want))
@@ -211,7 +150,7 @@ def test_compress_keeps_the_top_of_its_own_scores(dtype, n_first):
 @gpu
 def test_compress_replays_under_capture():
     native = _native()
-    v, wo, base = inputs(1, 4, 2, 3000, 64, 1024, torch.bfloat16, seed=9)
+    v, wo, base = ckv_inputs(1, 4, 2, 3000, 64, 1024, torch.bfloat16, seed=9)
     k = torch.randn_like(v)
     eager = native.criticalkv_compress(base, k, v, wo, 1e-4, 500, 1500, True, True)
     g = native.capture(lambda: native.criticalkv_compress(base, k, v, wo, 1e-4, 500, 1500, True, True))
@@ -228,7 +167,7 @@ def test_no_intermediate_at_32k():
     """Memory grows by no more than the workspace and the outputs: nothing of size S x hidden is allocated."""
     native = _native()
     B, Hkv, G, S, D, hidden = 1, 8, 4, 32768, 128, 4096
-    v, wo, base = inputs(B, Hkv, G, S, D, hidden, torch.bfloat16, seed=10)
+    v, wo, base = ckv_inputs(B, Hkv, G, S, D, hidden, torch.bfloat16, seed=10)
     k = torch.randn_like(v)
     n_kept = S // 2
     p = native.make_problem(k, v, n_kept, Hkv * G)

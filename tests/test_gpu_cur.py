@@ -30,9 +30,8 @@ from transformers import DynamicCache
 from oracle import press_oracle as O
 from tests import cur_backend as CB
 from tests.conftest import ulp16_diff
-from tests.test_gpu_lagkv import _ids, _masked, _model, _prefill, _shared, inputs, same
-from tests.test_gpu_non_causal_attention import ulp_at
-from tests.test_gpu_scorer_sweep import assert_compress
+from tests.gpu_support import (assert_compress, gpu_ids, lagkv_inputs, _masked, _name, _native, _prefill, same16,
+                               _shared, tiny_gpu_llama, ulp_at)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
@@ -40,16 +39,6 @@ U = 2.0 ** -24
 WINDOW_MAX, RANK_MAX = 1024, 32
 TYPES = CB.LEVERAGE_TYPES
 ROOT = Path(__file__).resolve().parent.parent
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
-
-
-def _name(dtype) -> str:
-    return "bf16" if dtype == torch.bfloat16 else "fp16"
 
 
 def projection(D: int, r: int, seed: int) -> torch.Tensor:
@@ -128,11 +117,11 @@ def run(k, v, sinks, leverage_type, w, G, what, n_kept=None):
     S = k.shape[2]
     sc = nat.cur_score(k, v, sinks, leverage_type, w, G)
     check(k, v, sinks, leverage_type, w, G, sc, what)
-    assert same(nat.cur_score(k, v, sinks, leverage_type, w, G), sc), f"{what}: two calls differ"
+    assert same16(nat.cur_score(k, v, sinks, leverage_type, w, G), sc), f"{what}: two calls differ"
     n_kept = max(1, O.kept_count(S, 0.5)) if n_kept is None else n_kept
     k_out, v_out, idx, sc2 = nat.cur_compress(k, v, sinks, leverage_type, w, G, n_kept, return_indices=True,
                                               return_scores=True)
-    assert same(sc2, sc), f"{what}: compress scores differ from the score call"
+    assert same16(sc2, sc), f"{what}: compress scores differ from the score call"
     assert_compress(k, v, k_out, v_out, idx, sc2, n_kept)
     return sc
 
@@ -162,7 +151,7 @@ def test_sweep_reaches_every_instantiation():
 @gpu
 @pytest.mark.parametrize("dtype,D", SWEEP, ids=[f"{_name(dt)}-d{D}" for dt, D in SWEEP])
 def test_instantiations(dtype, D):
-    k, v = inputs(2, 2, 1000 + D, D, dtype, seed=D)
+    k, v = lagkv_inputs(2, 2, 1000 + D, D, dtype, seed=D)
     G = projection(D, 20, D)
     for leverage_type in TYPES:
         for w in (16, 0):
@@ -173,7 +162,7 @@ def test_instantiations(dtype, D):
 @gpu
 @pytest.mark.parametrize("w", [1, 2, 15, 16, 17, 100, 255, 256, 257, 1000, WINDOW_MAX])
 def test_window_sizes(w):
-    k, v = inputs(1, 3, 2 * max(w, 300) + 37, 64, torch.bfloat16, seed=w)
+    k, v = lagkv_inputs(1, 3, 2 * max(w, 300) + 37, 64, torch.bfloat16, seed=w)
     for leverage_type in ("kv_product", "kv_avg"):
         run(k, v, 4, leverage_type, w, None, f"cur w{w} {leverage_type}")
 
@@ -182,7 +171,7 @@ def test_window_sizes(w):
 @pytest.mark.parametrize("S", [1, 2, 15, 16, 17, 255, 256, 257, 272, 511, 512, 513, 4099])
 def test_sequence_boundaries(S):
     """S through the window (16), unit (256) and tile boundaries, S below the window, and every num_sinks regime."""
-    k, v = inputs(2, 2, S, 128, torch.float16, seed=S)
+    k, v = lagkv_inputs(2, 2, S, 128, torch.float16, seed=S)
     for sinks in (0, 4, S, S + 1):
         for w in (16, 0, 300):
             run(k, v, sinks, "kv_product", w, None, f"cur S{S} sinks{sinks} w{w}")
@@ -190,27 +179,27 @@ def test_sequence_boundaries(S):
 
 @gpu
 def test_128k_and_many_rows():
-    k, v = inputs(1, 8, 131072, 128, torch.bfloat16, seed=1)
+    k, v = lagkv_inputs(1, 8, 131072, 128, torch.bfloat16, seed=1)
     run(k, v, 4, "kv_product", 16, None, "cur 128k")
     run(k, v, 4, "kv_product", 16, projection(128, 20, 3), "cur 128k projected")
     del k, v
-    k, v = inputs(30, 100, 300, 64, torch.bfloat16, seed=2)  # 3000 rows
+    k, v = lagkv_inputs(30, 100, 300, 64, torch.bfloat16, seed=2)  # 3000 rows
     sc = run(k, v, 4, "kv_product", 16, None, "cur 3000 rows")
     nat = _native()
     for b, h in ((0, 0), (17, 43), (29, 99)):
         alone = nat.cur_score(k[b:b + 1, h:h + 1], v[b:b + 1, h:h + 1], 4, "kv_product", 16)
-        assert same(alone[0, 0], sc[b, h])
+        assert same16(alone[0, 0], sc[b, h])
 
 
 @gpu
 def test_a_batch_equals_its_rows_run_alone():
     nat = _native()
-    k, v = inputs(3, 2, 5000, 128, torch.bfloat16, seed=5)
+    k, v = lagkv_inputs(3, 2, 5000, 128, torch.bfloat16, seed=5)
     G = projection(128, 20, 1)
     for g in (None, G):
         sc = nat.cur_score(k, v, 4, "kv_product", 16, g)
         for b in range(3):
-            assert same(nat.cur_score(k[b:b + 1], v[b:b + 1], 4, "kv_product", 16, g), sc[b:b + 1])
+            assert same16(nat.cur_score(k[b:b + 1], v[b:b + 1], 4, "kv_product", 16, g), sc[b:b + 1])
 
 
 # --------------------------------------------------------------------------------------------------
@@ -220,7 +209,7 @@ def test_a_batch_equals_its_rows_run_alone():
 @pytest.mark.parametrize("r", [1, 3, 20, RANK_MAX])
 def test_projection_ranks(r):
     for dtype, D in ((torch.bfloat16, 128), (torch.float16, 256), (torch.bfloat16, 40)):
-        k, v = inputs(1, 2, 1500, D, dtype, seed=r)
+        k, v = lagkv_inputs(1, 2, 1500, D, dtype, seed=r)
         G = projection(D, r, r)
         for leverage_type in TYPES:
             run(k, v, 4, leverage_type, 16, G, f"cur r{r} d{D} {leverage_type}")
@@ -235,7 +224,7 @@ def test_limits_and_the_press_fallback():
 
     nat = _native()
     w = WINDOW_MAX + 1
-    k, v = inputs(1, 2, 2 * w + 11, 64, torch.bfloat16, seed=4)
+    k, v = lagkv_inputs(1, 2, 2 * w + 11, 64, torch.bfloat16, seed=4)
     with pytest.raises(RuntimeError, match="unsupported shape"):
         nat.cur_score(k, v, 4, "kv_product", w)
     with pytest.raises(RuntimeError, match="unsupported shape"):
@@ -255,7 +244,7 @@ def test_limits_and_the_press_fallback():
     sc = press.score(None, None, k, v, None, {})
     torch.manual_seed(77)
     G = torch.randn(64, 20, device=DEV) / math.sqrt(20)
-    assert same(sc, nat.cur_score(k, v, 4, "kv_product", 16, G))
+    assert same16(sc, nat.cur_score(k, v, 4, "kv_product", 16, G))
     check(k, v, 4, "kv_product", 16, G, sc, "cur press draw")
 
 
@@ -267,7 +256,7 @@ def test_limits_and_the_press_fallback():
 def test_layouts(layout):
     nat = _native()
     B, H, S, D = 2, 4, 3000, 128
-    k, v = inputs(B, H, S, D, torch.bfloat16, seed=7)
+    k, v = lagkv_inputs(B, H, S, D, torch.bfloat16, seed=7)
     if layout == "strided":  # rows of D within rows of D + 64
         kb = torch.zeros((B, H, S, D + 64), dtype=k.dtype, device=DEV)
         vb = torch.zeros_like(kb)
@@ -281,7 +270,7 @@ def test_layouts(layout):
         assert not k.is_contiguous() and nat._rows_ok(k)
     for G in (None, projection(D, 20, 2)):
         sc = run(k, v, 4, "kv_product", 16, G, f"cur {layout}")
-        assert same(sc, nat.cur_score(k.contiguous(), v.contiguous(), 4, "kv_product", 16, G))
+        assert same16(sc, nat.cur_score(k.contiguous(), v.contiguous(), 4, "kv_product", 16, G))
 
 
 @gpu
@@ -294,11 +283,11 @@ def test_schedule_regimes(regime):
     sm = torch.cuda.get_device_properties(0).multi_processor_count
     units = {"fewer": 2 * sm, "equal": 4 * sm, "more": 8 * sm + 3}[regime]
     S = units * 256 - 5
-    k, v = inputs(1, 1, S, 64, torch.float16, seed=units)
+    k, v = lagkv_inputs(1, 1, S, 64, torch.float16, seed=units)
     sc = run(k, v, 4, "kv_product", 16, None, f"cur schedule {regime} ({units} units, {sm} SMs)")
     kb, vb = k.expand(1, 7, S, 64).contiguous(), v.expand(1, 7, S, 64).contiguous()  # ceil(4 sm / 7) CTAs per row
     batch = nat.cur_score(kb, vb, 4, "kv_product", 16)
-    assert all(same(batch[:, h:h + 1], sc) for h in range(7))
+    assert all(same16(batch[:, h:h + 1], sc) for h in range(7))
 
 
 # --------------------------------------------------------------------------------------------------
@@ -307,7 +296,7 @@ def test_schedule_regimes(regime):
 @gpu
 def test_zero_windows_zero_rows_nan_and_inf():
     nat = _native()
-    k, v = inputs(1, 4, 1000, 64, torch.bfloat16, seed=3)
+    k, v = lagkv_inputs(1, 4, 1000, 64, torch.bfloat16, seed=3)
     k[0, 0, 32:48] = 0                # an all-zero window: 0/0, the whole row NaN but the sinks
     v[0, 1, 5] = 0                    # a zero row inside a non-zero window: scores 0
     v[0, 2, 700, 3] = float("nan")    # a NaN input: its row NaN
@@ -324,25 +313,25 @@ def test_zero_windows_zero_rows_nan_and_inf():
         assert torch.isnan(sc[..., 4:]).all() and (sc[..., :4] == 1).all()
     # an inf input: inside a window inf / inf = NaN, so its row is NaN; without windows T is inf, the position itself
     # is inf / inf = NaN and every other position of the row is x / inf = 0
-    k, v = inputs(1, 2, 600, 64, torch.float16, seed=6)
+    k, v = lagkv_inputs(1, 2, 600, 64, torch.float16, seed=6)
     k[0, 1, 100, 0] = float("inf")
     sc = run(k, v, 4, "key", 16, None, "cur inf local")
     assert torch.isnan(sc[0, 1, 4:]).all() and torch.isfinite(sc[0, 0]).all()
     sc = nat.cur_score(k, v, 4, "key", 0)
     assert torch.isnan(sc[0, 1, 100]) and (sc[0, 1, 4:100] == 0).all() and (sc[0, 1, 101:] == 0).all()
-    assert same(sc, CB.cur_score(k, v, 4, "key", 0))
+    assert same16(sc, CB.cur_score(k, v, 4, "key", 0))
 
 
 @gpu
 def test_values_near_the_top_of_the_range():
     """fp16 near 65504: every fp32 intermediate stays finite (65504^2 * 256 squared is 1e24). bf16 scaled to 1e15: the
     squared norms (1e32) are finite, and with windows so is everything after them."""
-    k, v = inputs(1, 2, 1500, 128, torch.float16, seed=8)
+    k, v = lagkv_inputs(1, 2, 1500, 128, torch.float16, seed=8)
     k = (k.float() / k.float().abs().amax() * 65000).half()
     v = (v.float() / v.float().abs().amax() * 60000).half()
     for w in (16, 0):
         run(k, v, 4, "kv_product", w, None, f"cur fp16 top of range w{w}")
-    k, v = inputs(1, 2, 1500, 128, torch.bfloat16, seed=9, scale=1e15)
+    k, v = lagkv_inputs(1, 2, 1500, 128, torch.bfloat16, seed=9, scale=1e15)
     run(k, v, 4, "kv_product", 16, None, "cur bf16 1e15")
 
 
@@ -354,13 +343,13 @@ def test_planted_exact_ties_go_to_the_lowest_position():
     """Periodic K and V: every window repeats, so every score value occurs once per period; the kept set is the
     stand-in's, with ties to the lowest positions."""
     nat = _native()
-    k, v = inputs(1, 2, 64, 64, torch.bfloat16, seed=11)
+    k, v = lagkv_inputs(1, 2, 64, 64, torch.bfloat16, seed=11)
     k, v = k.repeat(1, 1, 20, 1), v.repeat(1, 1, 20, 1)
     sc = run(k, v, 0, "kv_product", 16, None, "cur ties", n_kept=333)
-    assert same(sc[..., :64], sc[..., 64:128]) and sc[0, 0].unique().numel() <= 64
+    assert same16(sc[..., :64], sc[..., 64:128]) and sc[0, 0].unique().numel() <= 64
     got = nat.cur_compress(k, v, 0, "kv_product", 16, None, 333, True, True)
     want = CB.cur_compress(k, v, 0, "kv_product", 16, None, 333, True, True)
-    if same(got[3], want[3]):  # identical scores: the selections must be identical
+    if same16(got[3], want[3]):  # identical scores: the selections must be identical
         assert all(torch.equal(a, b) for a, b in zip(got[:3], want[:3]))
 
 
@@ -369,13 +358,13 @@ def test_compress_edges_nullable_outputs_and_n_kept_zero():
     import ctypes
 
     nat = _native()
-    k, v = inputs(2, 2, 700, 64, torch.bfloat16, seed=12)
+    k, v = lagkv_inputs(2, 2, 700, 64, torch.bfloat16, seed=12)
     S = k.shape[2]
     for n_kept in (1, S):
         run(k, v, 4, "kv_product", 16, None, f"cur n_kept {n_kept}", n_kept=n_kept)
     full = nat.cur_compress(k, v, 4, "kv_product", 16, None, 300, True, True)
     bare = nat.cur_compress(k, v, 4, "kv_product", 16, None, 300)
-    assert bare[2] is None and bare[3] is None and same(bare[0], full[0]) and same(bare[1], full[1])
+    assert bare[2] is None and bare[3] is None and same16(bare[0], full[0]) and same16(bare[1], full[1])
     p = nat.make_problem(k, v, 0)
     ws = nat._workspace(p, nat.SCORER_CUR, k.device)
     outs = [torch.full((2, 2, 0, 64), 3, dtype=k.dtype, device=DEV) for _ in range(2)]
@@ -393,7 +382,7 @@ def test_compress_edges_nullable_outputs_and_n_kept_zero():
 @gpu
 def test_replays_under_capture_and_workspace_check():
     nat = _native()
-    k, v = inputs(1, 8, 8000, 128, torch.bfloat16, seed=9)
+    k, v = lagkv_inputs(1, 8, 8000, 128, torch.bfloat16, seed=9)
     G = projection(128, 20, 5)
     call = lambda: (nat.cur_score(k, v, 4, "kv_avg", 16, G),  # noqa: E731
                     *nat.cur_compress(k, v, 4, "kv_product", 16, None, 4000, True, True))
@@ -401,12 +390,12 @@ def test_replays_under_capture_and_workspace_check():
     g = nat.capture(call)
     out = g.replay()
     torch.cuda.synchronize()
-    assert all(same(a, b) for a, b in zip(out, eager))
+    assert all(same16(a, b) for a, b in zip(out, eager))
     k.copy_(torch.randn_like(k.float()).to(k.dtype))  # inputs updated in place
     v.mul_(-1)
     out = g.replay()
     torch.cuda.synchronize()
-    assert all(same(a, b) for a, b in zip(out, call()))
+    assert all(same16(a, b) for a, b in zip(out, call()))
     assert not torch.equal(out[3], eager[3])
     p = nat.make_problem(k, v, 4000)
     nat.workspace_check(p, nat.SCORER_CUR, nat._workspace(p, nat.SCORER_CUR, k.device))
@@ -418,7 +407,7 @@ def test_no_intermediate_at_128k():
     temporary."""
     nat = _native()
     B, H, S, D = 1, 8, 131072, 128
-    k, v = inputs(B, H, S, D, torch.bfloat16, seed=10)
+    k, v = lagkv_inputs(B, H, S, D, torch.bfloat16, seed=10)
     n_kept = S // 2
     p = nat.make_problem(k, v, n_kept)
     ws = nat.workspace_bytes(p, nat.SCORER_CUR)
@@ -468,7 +457,7 @@ def _standin(press_factory, forward, monkeypatch):
     kernels."""
     with monkeypatch.context() as m:
         CB.install(m)
-        model, cache = _model(), DynamicCache()
+        model, cache = tiny_gpu_llama(), DynamicCache()
         with press_factory()(model):
             forward(model, cache)
     return model, cache
@@ -479,9 +468,9 @@ def _standin(press_factory, forward, monkeypatch):
 def test_press_on_a_tiny_llama(checked, monkeypatch, leverage_type):
     from kvpress_b200 import CURPress
 
-    ids = _ids()
+    ids = gpu_ids()
     factory = lambda: CURPress(compression_ratio=0.5, leverage_type=leverage_type)  # noqa: E731
-    model, cache = _model(), DynamicCache()
+    model, cache = tiny_gpu_llama(), DynamicCache()
     with factory()(model):
         model.model(input_ids=ids, past_key_values=cache)
     assert cache.get_seq_length() == 120 and checked == [("compress", 240)] * 2
@@ -496,8 +485,8 @@ def test_wrapper_presses_on_a_tiny_llama(checked, monkeypatch):
     from kvpress_b200 import (AdaKVPress, ChunkPress, ComposedPress, CriticalKVPress, CURPress, DecodingPress,
                               KeyRerotationPress, KnormPress)
 
-    ids = _ids()
-    model = _model()
+    ids = gpu_ids()
+    model = tiny_gpu_llama()
     cache = DynamicCache()
     ada = lambda: AdaKVPress(CURPress(compression_ratio=0.5))  # noqa: E731
     with ada()(model):

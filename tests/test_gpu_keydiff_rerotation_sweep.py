@@ -55,7 +55,6 @@ decides positions in 2 of 142 checks, at most 2.8e-5 of a case, and the largest 
 0.27 of its bound. Rerotation: 14751 output elements over the file had two admissible results. Each bar is asserted as
 stated above, not at the measured values.
 """
-import math
 import re
 from pathlib import Path
 
@@ -64,53 +63,19 @@ import torch
 
 from oracle import press_oracle as O
 from tests.conftest import ulp16_diff
-from tests.test_gpu_knorm_sweep import _bits, _same
-from tests.test_gpu_scorer_sweep import LAYOUTS, _gather, _layout, _name, assert_compress, assert_vs_ref64
+from tests.gpu_support import (assert_compress, assert_e_small, assert_keydiff_vs_ref, assert_rerotated, _bits, CHUNK,
+                               _gather, kd_chain, kd_chunks, kd_dpad, kd_groups, kd_lanes, keydiff_error_bound,
+                               keydiff_ref64, _layout, LAYOUTS, MERGE_THREADS, _name, _native, rope_inv_freq, _same)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
 CSRC = Path(__file__).resolve().parent.parent / "kvpress_b200" / "csrc"
 DTYPES = [torch.bfloat16, torch.float16]
-U32 = 2.0 ** -24
-MANT_BITS = {torch.bfloat16: 7, torch.float16: 10}
-MIN_EXP = {torch.bfloat16: -126, torch.float16: -14}
-E_SCALE_FRACTION = 2.0 ** -8  # max E_s of a row, as a share of its largest |score|
-CHUNK = 256  # kScoreChunk: positions per anchor / score CTA
-MERGE_THREADS = 1024  # kKdMergeThreads
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
 
 
 # ---------------------------------------------------------------------------------------------------
 # KeyDiff's launch shape (launch_keydiff_t, keydiff_merge_kernel)
 # ---------------------------------------------------------------------------------------------------
-def kd_lanes(D: int) -> int:
-    """LPR of keydiff_anchor_kernel / keydiff_score_kernel: lanes per key row"""
-    nvec = D // 8
-    return 4 if nvec <= 4 else 8 if nvec <= 8 else 16 if nvec <= 16 else 32
-
-
-def kd_dpad(D: int) -> int:
-    return 32 if D <= 32 else 64 if D <= 64 else 128 if D <= 128 else 256
-
-
-def kd_groups(D: int) -> int:
-    """G of keydiff_merge_kernel"""
-    return MERGE_THREADS // kd_dpad(D)
-
-
-def kd_chunks(S: int) -> int:
-    return (S + CHUNK - 1) // CHUNK
-
-
-def kd_chain(S: int, D: int) -> int:
-    """L: the longest addition chain of an anchor component (see the module docstring)"""
-    lpr, G = kd_lanes(D), kd_groups(D)
-    return lpr + int(math.log2(32 // lpr)) + 8 + (kd_chunks(S) + 4 * G - 1) // (4 * G) + 3 + 2 + G + 1
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -195,17 +160,6 @@ def test_sweep_reaches_every_keydiff_and_rerotation_instantiation():
 # ---------------------------------------------------------------------------------------------------
 # KeyDiff references and bars
 # ---------------------------------------------------------------------------------------------------
-def keydiff_ref64(k: torch.Tensor) -> torch.Tensor:
-    """anchor = mean_s k_s / max(||k_s||, 1e-12); score_s = -(k_s . a) / (max(||k_s||, 1e-8) max(||a||, 1e-8)),
-    in float64 on k's device, one batch at a time."""
-    out = []
-    for b in range(k.shape[0]):
-        kk = k[b].double()
-        n = kk.norm(dim=-1)
-        a = (kk / n.clamp_min(1e-12)[..., None]).mean(1)
-        an = a.norm(dim=-1).clamp_min(1e-8)
-        out.append(-(kk @ a[..., None])[..., 0] / (n.clamp_min(1e-8) * an[:, None]))
-    return torch.stack(out)
 
 
 def keydiff_ref32(k: torch.Tensor) -> torch.Tensor:
@@ -215,70 +169,6 @@ def keydiff_ref32(k: torch.Tensor) -> torch.Tensor:
     a = (kf / kn.clamp_min(1e-12)[..., None]).mean(2, keepdim=True)
     an = (a * a).sum(-1).sqrt().clamp_min(1e-8)
     return -((kf * a).sum(-1) / kn.clamp_min(1e-8) / an)
-
-
-def keydiff_error_bound(k: torch.Tensor, chain: int) -> torch.Tensor:
-    """E_s of the module docstring, [B, H, S] float64. Keys that are not finite, or whose fp32 sum of squares is not,
-    weigh nothing in the kernel's anchor (their rows are NaN, or their 1 / ||k|| is 0) and are left out."""
-    D = k.shape[-1]
-    out = []
-    for b in range(k.shape[0]):
-        kf = k[b].float()
-        live = torch.isfinite((kf * kf).sum(-1))
-        kk = torch.where(live[..., None], k[b].double(), 0.0)
-        n = kk.norm(dim=-1)
-        kh = kk / n.clamp_min(1e-12)[..., None]
-        a = kh.mean(1)
-        an = a.norm(dim=-1).clamp_min(1e-8)
-        m = kh.abs().mean(1)
-        den = n.clamp_min(1e-8) * an[:, None]
-        ref = (kk @ a[..., None])[..., 0].abs() / den
-        e_dot = (kk.abs() @ a.abs()[..., None])[..., 0] / den
-        e_anchor = (kk.abs() @ m[..., None])[..., 0] / den + ref * ((a.abs() * m).sum(-1) / an ** 2)[:, None]
-        out.append(U32 * ((D + 8) * e_dot + (chain + 16) * e_anchor + 24 * ref))
-    return torch.stack(out)
-
-
-def ulp16(x: torch.Tensor) -> torch.Tensor:
-    """float64 spacing of x's 16-bit format at |x|"""
-    e = torch.floor(torch.log2(x.double().abs())).clamp_min(MIN_EXP[x.dtype])
-    return torch.exp2(e - MANT_BITS[x.dtype])
-
-
-def assert_keydiff_vs_ref(got, ref, E, what: str, bias: bool = True, e_factor: float = 1.0) -> dict:
-    """The bar of the module docstring: NaN where ref is NaN; elsewhere <= 1 ulp of round16(ref) or within
-    ulp16(got) / 2 + e_factor E_s of ref; no row bias. Returns the measured statistics."""
-    dtype = got.dtype
-    nan = torch.isnan(ref)
-    assert torch.equal(torch.isnan(got), nan), f"{what}: NaN scores differ from the reference's"
-    r16 = torch.where(nan, 0.0, ref).to(dtype)
-    g = torch.where(nan, torch.zeros_like(got), got)
-    d = ulp16_diff(g, r16)
-    ok = d <= 1
-    e_arm = (g.double() - torch.where(nan, 0.0, ref)).abs() <= 0.5 * ulp16(g) + e_factor * E
-    bad = ~(ok | e_arm)
-    if bad.any():
-        i = bad.nonzero()[0].tolist()
-        raise AssertionError(f"{what}: {int(bad.sum())} scores beyond both arms, first at {i}: got {float(got[tuple(i)])} "
-                             f"ref {float(ref[tuple(i)])} E {float(E[tuple(i)]):.3e} ({int(d[tuple(i)])} ulp)")
-    only_e = ~ok
-    # positions the E arm decides enter the 1-ulp and bias bars at round16(ref); NaN rows are left out (0)
-    stats = assert_vs_ref64(torch.where(only_e, r16, g), torch.where(nan, 0.0, ref), torch.zeros(ref.shape[-1], dtype=torch.bool),
-                            what, bias=bias)
-    fin = ~nan
-    stats["e_only"] = float(only_e[fin].float().mean()) if fin.any() else 0.0
-    stats["max_e"] = float(E[fin].max()) if fin.any() else 0.0
-    print(f"[measured] {what}: share decided by the E arm {stats['e_only']:.2e}, max E_s {stats['max_e']:.2e}")
-    return stats
-
-
-def assert_e_small(E, ref, what: str):
-    """max E_s of every (b, h) row <= E_SCALE_FRACTION of its largest |score|"""
-    fin = torch.isfinite(ref)
-    scale = torch.where(fin, ref.abs(), 0.0).amax(-1)
-    worst = torch.where(fin, E, 0.0).amax(-1)
-    ok = worst <= E_SCALE_FRACTION * scale
-    assert ok.all(), f"{what}: E_s up to {float((worst / scale.clamp_min(1e-300)).max()):.2e} of the row's score scale"
 
 
 def _check_workspace(nat, k, v, n_kept, scorer):
@@ -544,55 +434,6 @@ def test_keydiff_graph_replay(dtype):
 # ---------------------------------------------------------------------------------------------------
 # 2. KeyRerotationPress
 # ---------------------------------------------------------------------------------------------------
-def rope_inv_freq(kind: str, D: int, seed: int = 0) -> torch.Tensor:
-    """fp32 [D / 2] as a model computes it"""
-    exps = torch.arange(0, D, 2, dtype=torch.int64).float() / D
-    if kind.startswith("theta"):
-        return 1.0 / (float(kind[5:]) ** exps)
-    if kind == "yarn_like":  # the low frequencies interpolated by up to 8x, the high ones kept
-        return 1.0 / (500000.0 ** exps) / torch.linspace(1.0, 8.0, D // 2)
-    # random_first_one: log-uniform over [1e-7, 1], descending, the first exactly 1
-    g = torch.Generator().manual_seed(seed)
-    inv = torch.exp2(-torch.rand(D // 2, generator=g) * 23.25).sort(descending=True).values
-    inv[0] = 1.0
-    return inv
-
-
-def _ulp32(x: torch.Tensor) -> torch.Tensor:
-    return torch.exp2(torch.floor(torch.log2(x.abs())).clamp_min(-126) - 23)
-
-
-def rerotation_admissible(k: torch.Tensor, idx: torch.Tensor, inv_freq: torch.Tensor) -> torch.Tensor:
-    """[4, B, H, n, D]: k[idx] rotated by (j - idx_j) * inv_freq with every admissible (cos16, sin16) pair."""
-    dtype, D = k.dtype, k.shape[-1]
-    g = _gather(k, idx)
-    delta = torch.arange(idx.shape[-1], device=k.device, dtype=torch.float32) - idx.float()  # exact below 2^24
-    ang = (delta[..., None] * inv_freq.to(k.device, torch.float32)).double()  # one fp32 multiply, as the kernel's
-    cands = []
-    for f in (torch.cos, torch.sin):
-        x = f(ang)
-        tol = 2 * _ulp32(x * (1 + 2.0 ** -20))  # sincosf: 2 ulp, in the larger binade at a binade edge
-        cands.append([((x - tol).float().to(dtype)), ((x + tol).float().to(dtype))])
-    out = []
-    for c in cands[0]:
-        for s in cands[1]:
-            out.append(g * torch.cat((c, c), -1) + O.rotate_half(g) * torch.cat((s, s), -1))
-    return torch.stack(out)
-
-
-def assert_rerotated(k, v, scores, n, inv_freq, out, what: str) -> int:
-    """canonical idx, exact V' gather, every K' element one of the admissible results; returns the count of elements
-    with more than one admissible result."""
-    k_out, v_out, idx = out
-    assert torch.equal(idx.long().cpu(), O.select_lowest_index_ties(scores.cpu(), n)), f"{what}: not the canonical selection"
-    assert _same(v_out, _gather(v, idx)), f"{what}: V' is not an exact gather"
-    adm = _bits(rerotation_admissible(k, idx, inv_freq))
-    hit = (adm == _bits(k_out)[None]).any(0)
-    if not hit.all():
-        i = (~hit).nonzero()[0].tolist()
-        raise AssertionError(f"{what}: {int((~hit).sum())} of {hit.numel()} K' elements not admissible, first at {i}: "
-                             f"got {float(k_out[tuple(i)])}, admissible {adm[(slice(None), *i)].view(k.dtype).tolist()}")
-    return int((adm != adm[:1]).any(0).sum())
 
 
 def rr_inputs(B, H, S, D, dtype, seed):

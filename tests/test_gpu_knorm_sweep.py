@@ -33,10 +33,8 @@ score on every path; at most 2e-4 of a case's positions at 1 ulp on the cluster 
 values.
 """
 import json
-import os
 import re
 import subprocess
-import sys
 from collections import namedtuple
 from pathlib import Path
 
@@ -45,7 +43,9 @@ import torch
 
 from oracle import press_oracle as O
 from tests.conftest import ulp16_diff
-from tests.test_gpu_scorer_sweep import LAYOUTS, _gather, _layout, _name, assert_compress, assert_vs_ref64
+from tests.abi_cases import PYTHON, child_env
+from tests.gpu_support import (assert_compress, assert_vs_ref64, _bits, _gather, knorm_ref64, _layout, LAYOUTS, _name,
+                               _native, _same)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
@@ -53,12 +53,6 @@ ROOT = Path(__file__).resolve().parent.parent
 CSRC = ROOT / "kvpress_b200" / "csrc"
 DTYPES = [torch.bfloat16, torch.float16]
 PATH_OF_LAUNCHES = {1: "cluster", 2: "fused", 3: "two_kernels"}
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -199,16 +193,6 @@ print(json.dumps(out))
 """
 
 
-def _child_env(**knobs) -> dict:
-    env = {k: v for k, v in os.environ.items() if not k.startswith("KVP_")}  # the library's knobs at their defaults
-    env.update(knobs)
-    return env
-
-
-def _python():
-    return [sys.executable, *(["-s"] if sys.flags.no_user_site else [])]
-
-
 def test_knorm_dispatch_matches_launch_count():
     """kvp_launches_per_compress (1 = cluster, 2 = fused, 3 = two kernels) agrees with knorm_dispatch on every case
     shape, and every case is listed under the path knorm_dispatch gives it. No device: a child process that sees none."""
@@ -216,8 +200,8 @@ def test_knorm_dispatch_matches_launch_count():
     for path, shape in cases:
         assert knorm_dispatch(*shape, torch.bfloat16).path == path, (path, shape)
     shapes = [s for _, s in cases]
-    r = subprocess.run([*_python(), "-c", _LAUNCHES_CHILD, str(ROOT / "kvpress_b200" / "native.py"), json.dumps(shapes)],
-                       cwd=ROOT, env=_child_env(CUDA_VISIBLE_DEVICES=""), capture_output=True, text=True, timeout=300)
+    r = subprocess.run([*PYTHON, "-c", _LAUNCHES_CHILD, str(ROOT / "kvpress_b200" / "native.py"), json.dumps(shapes)],
+                       cwd=ROOT, env=child_env(CUDA_VISIBLE_DEVICES=""), capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr[-4000:]
     got = json.loads(r.stdout.strip().splitlines()[-1])
     wrong = [(shape, PATH_OF_LAUNCHES[n], path) for (path, shape), n in zip(cases, got) if PATH_OF_LAUNCHES[n] != path]
@@ -263,9 +247,6 @@ def test_knorm_sweep_reaches_every_instantiation_and_regime():
 # ---------------------------------------------------------------------------------------------------
 # GPU helpers
 # ---------------------------------------------------------------------------------------------------
-def knorm_ref64(k: torch.Tensor) -> torch.Tensor:
-    """-sqrt(sum k^2) in float64 on the device, one batch at a time."""
-    return torch.stack([-(k[b].double() ** 2).sum(-1).sqrt() for b in range(k.shape[0])])
 
 
 def sweep_inputs(B, H, S, D, dtype, seed):
@@ -284,19 +265,6 @@ def n_kept_values(S: int):
 
 def _path(nat, k, v) -> str:
     return PATH_OF_LAUNCHES[nat.launches_per_compress(nat.make_problem(k, v, 1), nat.SCORER_KNORM)]
-
-
-def _bits(x: torch.Tensor) -> torch.Tensor:
-    return x.contiguous().view(torch.int16)
-
-
-def _same(a, b) -> bool:
-    """bitwise equal (None == None)"""
-    if a is None or b is None:
-        return a is None and b is None
-    if a.dtype in (torch.bfloat16, torch.float16):
-        return torch.equal(_bits(a), _bits(b))
-    return torch.equal(a, b)
 
 
 def _check_workspace(nat, k, v, n_kept):
@@ -534,9 +502,9 @@ def test_knorm_paths_agree_on_one_input(tmp_path):
     for path, knobs in CROSS_RUNS.items():
         out = tmp_path / f"{path}.pt"
         launches = {"cluster": 1, "fused": 2, "two_kernels": 3}[path]
-        r = subprocess.run([*_python(), "-c", _CROSS_CHILD, str(ROOT / "kvpress_b200" / "native.py"), str(out),
+        r = subprocess.run([*PYTHON, "-c", _CROSS_CHILD, str(ROOT / "kvpress_b200" / "native.py"), str(out),
                             str(launches), json.dumps(CROSS_SHAPES)],
-                           cwd=ROOT, env=_child_env(**knobs), capture_output=True, text=True, timeout=300)
+                           cwd=ROOT, env=child_env(**knobs), capture_output=True, text=True, timeout=300)
         assert r.returncode == 0, f"{path}: {r.stderr[-4000:]}"
         got[path] = torch.load(out)
     assert len(got["cluster"]) == 2 * 2 * len(CROSS_SHAPES)

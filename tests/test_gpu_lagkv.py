@@ -36,40 +36,14 @@ from transformers import DynamicCache
 from oracle import press_oracle as O
 from tests import lagkv_backend as LB
 from tests.conftest import ulp16_diff
-from tests.test_gpu_non_causal_attention import ulp_at
-from tests.test_gpu_scorer_sweep import assert_compress
-from tests.tiny_models import tiny_llama
+from tests.gpu_support import (assert_compress, gpu_ids, lagkv_inputs, _masked, _name, _native, _prefill, same16,
+                               _shared, tiny_gpu_llama, ulp_at)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
 U = 2.0 ** -24
 LAG_MAX = 1024
 ROOT = Path(__file__).resolve().parent.parent
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
-
-
-def same(a: torch.Tensor, b: torch.Tensor) -> bool:
-    """Bitwise equality of two 16-bit tensors (torch.equal is False wherever both hold NaN)."""
-    return a.shape == b.shape and torch.equal(a.view(torch.int16), b.view(torch.int16))
-
-
-def _name(dtype) -> str:
-    return "bf16" if dtype == torch.bfloat16 else "fp16"
-
-
-def inputs(B, H, S, D, dtype, seed, scale=1.0):
-    """Gaussian K and V, with a per-row scale that spreads log-normally (the rows of a real cache differ in norm)."""
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    k = (scale * torch.exp(0.3 * torch.randn((B, H, S, 1), generator=g, device=DEV))
-         * torch.randn((B, H, S, D), generator=g, device=DEV)).to(dtype)
-    v = (scale * torch.exp(0.3 * torch.randn((B, H, S, 1), generator=g, device=DEV))
-         * torch.randn((B, H, S, D), generator=g, device=DEV)).to(dtype)
-    return k, v
 
 
 # --------------------------------------------------------------------------------------------------
@@ -136,7 +110,7 @@ def check(k, v, n_sink: int, L: int, cross: bool, sc, what: str, bias: bool = Tr
     dtype = sc.dtype
     want = LB.lagkv_score(k, v, n_sink, L, cross)
     if LB.is_short(S, n_sink, L):
-        assert same(sc, want), f"{what}: short cache differs"
+        assert same16(sc, want), f"{what}: short cache differs"
         return {}
     P = (S - n_sink) // L
     a, b = n_sink, n_sink + (P - 1) * L
@@ -186,11 +160,11 @@ def run(k, v, n_sink, L, cross, what, n_kept=None, bias=True):
     S = k.shape[2]
     sc = nat.lagkv_score(k, v, n_sink, L, cross)
     check(k, v, n_sink, L, cross, sc, what, bias=bias)
-    assert same(nat.lagkv_score(k, v, n_sink, L, cross), sc), f"{what}: two calls differ"
+    assert same16(nat.lagkv_score(k, v, n_sink, L, cross), sc), f"{what}: two calls differ"
     n_kept = max(1, O.kept_count(S, 0.5)) if n_kept is None else n_kept
     k_out, v_out, idx, sc2 = nat.lagkv_compress(k, v, n_sink, L, cross, n_kept, return_indices=True,
                                                 return_scores=True)
-    assert same(sc2, sc), f"{what}: compress scores differ from the score call"
+    assert same16(sc2, sc), f"{what}: compress scores differ from the score call"
     assert_compress(k, v, k_out, v_out, idx, sc2, n_kept)
     return sc
 
@@ -222,7 +196,7 @@ def test_sweep_reaches_every_instantiation():
 @pytest.mark.parametrize("dtype,D,cross", SWEEP, ids=[f"{_name(dt)}-d{D}-{'cross' if c else 'rank'}"
                                                        for dt, D, c in SWEEP])
 def test_instantiations(dtype, D, cross):
-    k, v = inputs(1, 2, 4 + 12 * 128 + 37, D, dtype, seed=D + 7 * cross)
+    k, v = lagkv_inputs(1, 2, 4 + 12 * 128 + 37, D, dtype, seed=D + 7 * cross)
     run(k, v, 4, 128, cross, f"lagkv {_name(dtype)} d{D} cross={cross}")
 
 
@@ -236,7 +210,7 @@ def test_lag_sizes(L, cross):
     dtype = (torch.bfloat16, torch.float16)[LAGS.index(L) % 2]
     n_parts = 6 if L >= 100 else 40
     S = 4 + n_parts * L + L // 3
-    k, v = inputs(2, 2, S, 128, dtype, seed=L)
+    k, v = lagkv_inputs(2, 2, S, 128, dtype, seed=L)
     sc = run(k, v, 4, L, cross, f"lagkv L{L} cross={cross}")
     if L == 1:  # one-row reference partitions: every scored partition is NaN
         scored = sc[..., 4:4 + (n_parts - 1)]
@@ -262,7 +236,7 @@ EDGES = _edges()
 def test_sequence_edges(S, n_sink, L, cross):
     i = EDGES.index((S, n_sink, L))
     dtype, D, _ = SWEEP[(5 * i) % len(SWEEP)]
-    k, v = inputs(1, 3, S, D, dtype, seed=1000 + i)
+    k, v = lagkv_inputs(1, 3, S, D, dtype, seed=1000 + i)
     run(k, v, n_sink, L, cross, f"lagkv {_name(dtype)} d{D} S{S} sink{n_sink} L{L}", n_kept=max(1, S // 3),
         bias=False)
 
@@ -272,7 +246,7 @@ def test_sequence_edges(S, n_sink, L, cross):
 @pytest.mark.parametrize("S", [4096, 16384, 32768, 131072])
 def test_llama_layer_shape(S, cross):
     """The Llama-3.1-8B layer shape [1, 8, S, 128] bf16 with the reference defaults, up to 128k."""
-    k, v = inputs(1, 8, S, 128, torch.bfloat16, seed=S % 997)
+    k, v = lagkv_inputs(1, 8, S, 128, torch.bfloat16, seed=S % 997)
     run(k, v, 4, 128, cross, f"lagkv llama8b S{S}", n_kept=O.kept_count(S, 0.5))
 
 
@@ -280,12 +254,12 @@ def test_llama_layer_shape(S, cross):
 def test_thousands_of_rows_and_a_row_alone():
     """B Hkv = 3000: a row's scores are bitwise those of the same row scored alone."""
     nat = _native()
-    k, v = inputs(3, 1000, 4 + 9 * 32 + 5, 64, torch.float16, seed=3)
+    k, v = lagkv_inputs(3, 1000, 4 + 9 * 32 + 5, 64, torch.float16, seed=3)
     for cross in (False, True):
         sc = run(k, v, 4, 32, cross, f"lagkv 3000 rows cross={cross}")
         for b, h in ((0, 0), (1, 517), (2, 999)):
             alone = nat.lagkv_score(k[b:b + 1, h:h + 1].contiguous(), v[b:b + 1, h:h + 1].contiguous(), 4, 32, cross)
-            assert same(alone[0, 0], sc[b, h])
+            assert same16(alone[0, 0], sc[b, h])
 
 
 # --------------------------------------------------------------------------------------------------
@@ -298,7 +272,7 @@ def test_degenerate_partitions(cross):
     channel everywhere makes every scored partition of that head NaN; an all-equal partition ranks by position."""
     nat = _native()
     L, n_sink = 32, 4
-    k, v = inputs(1, 3, n_sink + 8 * L + 9, 64, torch.bfloat16, seed=21)
+    k, v = lagkv_inputs(1, 3, n_sink + 8 * L + 9, 64, torch.bfloat16, seed=21)
     k[0, 0, n_sink + 3 * L:n_sink + 4 * L, 17] = 0.5
     v[0, 1, :, 40] = 0
     k[0, 2, n_sink + 5 * L:n_sink + 6 * L] = k[0, 2, n_sink + 5 * L]
@@ -323,12 +297,12 @@ def test_nan_input_propagates_like_torch_min_max(cross):
     the reference of are NaN, as torch.min / max carry the NaN into lo / hi."""
     nat = _native()
     L, n_sink = 32, 4
-    k, v = inputs(1, 2, n_sink + 8 * L + 9, 64, torch.bfloat16, seed=23)
+    k, v = lagkv_inputs(1, 2, n_sink + 8 * L + 9, 64, torch.bfloat16, seed=23)
     k[0, 0, n_sink + 4 * L + 5, 11] = float("nan")
     v[0, 1, n_sink + 2 * L + 30, 60] = float("nan")
     sc = nat.lagkv_score(k, v, n_sink, L, cross)
     check(k, v, n_sink, L, cross, sc, f"lagkv NaN input cross={cross}", bias=False)
-    assert same(nat.lagkv_score(k, v, n_sink, L, cross), sc)
+    assert same16(nat.lagkv_score(k, v, n_sink, L, cross), sc)
     ramp = (torch.arange(L, device=DEV, dtype=torch.float32) / L).to(sc.dtype)
     for h, p in ((0, 4), (1, 2)):
         for c in (p - 1, p):
@@ -342,7 +316,7 @@ def test_nan_input_propagates_like_torch_min_max(cross):
 def test_planted_ties_rank_by_position():
     """Duplicate (k, v) rows inside a partition get equal c: they rank in position order, exactly."""
     L, n_sink = 64, 4
-    k, v = inputs(2, 2, n_sink + 6 * L + 3, 128, torch.bfloat16, seed=5)
+    k, v = lagkv_inputs(2, 2, n_sink + 6 * L + 3, 128, torch.bfloat16, seed=5)
     p0 = n_sink + 2 * L
     dup = [p0 + 3, p0 + 10, p0 + 40, p0 + 63]
     k[:, :, dup], v[:, :, dup] = k[:, :, p0 + 20:p0 + 21], v[:, :, p0 + 20:p0 + 21]
@@ -357,7 +331,7 @@ def test_planted_ties_rank_by_position():
 @gpu
 @pytest.mark.parametrize("cross", [False, True], ids=["rank", "cross"])
 def test_fp16_near_the_top_of_the_range(cross):
-    k, v = inputs(1, 2, 4 + 10 * 128, 128, torch.float16, seed=8, scale=1.0)
+    k, v = lagkv_inputs(1, 2, 4 + 10 * 128, 128, torch.float16, seed=8, scale=1.0)
     k = (k.float() / k.float().abs().amax() * 65000).half()
     v = (v.float() / v.float().abs().amax() * 60000).half()
     assert torch.isfinite(k).all() and torch.isfinite(v).all()
@@ -372,7 +346,7 @@ def test_fp16_near_the_top_of_the_range(cross):
 def test_layouts(layout):
     nat = _native()
     B, H, S, D = 2, 4, 3000, 128
-    k, v = inputs(B, H, S, D, torch.bfloat16, seed=7)
+    k, v = lagkv_inputs(B, H, S, D, torch.bfloat16, seed=7)
     if layout == "strided":  # rows of D within rows of D + 64
         kb = torch.zeros((B, H, S, D + 64), dtype=k.dtype, device=DEV)
         vb = torch.zeros_like(kb)
@@ -386,7 +360,7 @@ def test_layouts(layout):
         assert not k.is_contiguous() and nat._rows_ok(k)
     for cross in (False, True):
         sc = run(k, v, 4, 128, cross, f"lagkv {layout}")
-        assert same(sc, nat.lagkv_score(k.contiguous(), v.contiguous(), 4, 128, cross))
+        assert same16(sc, nat.lagkv_score(k.contiguous(), v.contiguous(), 4, 128, cross))
 
 
 def scoring_items(R: int, n_scored: int, sm: int) -> int:
@@ -406,7 +380,7 @@ def test_schedule_regimes(regime):
     assert (items < sm, items == sm, items > sm)[["fewer", "equal", "more"].index(regime)], (items, sm)
     L = 16
     S = 4 + (n_scored + 1) * L + 3
-    k, v = inputs(1, R, S, 64, torch.float16, seed=n_scored)
+    k, v = lagkv_inputs(1, R, S, 64, torch.float16, seed=n_scored)
     for cross in (False, True):
         run(k, v, 4, L, cross, f"lagkv schedule {regime} ({items} items, {sm} SMs)")
 
@@ -417,7 +391,7 @@ def test_schedule_regimes(regime):
 @gpu
 def test_compress_edges_and_n_kept_zero():
     nat = _native()
-    k, v = inputs(2, 2, 4 + 5 * 128 + 50, 64, torch.bfloat16, seed=12)
+    k, v = lagkv_inputs(2, 2, 4 + 5 * 128 + 50, 64, torch.bfloat16, seed=12)
     S = k.shape[2]
     for cross in (False, True):
         for n_kept in (1, S):
@@ -439,21 +413,21 @@ def test_compress_edges_and_n_kept_zero():
 @gpu
 def test_replays_under_capture_and_workspace_check():
     nat = _native()
-    k, v = inputs(1, 8, 8000, 128, torch.bfloat16, seed=9)
+    k, v = lagkv_inputs(1, 8, 8000, 128, torch.bfloat16, seed=9)
     eager = nat.lagkv_compress(k, v, 4, 128, False, 4000, True, True)
     again = nat.lagkv_compress(k, v, 4, 128, False, 4000, True, True)
-    assert all(same(a, b) for a, b in zip(eager, again))
+    assert all(same16(a, b) for a, b in zip(eager, again))
     g = nat.capture(lambda: (nat.lagkv_score(k, v, 4, 128, True), *nat.lagkv_compress(k, v, 4, 128, False, 4000,
                                                                                          True, True)))
     out = g.replay()
     torch.cuda.synchronize()
-    assert all(same(a, b) for a, b in zip(out[1:], eager))
+    assert all(same16(a, b) for a, b in zip(out[1:], eager))
     k.copy_(torch.randn_like(k.float()).to(k.dtype))  # inputs updated in place
     v.mul_(-1)
     out = g.replay()
     torch.cuda.synchronize()
     fresh = (nat.lagkv_score(k, v, 4, 128, True), *nat.lagkv_compress(k, v, 4, 128, False, 4000, True, True))
-    assert all(same(a, b) for a, b in zip(out, fresh))
+    assert all(same16(a, b) for a, b in zip(out, fresh))
     assert not torch.equal(out[3], eager[2])
     p = nat.make_problem(k, v, 4000)
     nat.workspace_check(p, nat.SCORER_LAGKV, nat._workspace(p, nat.SCORER_LAGKV, k.device))
@@ -464,7 +438,7 @@ def test_no_intermediate_at_128k():
     """Memory grows by no more than the workspace and the outputs: no cache-sized temporary."""
     nat = _native()
     B, H, S, D = 1, 8, 131072, 128
-    k, v = inputs(B, H, S, D, torch.bfloat16, seed=10)
+    k, v = lagkv_inputs(B, H, S, D, torch.bfloat16, seed=10)
     n_kept = S // 2
     p = nat.make_problem(k, v, n_kept)
     ws = nat.workspace_bytes(p, nat.SCORER_LAGKV)
@@ -487,7 +461,7 @@ def test_unsupported_lag_and_the_press_fallback():
 
     nat = _native()
     L = LAG_MAX + 1
-    k, v = inputs(1, 2, 4 + 4 * L + 11, 64, torch.bfloat16, seed=4)
+    k, v = lagkv_inputs(1, 2, 4 + 4 * L + 11, 64, torch.bfloat16, seed=4)
     with pytest.raises(RuntimeError, match="unsupported shape"):
         nat.lagkv_score(k, v, 4, L, False)
     with pytest.raises(RuntimeError, match="bad argument"):
@@ -508,15 +482,6 @@ def test_unsupported_lag_and_the_press_fallback():
 # --------------------------------------------------------------------------------------------------
 # presses on a GPU tiny Llama, every native call checked against the float64 definition
 # --------------------------------------------------------------------------------------------------
-def _model(head_dim=64):
-    model = tiny_llama(dtype=torch.bfloat16, device=DEV, head_dim=head_dim, heads=8, kv_heads=2)
-    model.config._attn_implementation = "sdpa"
-    return model
-
-
-def _ids(n=240):
-    g = torch.Generator().manual_seed(11)
-    return torch.stack([torch.randperm(250, generator=g)[:n] + 2 for _ in range(2)]).to(DEV)
 
 
 @pytest.fixture
@@ -545,16 +510,12 @@ def checked(monkeypatch):
     return calls
 
 
-def _prefill(ids):
-    return lambda model, cache: model.model(input_ids=ids, past_key_values=cache)
-
-
 def _standin(press_factory, forward, monkeypatch):
     """(model, cache) the same press leaves, run through `forward`, with the float64 stand-ins in place of the
     kernels."""
     with monkeypatch.context() as m:
         LB.install(m)
-        model, cache = _model(), DynamicCache()
+        model, cache = tiny_gpu_llama(), DynamicCache()
         with press_factory()(model):
             forward(model, cache)
     return model, cache
@@ -565,30 +526,14 @@ def _standin_rows(press_factory, ids, monkeypatch):
     return _standin(press_factory, _prefill(ids), monkeypatch)[1]
 
 
-def _shared(a: DynamicCache, b: DynamicCache) -> float:
-    """Fraction of the value rows of `a` that `b` holds too, per head (values are gathered as they are under every
-    press, keys may be re-rotated)."""
-    hits = total = 0
-    for la, lb in zip(a.layers, b.layers):
-        va, vb = la.values.float(), lb.values.float()
-        same = (va[..., :, None, :] == vb[..., None, :, :]).all(dim=-1).any(dim=-1)
-        hits, total = hits + int(same.sum()), total + same.numel()
-    return hits / total
-
-
-def _masked(model) -> list:
-    """Per layer, the set of (b, h, s) an AdaKVPress masked."""
-    return [set(zip(*(t.tolist() for t in layer.self_attn.masked_key_indices))) for layer in model.model.layers]
-
-
 @gpu
 @pytest.mark.parametrize("cross", [False, True], ids=["rank", "cross"])
 def test_press_on_a_tiny_llama(checked, monkeypatch, cross):
     from kvpress_b200 import LagKVPress
 
-    ids = _ids()
+    ids = gpu_ids()
     factory = lambda: LagKVPress(compression_ratio=0.5, lag_size=16, cross_scoring=cross)  # noqa: E731
-    model, cache = _model(), DynamicCache()
+    model, cache = tiny_gpu_llama(), DynamicCache()
     with factory()(model):
         model.model(input_ids=ids, past_key_values=cache)
     assert cache.get_seq_length() == 120 and checked == [("compress", 240)] * 2
@@ -602,8 +547,8 @@ def test_wrapper_presses_on_a_tiny_llama(checked, monkeypatch):
     its threshold (97 % of the masked positions or kept rows shared)."""
     from kvpress_b200 import AdaKVPress, ChunkPress, DecodingPress, KeyRerotationPress, LagKVPress
 
-    ids = _ids()
-    model = _model()
+    ids = gpu_ids()
+    model = tiny_gpu_llama()
     cache = DynamicCache()
     ada = lambda: AdaKVPress(LagKVPress(compression_ratio=0.5, lag_size=16, cross_scoring=True))  # noqa: E731
     with ada()(model):

@@ -31,76 +31,16 @@ import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 from transformers import DynamicCache
 
 from oracle import press_oracle as O
 from tests import non_causal_attention_backend as NB
-from tests.test_gpu_scorer_sweep import assert_compress, ulp16_diff
-from tests.tiny_models import tiny_llama
+from tests.gpu_support import (assert_compress, gpu_ids, _name, _native, nca_inputs, nca_ref, _sm_count,
+                               tiny_gpu_llama, ulp16_diff, ulp_at)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
-U = 2.0 ** -24
 L2E = 1.0 / math.log(2.0)
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
-
-
-def _sm_count() -> int:
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _name(dtype) -> str:
-    return "bf16" if dtype == torch.bfloat16 else "fp16"
-
-
-def inputs(B, Hkv, G, S, D, dtype, seed, negative_tail: bool = False):
-    """Unscaled logits q.k of standard deviation about 6 (chunk maxima of 20-25, within the 10-100 of real layers) and
-    value rows whose norms spread log-normally, as real caches' do (a near-constant ||v|| makes the z-score
-    ill-conditioned: its std is then small against its mean). With `negative_tail`, every logit of the last chunk's
-    valid rows is -D, so the padded keys take almost all of their mass."""
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    sig = 6 ** 0.5 / D ** 0.25
-    k = (sig * torch.randn((B, Hkv, S, D), generator=g, device=DEV)).to(dtype)
-    scale = torch.exp(0.7 * torch.randn((B, Hkv, S, 1), generator=g, device=DEV))
-    v = (scale * torch.randn((B, Hkv, S, D), generator=g, device=DEV)).to(dtype)
-    q = (sig * torch.randn((B, Hkv * G, S, D), generator=g, device=DEV)).to(dtype)
-    if negative_tail:
-        cs = 256
-        s0 = (S - 1) // cs * cs
-        k[:, :, s0:] = 1.0
-        q[:, :, s0:] = -1.0
-    return k, v, q
-
-
-def ulp_at(z: torch.Tensor, dtype) -> torch.Tensor:
-    """Spacing of the 16-bit dtype at |z| (its subnormal spacing below the normal range)."""
-    mant, emin = (7, -126) if dtype == torch.bfloat16 else (10, -14)
-    e = torch.floor(torch.log2(z.abs().clamp_min(2.0 ** emin)))
-    return torch.exp2(e - mant)
-
-
-def error_bound(x64, tau, z64, chunk_size: int, D: int, G: int) -> torch.Tensor:
-    """E_s of the module docstring, per position."""
-    B, Hkv, S = x64.shape
-    cs = chunk_size
-    gamma = (D + 1) * U
-    tau_s = tau.repeat_interleave(cs, dim=-1)[..., :S]
-    dz = gamma * tau_s + 4 * U * tau_s + 2.0 ** -22 + cs * U
-    dp_rel = gamma * tau_s + dz + 4 * U * tau_s + 4 * U * math.log2(cs) + 2.0 ** -22
-    eps_x = dp_rel + (cs * G + 2) * U + (D + 4) * U
-    pooled = F.avg_pool1d(x64, 3, padding=1, stride=1)
-    dp = F.avg_pool1d(eps_x * x64.abs(), 3, padding=1, stride=1) + 3 * U * pooled.abs()
-    e = float(eps_x.max()) + 3 * U
-    std = max(float(pooled.std()), 1e-6)
-    d_mean = e * float(pooled.abs().mean())
-    d_std = e * float(pooled.pow(2).mean().sqrt())
-    return 1.01 * ((dp + d_mean) / std + z64.abs() * d_std / std)
 
 
 def assert_vs_z64(got, z64, E, what: str, bias: bool = True) -> dict:
@@ -123,21 +63,12 @@ def assert_vs_z64(got, z64, E, what: str, bias: bool = True) -> dict:
     return stats
 
 
-def ref(k, v, q, cs):
-    B, Hkv, S, D = k.shape
-    G = q.shape[1] // Hkv
-    block = max(1, (1 << 25) // (B * q.shape[1] * cs * cs))
-    x64, tau = NB.non_causal_attention_parts64(k, v, q, cs, block=block, with_bound=True)
-    z64 = NB.zscore64(x64)
-    return z64, error_bound(x64, tau, z64, cs, D, G)
-
-
 def run(k, v, q, cs, what, n_kept=None, bias=True):
     """score and compress of one problem, both checked against fp64; returns (scores, z64)."""
     nat = _native()
     S = k.shape[2]
     sc = nat.non_causal_attention_score(k, v, q, cs)
-    z64, E = ref(k, v, q, cs)
+    z64, E = nca_ref(k, v, q, cs)
     assert_vs_z64(sc, z64, E, what, bias=bias)
     assert torch.equal(nat.non_causal_attention_score(k, v, q, cs), sc), f"{what}: two calls differ"
     n_kept = max(1, O.kept_count(S, 0.5)) if n_kept is None else n_kept
@@ -158,7 +89,7 @@ SWEEP = [(dt, D, cs, G) for dt in (torch.bfloat16, torch.float16) for D in (64, 
 @gpu
 @pytest.mark.parametrize("dtype,D,cs,G", SWEEP, ids=[f"{_name(dt)}-d{D}-cs{cs}-g{G}" for dt, D, cs, G in SWEEP])
 def test_instantiations(dtype, D, cs, G):
-    k, v, q = inputs(1, 2, G, 1000, D, dtype, seed=G * 10 + D + cs)
+    k, v, q = nca_inputs(1, 2, G, 1000, D, dtype, seed=G * 10 + D + cs)
     run(k, v, q, cs, f"nca {_name(dtype)} d{D} cs{cs} g{G}")
 
 
@@ -170,7 +101,7 @@ EDGES = sorted({(S, cs) for cs in (128, 256) for S in (1, 2, cs - 1, cs, cs + 1,
 def test_sequence_edges(S, cs):
     i = EDGES.index((S, cs))
     dtype, D, _, G = SWEEP[(7 * i) % len(SWEEP)]  # spread the instantiations over the edges
-    k, v, q = inputs(1, 2, G, S, D, dtype, seed=100 + i)
+    k, v, q = nca_inputs(1, 2, G, S, D, dtype, seed=100 + i)
     run(k, v, q, cs, f"nca {_name(dtype)} d{D} g{G} S{S} cs{cs}", bias=S >= 1000)
 
 
@@ -178,7 +109,7 @@ def test_sequence_edges(S, cs):
 @pytest.mark.parametrize("S", [32768, 131072])
 def test_long(S):
     """The Llama-3.1-8B layer shape (Hkv 8, G 4, D 128, cs 256) at 32k and 128k."""
-    k, v, q = inputs(1, 8, 4, S, 128, torch.bfloat16, seed=S % 1000)
+    k, v, q = nca_inputs(1, 8, 4, S, 128, torch.bfloat16, seed=S % 1000)
     run(k, v, q, 256, f"nca llama8b S{S}", n_kept=O.kept_count(S, 0.7))
 
 
@@ -188,7 +119,7 @@ def test_padded_keys_take_the_mass(S):
     """Every logit of the last chunk's valid rows is below -100: the unmasked padded keys (logit 0) take their mass and
     the valid keys keep little beyond the padded query rows' pad / cs."""
     cs = 256
-    k, v, q = inputs(1, 2, 2, S, 128, torch.bfloat16, seed=S, negative_tail=True)
+    k, v, q = nca_inputs(1, 2, 2, S, 128, torch.bfloat16, seed=S, negative_tail=True)
     sc, z64 = run(k, v, q, cs, f"nca negative tail S{S}", bias=False)
     x64 = NB.non_causal_attention_parts64(k, v, q, cs)
     s0 = (S - 1) // cs * cs
@@ -221,7 +152,7 @@ def test_constant_x_clamps_the_std():
 def test_batch_couples_the_rows():
     """B = 3: mean and std run over the whole batch, so each sequence's scores depend on the others."""
     nat = _native()
-    k, v, q = inputs(3, 2, 4, 1500, 128, torch.bfloat16, seed=33)
+    k, v, q = nca_inputs(3, 2, 4, 1500, 128, torch.bfloat16, seed=33)
     v[1] *= 4
     sc, _ = run(k, v, q, 256, "nca batch3")
     alone = nat.non_causal_attention_score(k[:1].contiguous(), v[:1].contiguous(), q[:1].contiguous(), 256)
@@ -236,7 +167,7 @@ def test_batch_couples_the_rows():
 def test_layouts(layout):
     nat = _native()
     B, Hkv, G, S, D = 2, 2, 4, 1500, 128
-    k, v, q = inputs(B, Hkv, G, S, D, torch.bfloat16, seed=7)
+    k, v, q = nca_inputs(B, Hkv, G, S, D, torch.bfloat16, seed=7)
     if layout == "strided":  # rows of D within rows of D + 64, for K and V
         kb = torch.zeros((B, Hkv, S, D + 64), dtype=k.dtype, device=DEV)
         vb = torch.zeros_like(kb)
@@ -262,7 +193,7 @@ def test_schedule_regimes(regime):
     S = chunks * 128 - 5
     items = R * -(-S // 128)
     assert (items < sm, items == sm, items > sm)[["fewer", "equal", "more"].index(regime)]
-    k, v, q = inputs(1, R, 2, S, 64, torch.float16, seed=chunks)
+    k, v, q = nca_inputs(1, R, 2, S, 64, torch.float16, seed=chunks)
     run(k, v, q, 128, f"nca schedule {regime} ({items} items, {sm} SMs)")
 
 
@@ -270,7 +201,7 @@ def test_schedule_regimes(regime):
 def test_unsupported_shapes_and_arguments():
     nat = _native()
     for G, D, cs in ((16, 128, 256), (2, 96, 256), (2, 128, 64), (2, 128, 512)):
-        k, v, q = inputs(1, 2, G, 300, D, torch.bfloat16, seed=1)
+        k, v, q = nca_inputs(1, 2, G, 300, D, torch.bfloat16, seed=1)
         with pytest.raises(RuntimeError, match="unsupported shape"):
             nat.non_causal_attention_score(k, v, q, cs)
     with pytest.raises(RuntimeError, match="bad argument"):
@@ -283,7 +214,7 @@ def test_unsupported_shapes_and_arguments():
 @gpu
 def test_replays_under_capture_and_workspace_check():
     nat = _native()
-    k, v, q = inputs(1, 4, 4, 3000, 128, torch.bfloat16, seed=9)
+    k, v, q = nca_inputs(1, 4, 4, 3000, 128, torch.bfloat16, seed=9)
     eager = nat.non_causal_attention_compress(k, v, q, 256, 1500, True, True)
     g = nat.capture(lambda: (nat.non_causal_attention_score(k, v, q, 256),
                              *nat.non_causal_attention_compress(k, v, q, 256, 1500, True, True)))
@@ -304,7 +235,7 @@ def test_no_intermediate_at_128k():
     """Memory grows by no more than the workspace and the outputs: no cs x cs tensor."""
     nat = _native()
     B, Hkv, G, S, D = 1, 8, 4, 131072, 128
-    k, v, q = inputs(B, Hkv, G, S, D, torch.bfloat16, seed=10)
+    k, v, q = nca_inputs(B, Hkv, G, S, D, torch.bfloat16, seed=10)
     n_kept = S // 2
     p = nat.make_problem(k, v, n_kept, Hkv * G)
     ws = nat.workspace_bytes(p, nat.SCORER_NON_CAUSAL_ATTENTION)
@@ -322,15 +253,6 @@ def test_no_intermediate_at_128k():
 # --------------------------------------------------------------------------------------------------
 # the press on GPU tiny Llamas (head_dim 64 and 128)
 # --------------------------------------------------------------------------------------------------
-def _model(head_dim):
-    model = tiny_llama(dtype=torch.bfloat16, device=DEV, head_dim=head_dim, heads=8, kv_heads=2)
-    model.config._attn_implementation = "sdpa"
-    return model
-
-
-def _ids(n=240):
-    g = torch.Generator().manual_seed(11)
-    return torch.stack([torch.randperm(250, generator=g)[:n] + 2 for _ in range(2)]).to(DEV)
 
 
 @gpu
@@ -338,13 +260,13 @@ def _ids(n=240):
 def test_press_adakv_and_key_rerotation_on_a_tiny_llama(monkeypatch, head_dim):
     from kvpress_b200 import AdaKVPress, KeyRerotationPress, NonCausalAttnPress, native
 
-    model, ids = _model(head_dim), _ids()
+    model, ids = tiny_gpu_llama(head_dim), gpu_ids()
     calls = []
     real = native.non_causal_attention_compress
 
     def checked(keys, values, q, cs, n_kept, return_indices=False, return_scores=False):
         k_out, v_out, idx, sc = real(keys, values, q, cs, n_kept, True, True)
-        z64, E = ref(keys, values, q, cs)
+        z64, E = nca_ref(keys, values, q, cs)
         assert_vs_z64(sc, z64, E, "press call", bias=False)
         assert_compress(keys, values, k_out, v_out, idx, sc, n_kept)
         calls.append(q.shape[2])
@@ -372,7 +294,7 @@ def test_press_adakv_and_key_rerotation_on_a_tiny_llama(monkeypatch, head_dim):
 def test_decoding_press_fails_like_the_reference():
     from kvpress_b200 import DecodingPress, NonCausalAttnPress
 
-    model, ids = _model(64), _ids()
+    model, ids = tiny_gpu_llama(64), gpu_ids()
     cache = DynamicCache()
     with pytest.raises(AssertionError, match="only supports prefill"):
         with DecodingPress(NonCausalAttnPress(), compression_interval=4, target_size=100)(model):

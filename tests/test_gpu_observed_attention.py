@@ -13,39 +13,11 @@ from transformers import DynamicCache
 
 from oracle import press_oracle as O
 from tests import observed_attention_backend as OB
-from tests.test_gpu_scorer_sweep import assert_compress, assert_vs_ref64
-from tests.tiny_models import tiny_llama
+from tests.gpu_support import (assert_compress, assert_vs_ref64, gpu_ids, _name, _native, oa_inputs, oa_ref64,
+                               _sm_count, tiny_gpu_llama)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
-
-
-def _sm_count() -> int:
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _name(dtype) -> str:
-    return "bf16" if dtype == torch.bfloat16 else "fp16"
-
-
-def inputs(B, Hkv, G, S, n_q, D, dtype, seed, q_scale=1.5):
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    k = torch.randn((B, Hkv, S, D), generator=g, device=DEV).to(dtype)
-    v = torch.randn((B, Hkv, S, D), generator=g, device=DEV).to(dtype)
-    q = (q_scale * torch.randn((B, Hkv * G, n_q, D), generator=g, device=DEV)).to(dtype)
-    return k, v, q
-
-
-def ref64(k, q, scaling):
-    B, Hkv, S, _ = k.shape
-    block = max(1, (1 << 26) // (B * q.shape[1] * S))
-    return OB.observed_attention_scores64(k, q, scaling, block=block)
 
 
 def run(k, v, q, scaling, what, n_kept=None, bias=True):
@@ -53,7 +25,7 @@ def run(k, v, q, scaling, what, n_kept=None, bias=True):
     nat = _native()
     S = k.shape[2]
     sc = nat.observed_attention_score(k, q, scaling)
-    ref = ref64(k, q, scaling)
+    ref = oa_ref64(k, q, scaling)
     assert_vs_ref64(sc, ref, torch.zeros(S, dtype=torch.bool), what, ftz=True, bias=bias)
     assert torch.equal(nat.observed_attention_score(k, q, scaling), sc), f"{what}: two calls differ"
     n_kept = max(1, O.kept_count(S, 0.5)) if n_kept is None else n_kept
@@ -73,7 +45,7 @@ SWEEP = [(dt, D, G) for dt in (torch.bfloat16, torch.float16) for D in (64, 128)
 @gpu
 @pytest.mark.parametrize("dtype,D,G", SWEEP, ids=[f"{_name(dt)}-d{D}-g{G}" for dt, D, G in SWEEP])
 def test_instantiations(dtype, D, G):
-    k, v, q = inputs(1, 2, G, 1000, 1000, D, dtype, seed=G * 10 + D)
+    k, v, q = oa_inputs(1, 2, G, 1000, 1000, D, dtype, seed=G * 10 + D)
     run(k, v, q, D ** -0.5, f"obs {_name(dtype)} d{D} g{G}")
 
 
@@ -86,13 +58,13 @@ EDGES = [(S, n_q) for S in (1, 2, 127, 128, 129, 255, 256, 257, 1000, 4097, 1638
 def test_sequence_and_query_edges(S, n_q):
     i = EDGES.index((S, n_q))
     dtype, D, G = SWEEP[(5 * i) % len(SWEEP)]  # spread the instantiations over the edges
-    k, v, q = inputs(1, 2, G, S, n_q, D, dtype, seed=i)
+    k, v, q = oa_inputs(1, 2, G, S, n_q, D, dtype, seed=i)
     run(k, v, q, D ** -0.5, f"obs {_name(dtype)} d{D} g{G} S{S} n_q{n_q}")
 
 
 @gpu
 def test_32k():
-    k, v, q = inputs(1, 2, 4, 32768, 32768, 128, torch.bfloat16, seed=32)
+    k, v, q = oa_inputs(1, 2, 4, 32768, 32768, 128, torch.bfloat16, seed=32)
     run(k, v, q, 128 ** -0.5, "obs bf16 d128 g4 S32768")
 
 
@@ -100,7 +72,7 @@ def test_32k():
 @pytest.mark.parametrize("layout", ["batch3", "strided", "transposed", "scaling"])
 def test_layouts_and_scaling(layout):
     B, Hkv, G, S, D = (3 if layout == "batch3" else 2), 2, 4, 1500, 128
-    k, v, q = inputs(B, Hkv, G, S, S - 200, D, torch.bfloat16, seed=7)
+    k, v, q = oa_inputs(B, Hkv, G, S, S - 200, D, torch.bfloat16, seed=7)
     scaling = 0.3 if layout == "scaling" else D ** -0.5
     if layout == "strided":  # rows of D within rows of D + 64: consumed in place through the TMA map
         big = torch.zeros((B, Hkv, S, D + 64), dtype=k.dtype, device=DEV)
@@ -122,7 +94,7 @@ def test_schedule_regimes(regime):
     S = tiles * 128
     items = R * -(-S // 128)
     assert (items < sm, items == sm, items > sm)[["fewer", "equal", "more"].index(regime)]
-    k, v, q = inputs(1, R, 1, S, S, 64, torch.float16, seed=tiles)
+    k, v, q = oa_inputs(1, R, 1, S, S, 64, torch.float16, seed=tiles)
     run(k, v, q, 64 ** -0.5, f"obs schedule {regime} ({items} items, {sm} SMs)")
 
 
@@ -130,12 +102,12 @@ def test_schedule_regimes(regime):
 def test_fp16_divisor_overflow():
     """S - s >= 65520 is inf in fp16: those first positions score exactly 0; the rest meet the 1-ulp bar."""
     S = 65600
-    k, v, q = inputs(1, 1, 1, S, S, 64, torch.float16, seed=3)
+    k, v, q = oa_inputs(1, 1, 1, S, S, 64, torch.float16, seed=3)
     sc = _native().observed_attention_score(k, q, 64 ** -0.5)
     zero = torch.arange(S, device=DEV) <= S - 65520
     assert int(zero.sum()) == 81
     assert (sc[..., zero] == 0).all() and not sc[..., zero].signbit().any()
-    ref = ref64(k, q, 64 ** -0.5)
+    ref = oa_ref64(k, q, 64 ** -0.5)
     assert (ref[..., zero] == 0).all()
     assert_vs_ref64(sc, ref, torch.zeros(S, dtype=torch.bool), "obs fp16 S65600", ftz=True)
 
@@ -143,10 +115,10 @@ def test_fp16_divisor_overflow():
 @gpu
 def test_unsupported_shapes():
     nat = _native()
-    k, _, q = inputs(1, 2, 16, 300, 300, 128, torch.bfloat16, seed=1)
+    k, _, q = oa_inputs(1, 2, 16, 300, 300, 128, torch.bfloat16, seed=1)
     with pytest.raises(RuntimeError, match="unsupported shape"):
         nat.observed_attention_score(k, q, 0.1)
-    k, _, q = inputs(1, 2, 2, 300, 300, 96, torch.bfloat16, seed=1)
+    k, _, q = oa_inputs(1, 2, 2, 300, 300, 96, torch.bfloat16, seed=1)
     with pytest.raises(RuntimeError, match="unsupported shape"):
         nat.observed_attention_score(k, q, 0.1)
 
@@ -157,7 +129,7 @@ def test_unsupported_shapes():
 @gpu
 def test_replays_under_capture():
     nat = _native()
-    k, v, q = inputs(1, 4, 4, 3000, 3000, 128, torch.bfloat16, seed=9)
+    k, v, q = oa_inputs(1, 4, 4, 3000, 3000, 128, torch.bfloat16, seed=9)
     eager = nat.observed_attention_compress(k, v, q, 128 ** -0.5, 1500, True, True)
     g = nat.capture(lambda: (nat.observed_attention_score(k, q, 128 ** -0.5),
                              *nat.observed_attention_compress(k, v, q, 128 ** -0.5, 1500, True, True)))
@@ -175,7 +147,7 @@ def test_no_intermediate_at_32k():
     """Memory grows by no more than the workspace, the outputs and the query tensor: no S x S weights."""
     nat = _native()
     B, Hkv, G, S, D = 1, 8, 4, 32768, 128
-    k, v, q = inputs(B, Hkv, G, S, S, D, torch.bfloat16, seed=10)
+    k, v, q = oa_inputs(B, Hkv, G, S, S, D, torch.bfloat16, seed=10)
     n_kept = S // 2
     p = nat.make_problem(k, v, n_kept, Hkv * G)
     ws = nat.workspace_bytes(p, nat.SCORER_OBSERVED_ATTENTION)
@@ -195,15 +167,6 @@ def test_no_intermediate_at_32k():
 # --------------------------------------------------------------------------------------------------
 # the press on a GPU tiny Llama (head_dim 64)
 # --------------------------------------------------------------------------------------------------
-def _model():
-    model = tiny_llama(dtype=torch.bfloat16, device=DEV, head_dim=64, heads=8, kv_heads=2)
-    model.config._attn_implementation = "sdpa"
-    return model
-
-
-def _ids(n=240):
-    g = torch.Generator().manual_seed(11)
-    return torch.stack([torch.randperm(250, generator=g)[:n] + 2 for _ in range(2)]).to(DEV)
 
 
 def _checked_compress(monkeypatch, calls):
@@ -227,7 +190,7 @@ def _checked_compress(monkeypatch, calls):
 def test_press_and_decoding_press_on_a_tiny_llama(monkeypatch):
     from kvpress_b200 import DecodingPress, ObservedAttentionPress
 
-    model, ids = _model(), _ids()
+    model, ids = tiny_gpu_llama(), gpu_ids()
     calls = []
     _checked_compress(monkeypatch, calls)
     cache = DynamicCache()
@@ -247,7 +210,7 @@ def test_press_and_decoding_press_on_a_tiny_llama(monkeypatch):
 def test_adakv_and_key_rerotation_run_under_sdpa():
     from kvpress_b200 import AdaKVPress, KeyRerotationPress, ObservedAttentionPress
 
-    model, ids = _model(), _ids()
+    model, ids = tiny_gpu_llama(), gpu_ids()
     cache = DynamicCache()
     with AdaKVPress(ObservedAttentionPress(compression_ratio=0.5))(model):
         model.model(input_ids=ids, past_key_values=cache)

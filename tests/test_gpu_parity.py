@@ -12,6 +12,7 @@ import torch
 
 from oracle import press_oracle as O
 from tests.conftest import ulp16_diff
+from tests.gpu_support import _native
 
 pytestmark = pytest.mark.gpu
 
@@ -26,12 +27,6 @@ HOST_ORACLE_ULP_BOUND = 8
 # tie band of the kept-set validity check against the reference's STORED scores: a kept position may sit one score distance
 # below the kernel's threshold, which itself may sit one score distance below the reference's
 SEL_ULP_SLACK = 2 * REF_ULP_BOUND
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
 
 
 def _check_compaction(k, v, k_out, v_out, idx):
@@ -502,10 +497,10 @@ def test_key_rerotation_vs_golden():
     import numpy as np
 
     from tests.golden.make_golden import digest16
-    from tests.test_oracle_golden import _rerotation_cases
+    from tests.support import rerotation_cases
     nat = _native()
     # the reference's re-rotated keys are stored as digests; the oracle's are bit-identical to them (checked here)
-    for tag, S, ratios, (keys_c, values_c, inv_freq_c, scores_c), get in _rerotation_cases():
+    for tag, S, ratios, (keys_c, values_c, inv_freq_c, scores_c), get in rerotation_cases():
         keys, values, scores, inv_freq = keys_c.to(DEV), values_c.to(DEV), scores_c.to(DEV), inv_freq_c.to(DEV)
         for i, r in enumerate(ratios):
             n_kept = O.kept_count(S, r)

@@ -16,37 +16,20 @@ rounded fp64 score; at most 4e-4 of a case's positions at 1 ulp for ExpectedAtte
 window 1); the worst row bias is 0.30 of its bound. Each bar is asserted as stated above, not at the measured values.
 """
 import ctypes
-import math
 import re
 from pathlib import Path
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from oracle import press_oracle as O
-from tests.conftest import ulp16_diff
+from tests.gpu_support import (assert_compress, assert_vs_ref64, ea_inputs, ea_ref64, _forced_head, _forced_tail,
+                               _gather, _layout, LAYOUTS, _name, _native, _sm_count, snap_inputs, snap_ref64)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
 CSRC = Path(__file__).resolve().parent.parent / "kvpress_b200" / "csrc"
-UNIT_ROUNDOFF = {torch.bfloat16: 2.0 ** -7, torch.float16: 2.0 ** -10}
 DTYPES = [torch.bfloat16, torch.float16]
-BIAS_MIN_N = 500
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
-
-
-def _sm_count() -> int:
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _name(dtype) -> str:
-    return "bf16" if dtype == torch.bfloat16 else "fp16"
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -101,127 +84,16 @@ def test_sweep_reaches_every_instantiation():
 # ---------------------------------------------------------------------------------------------------
 # fp64 references
 # ---------------------------------------------------------------------------------------------------
-def ea_ref64(k, v, mu, cov, eps: float, n_sink: int, use_vnorm: bool) -> torch.Tensor:
-    """expected_attention_scores_fp32 in float64, one (b, h) row at a time; forced positions are +inf."""
-    B, H, S, D = k.shape
-    G = mu.shape[1] // H
-    eps = float(torch.tensor(eps, dtype=torch.float32))  # the kernel adds the fp32 epsilon
-    out = torch.full((B, H, S), math.inf, dtype=torch.float64, device=k.device)
-    for b in range(B):
-        for h in range(H):
-            kk = k[b, h, n_sink:].double()
-            p = torch.zeros(S - n_sink, dtype=torch.float64, device=k.device)
-            for g in range(G):
-                hq = h * G + g
-                logit = kk @ mu[b, hq].double() / math.sqrt(D)
-                if cov is not None:
-                    logit = logit + ((kk @ cov[b, hq].double()) * kk).sum(-1) / (2 * D)
-                p += torch.softmax(logit, dim=-1)
-            p /= G
-            if use_vnorm:
-                p = (p + eps) * v[b, h, n_sink:].double().norm(dim=-1)
-            out[b, h, n_sink:] = p
-    return out
-
-
-def snap_ref64(q, k, window: int, kernel_size: int) -> torch.Tensor:
-    """snapkv_scores_fp32 in float64, one (b, h) row at a time; the forced window is +inf. Window mean, box filter and
-    group mean are linear, so the mean over all G * window rows is taken first."""
-    B, H, S, D = k.shape
-    G = q.shape[1] // H
-    n = S - window
-    out = torch.full((B, H, S), math.inf, dtype=torch.float64, device=k.device)
-    i = torch.arange(G * window, device=k.device) % window
-    mask = torch.arange(S, device=k.device)[None, :] > (S - window + i)[:, None]
-    for b in range(B):
-        for h in range(H):
-            qq = q[b, h * G:(h + 1) * G].reshape(G * window, D).double()
-            logits = (qq @ k[b, h].double().T) / math.sqrt(D)
-            p = torch.softmax(logits.masked_fill(mask, -math.inf), dim=-1)[:, :n].mean(0)
-            out[b, h, :n] = F.avg_pool1d(p[None, None], kernel_size, stride=1, padding=kernel_size // 2)[0, 0]
-    return out
 
 
 # ---------------------------------------------------------------------------------------------------
 # the bars
 # ---------------------------------------------------------------------------------------------------
-def assert_vs_ref64(got, ref, forced, what: str, ftz: bool = False, bias: bool = True) -> dict:
-    """Bars 1-3 of the module docstring. got: [B, H, S] kernel scores; ref: float64 [B, H, S]; forced: bool [S]."""
-    dtype = got.dtype
-    ref = ref.to(got.device)
-    forced = forced.to(got.device)
-    g, r = got[..., ~forced], ref[..., ~forced]
-    d = ulp16_diff(g, r.to(dtype))
-    ok = d <= 1
-    if ftz:  # ex2.approx.ftz: fp32 results below 2^-126 are flushed to zero
-        ok |= (r < 2.0 ** -126) & (g == 0)
-    assert ok.all(), f"{what}: {int((~ok).sum())} positions beyond 1 ulp of the fp64 score (max {int(d.max())})"
-    stats = {"max_ulp": int(d.max()) if d.numel() else 0, "one_ulp": float((d == 1).float().mean()) if d.numel() else 0.0,
-             "bias": 0.0}
-    if bias:
-        normal = r.abs() >= torch.finfo(dtype).tiny
-        n = normal.sum(-1)
-        rel = torch.where(normal, (g.double() - r) / r, torch.zeros_like(r))
-        mean = rel.sum(-1) / n.clamp_min(1)
-        bound = 8 * UNIT_ROUNDOFF[dtype] / torch.sqrt(12.0 * n.clamp_min(1).double())
-        rows = n >= BIAS_MIN_N
-        ratio = (mean.abs() / bound)[rows]
-        if ratio.numel():
-            stats["bias"] = float(ratio.max())
-            assert (ratio <= 1).all(), f"{what}: row bias {float(ratio.max()):.1f}x its bound " \
-                                       f"(mean rel error {float(mean[rows][ratio.argmax()]):.3e})"
-    if forced.any():
-        sentinel = (g.float().max() + 1).to(dtype)
-        assert (got[..., forced] == sentinel).all(), f"{what}: forced positions are not round(max + 1)"
-    print(f"[measured] {what}: max ulp {stats['max_ulp']}, 1-ulp fraction {stats['one_ulp']:.4f}, "
-          f"worst row bias {stats['bias']:.3f} of the bound")
-    return stats
-
-
-def _gather(x, idx):
-    return x.gather(2, idx.long().unsqueeze(-1).expand(-1, -1, -1, x.shape[-1]))
-
-
-def assert_compress(k, v, k_out, v_out, idx, scores, n_kept: int):
-    """Bar 4: the canonical selection of the kernel's own scores, and exact gathers."""
-    want = O.select_lowest_index_ties(scores.cpu(), n_kept)
-    assert torch.equal(idx.long().cpu(), want)
-    assert torch.equal(k_out, _gather(k, idx)) and torch.equal(v_out, _gather(v, idx))
-
-
-def _forced_head(S: int, n: int) -> torch.Tensor:
-    m = torch.zeros(S, dtype=torch.bool)
-    m[:n] = True
-    return m
-
-
-def _forced_tail(S: int, n: int) -> torch.Tensor:
-    m = torch.zeros(S, dtype=torch.bool)
-    m[S - n:] = True
-    return m
 
 
 # ---------------------------------------------------------------------------------------------------
 # inputs
 # ---------------------------------------------------------------------------------------------------
-def ea_inputs(B, H, G, S, D, dtype, seed, cov=True, mu_scale=0.5):
-    gen = torch.Generator(device=DEV).manual_seed(seed)
-    rn = lambda *s: torch.randn(*s, generator=gen, device=DEV)  # noqa: E731
-    k, v = rn(B, H, S, D).to(dtype), rn(B, H, S, D).to(dtype)
-    mu = (mu_scale * rn(B, H * G, D)).to(dtype)
-    c = None
-    if cov:
-        a = rn(B, H * G, D, D) / D ** 0.5
-        c = (a @ a.transpose(-1, -2)).to(dtype)
-    return k, v, mu, c
-
-
-def snap_inputs(B, H, G, S, D, window, dtype, seed):
-    gen = torch.Generator(device=DEV).manual_seed(seed)
-    rn = lambda *s: torch.randn(*s, generator=gen, device=DEV)  # noqa: E731
-    k, v = rn(B, H, S, D).to(dtype), rn(B, H, S, D).to(dtype)
-    q = (1.5 * rn(B, H * G, window, D)).to(dtype)
-    return k, v, q
 
 
 def run_ea(k, v, mu, cov, eps, n_sink, use_vnorm, what, bias=True, n_kept=None):
@@ -420,23 +292,6 @@ def test_snapkv_schedule_regimes(regime):
 # ---------------------------------------------------------------------------------------------------
 # 4. strided layouts: consumed in place, bitwise equal to contiguous copies
 # ---------------------------------------------------------------------------------------------------
-def _layout(kind, B, H, S, D, dtype, seed):
-    gen = torch.Generator(device=DEV).manual_seed(seed)
-    rn = lambda *s: torch.randn(*s, generator=gen, device=DEV).to(dtype)  # noqa: E731
-    if kind == "slice_along_s":
-        k, v = rn(B, H, S + 300, D)[:, :, 100:100 + S], rn(B, H, S + 50, D)[:, :, 50:]
-    elif kind == "every_other_head":
-        k, v = rn(B, 2 * H, S, D)[:, ::2], rn(B, 2 * H, S, D)[:, 1::2]
-    elif kind == "transposed_bshd":
-        k, v = rn(B, S, H, D).transpose(1, 2), rn(B, S, H, D).transpose(1, 2)
-    elif kind == "one_head_of_wider_cache":
-        k, v = rn(B, 4, S, D)[:, 2:3], rn(B, 3, S, D)[:, 1:2]
-    else:  # "v_strided_k_contiguous"
-        k, v = rn(B, H, S, D), rn(B, S, H, D).transpose(1, 2)
-    return k, v
-
-
-LAYOUTS = ["slice_along_s", "every_other_head", "transposed_bshd", "one_head_of_wider_cache", "v_strided_k_contiguous"]
 
 
 @gpu

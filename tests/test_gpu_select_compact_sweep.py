@@ -43,7 +43,7 @@ import pytest
 import torch
 
 from oracle import press_oracle as O
-from tests.test_gpu_keydiff_rerotation_sweep import rerotation_admissible, rope_inv_freq
+from tests.gpu_support import _name, _native, rerotation_admissible, rope_inv_freq, _sm_count
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
@@ -83,20 +83,6 @@ SHAPE_TILES = (1, GROUP_TILES, GROUP_TILES + 1, 2 * GROUP_TILES, 2 * GROUP_TILES
 SHAPE_S = [1, 2] + [t * TILE + d for t in SHAPE_TILES for d in (-1, 0, 1)]
 HEAD_DIMS = list(range(8, 257, 8))
 LAYOUTS = ["contiguous", "k_contiguous_v_bshd", "v_row_slice", "k_broadcast_head", "offset_views"]
-
-
-def _name(dtype) -> str:
-    return "bf16" if dtype == torch.bfloat16 else "fp16"
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
-
-
-def _sm_count() -> int:
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 # ---------------------------------------------------------------------------------------------------

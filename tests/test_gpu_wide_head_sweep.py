@@ -48,28 +48,17 @@ from pathlib import Path
 import pytest
 import torch
 
-import tests.test_gpu_criticalkv as CK
-import tests.test_gpu_non_causal_attention as NC
-import tests.test_gpu_observed_attention as OA
-import tests.test_gpu_scorer_sweep as SW
 from kvpress_b200 import wide_head_scores as W
 from oracle import press_oracle as O
 from tests.conftest import ulp16_diff
+from tests.gpu_support import (assert_compress, assert_vs_ref64, ckv_assert_scores, ckv_inputs, ea_inputs, ea_ref64,
+                               _forced_head, _forced_tail, _name, _native, nca_inputs, nca_ref, oa_inputs, oa_ref64,
+                               snap_inputs, snap_ref64, ulp_at)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
 DTYPES = [torch.bfloat16, torch.float16]
 MODULE = Path(W.__file__)
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
-
-
-def _name(dtype) -> str:
-    return "bf16" if dtype == torch.bfloat16 else "fp16"
 
 
 @pytest.fixture(params=["ieee", "tf32"])
@@ -93,7 +82,7 @@ def _check_compress(sc, k, v, ratio: float = 0.5):
     """native.scores_compress on the fallback's scores: the canonical selection and exact gathers."""
     n_kept = max(1, O.kept_count(k.shape[2], ratio))
     k_out, v_out, idx = _native().scores_compress(sc, k, v, n_kept, return_indices=True)
-    SW.assert_compress(k, v, k_out, v_out, idx, sc, n_kept)
+    assert_compress(k, v, k_out, v_out, idx, sc, n_kept)
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -302,13 +291,13 @@ def test_snapkv_fallback(case, dtype, fp32_precision):
     c = _full(SNAP_DEFAULTS, case)
     B, D, G, w, S, ksz = c["B"], c["D"], c["G"], c["w"], c["S"], c["k"]
     what = f"snapkv {_name(dtype)} {fp32_precision} {case}"
-    k, v, q = SW.snap_inputs(B, 2, G, S, D, w, dtype, 3000 + SNAP.index(case))
+    k, v, q = snap_inputs(B, 2, G, S, D, w, dtype, 3000 + SNAP.index(case))
     if c["peak"]:
         q = (q.float() * 4).to(dtype)  # logits of standard deviation 6
         _assert_peaked(q.double().reshape(B, 2, G * w, D) @ k.double().transpose(-1, -2) / math.sqrt(D), what)
     kw = {} if c["chunk"] is None else {"chunk": c["chunk"]}
     sc = _call(W.snapkv_scores, fp32_precision, k, q, w, ksz, **kw)
-    SW.assert_vs_ref64(sc, SW.snap_ref64(q, k, w, ksz), SW._forced_tail(S, w), what)
+    assert_vs_ref64(sc, snap_ref64(q, k, w, ksz), _forced_tail(S, w), what)
     _check_compress(sc, k, v)
 
 
@@ -319,14 +308,14 @@ def test_expected_attention_fallback(case, dtype, fp32_precision):
     c = _full(EA_DEFAULTS, case)
     B, D, G, S, n_sink = c["B"], c["D"], c["G"], c["S"], c["n_sink"]
     what = f"ea {_name(dtype)} {fp32_precision} {case}"
-    k, v, mu, cov = SW.ea_inputs(B, 2, G, S, D, dtype, 4000 + EA.index(case), cov=c["cov"],
+    k, v, mu, cov = ea_inputs(B, 2, G, S, D, dtype, 4000 + EA.index(case), cov=c["cov"],
                                  mu_scale=6.0 if c["peak"] else 0.5)
     if c["peak"]:
         _assert_peaked(mu.double().reshape(B, 2, G, D) @ k.double().transpose(-1, -2) / math.sqrt(D), what)
     kw = {} if c["chunk"] is None else {"chunk": c["chunk"]}
     sc = _call(W.expected_attention_scores, fp32_precision, k, v, mu, cov, c["eps"], n_sink, c["vn"], **kw)
-    ref = SW.ea_ref64(k, v, mu, cov, c["eps"], n_sink, c["vn"])
-    SW.assert_vs_ref64(sc, ref, SW._forced_head(S, n_sink), what)
+    ref = ea_ref64(k, v, mu, cov, c["eps"], n_sink, c["vn"])
+    assert_vs_ref64(sc, ref, _forced_head(S, n_sink), what)
     _check_compress(sc, k, v, 0.3)
 
 
@@ -337,10 +326,10 @@ def test_criticalkv_fallback(case, dtype, fp32_precision):
     c = _full(CKV_DEFAULTS, case)
     B, D, G, S, n_first = c["B"], c["D"], c["G"], c["S"], c["n_first"]
     what = f"ckv {_name(dtype)} {fp32_precision} {case}"
-    v, wo, base = CK.inputs(B, 2, G, S, D, c["hidden"], dtype, seed=5000 + CKV.index(case))
+    v, wo, base = ckv_inputs(B, 2, G, S, D, c["hidden"], dtype, seed=5000 + CKV.index(case))
     kw = {} if c["chunk"] is None else {"chunk": c["chunk"]}
     sc = _call(W.criticalkv_scores, fp32_precision, base, v, wo, 1e-4, n_first, **kw)
-    CK.assert_scores(sc, base, v, wo, 1e-4, n_first, what)
+    ckv_assert_scores(sc, base, v, wo, 1e-4, n_first, what)
     _check_compress(sc, torch.randn_like(v), v)
 
 
@@ -351,12 +340,12 @@ def test_observed_attention_fallback(case, dtype, fp32_precision):
     c = _full(OBS_DEFAULTS, case)
     B, D, G, S, n_q = c["B"], c["D"], c["G"], c["S"], c["n_q"]
     what = f"obs {_name(dtype)} {fp32_precision} {case}"
-    k, v, q = OA.inputs(B, 2, G, S, n_q, D, dtype, seed=6000 + OBS.index(case), q_scale=6.0 if c["peak"] else 1.5)
+    k, v, q = oa_inputs(B, 2, G, S, n_q, D, dtype, seed=6000 + OBS.index(case), q_scale=6.0 if c["peak"] else 1.5)
     if c["peak"]:
         _assert_peaked(q.double().reshape(B, 2, G * n_q, D) @ k.double().transpose(-1, -2) / math.sqrt(D), what)
     max_logits = 1 << 20 if c["rows"] is None else c["rows"] * B * 2 * G * S   # several query blocks either way
     sc = _call(W.observed_attention_scores, fp32_precision, k, q, D ** -0.5, max_logits=max_logits)
-    SW.assert_vs_ref64(sc, OA.ref64(k, q, D ** -0.5), torch.zeros(S, dtype=torch.bool), what)
+    assert_vs_ref64(sc, oa_ref64(k, q, D ** -0.5), torch.zeros(S, dtype=torch.bool), what)
     _check_compress(sc, k, v)
 
 
@@ -364,18 +353,18 @@ def test_observed_attention_fallback(case, dtype, fp32_precision):
 @pytest.mark.parametrize("dtype", DTYPES, ids=_name)
 @pytest.mark.parametrize("case", NCA, ids=_ids(NCA))
 def test_non_causal_attention_fallback(case, dtype, fp32_precision):
-    """NC.inputs gives every case logits of standard deviation 6 (chunk maxima of 20-25): all of them are peaked."""
+    """nca_inputs gives every case logits of standard deviation 6 (chunk maxima of 20-25): all of them are peaked."""
     c = _full(NCA_DEFAULTS, case)
     B, D, G, S, cs = c["B"], c["D"], c["G"], c["S"], c["cs"]
     what = f"nca {_name(dtype)} {fp32_precision} {case}"
-    k, v, q = NC.inputs(B, 2, G, S, D, dtype, seed=7000 + NCA.index(case))
+    k, v, q = nca_inputs(B, 2, G, S, D, dtype, seed=7000 + NCA.index(case))
     if c["peak"]:
         _assert_peaked(q[..., :cs, :].double().reshape(B, 2, G * cs, D) @ k[..., :cs, :].double().transpose(-1, -2),
                        what)
     max_logits = 1 << 20 if c["chunks"] is None else c["chunks"] * B * 2 * G * cs * cs
     sc = _call(W.non_causal_attention_scores, fp32_precision, k, v, q, cs, max_logits=max_logits)
-    z64, E = NC.ref(k, v, q, cs)
-    bar = NC.ulp_at(z64, dtype) + 4 * E
+    z64, E = nca_ref(k, v, q, cs)
+    bar = ulp_at(z64, dtype) + 4 * E
     d = (sc.double() - z64).abs()
     assert (d <= bar).all(), f"{what}: {int((d > bar).sum())} positions beyond ulp + 4 E_s ({float((d / bar).max()):.2f})"
     print(f"[measured] {what}: max ulp {int(ulp16_diff(sc, z64.to(dtype)).max())}, "

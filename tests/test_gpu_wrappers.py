@@ -10,15 +10,10 @@ import torch
 from oracle import press_oracle as O
 from tests.conftest import GOLDEN_DIR, ulp16_diff
 from tests.golden.make_golden import large_inputs, tensor_checksum
+from tests.gpu_support import _native
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-
-
-def _native():
-    from kvpress_b200 import native
-    native.load()
-    return native
 
 
 def _llama_attention(Hq, Hkv, D, hidden, q_weight, dtype=torch.bfloat16, theta=10000.0, max_pos=8192, device=None):

@@ -13,164 +13,62 @@ To re-record it from a checkout of the reference (located as in oracle/build_ref
     KVP_RECORD_LAGKV=1 python -m pytest tests/test_lagkv_host.py
 """
 import ctypes
-import itertools
-import json
-import os
-import subprocess
-import sys
 from pathlib import Path
 
-import numpy as np
 import pytest
 import torch
 
 from kvpress_b200 import LagKVPress, native
 from kvpress_b200.presses.lagkv_press import _lagkv_scores_fp32
-from tests import lagkv_backend as LB
-from tests.test_native_marshalling import _kv, rec  # noqa: F401  (fixture)
-from tests.test_reference_differential import _import_reference
+from tests import abi_cases, lagkv_backend as LB
+from tests.abi_cases import GOOD, ODD16
+from tests.support import kv, rec, reference_store  # noqa: F401  (rec: fixture)
 
-ROOT = Path(__file__).resolve().parent.parent
-STORE = ROOT / "tests" / "golden" / "lagkv_reference.npz"
-RECORD = os.environ.get("KVP_RECORD_LAGKV") == "1"
+STORE = Path(__file__).resolve().parent / "golden" / "lagkv_reference.npz"
 LAG_MAX = 1024
 
 # --------------------------------------------------------------------------------------------------
 # C ABI statuses
 # --------------------------------------------------------------------------------------------------
-GOOD, ODD16 = 0x10000, 0x1000C  # aligned; 4-byte but not 16-byte aligned
-FIELDS = dict(B=1, Hkv=2, Hq=2, S=1000, D=128, n_kept=500, dtype=0)
-STRIDES = (256000, 128000, 128)
-VALID = dict(K=GOOD, V=GOOD, n_sink=4, L=128, cross=0, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD, ws=GOOD,
-             ws_bytes="enough", stream=0)
-SLOTS = {
-    "kvp_lagkv_score": "K V n_sink L cross scores ws ws_bytes stream",
-    "kvp_lagkv_compress": "K V n_sink L cross K_out V_out idx scores ws ws_bytes stream",
-}
-CHANGES = {  # slot -> {label: value}
-    "p": {"null": None},
-    "dtype": {"1": 1, "3": 3},
-    "S": {"0": 0, "1": 1},
-    "D": {"8": 8, "12": 12, "64": 64, "264": 264},
-    "Hq": {"5": 5, "8": 8},
-    "n_kept": {"-1": -1, "0": 0, "1000": 1000, "1001": 1001},
-    "v_stride": {"s100": (256000, 128000, 100)},
-    "K": {"null": None, "odd": ODD16},
-    "V": {"null": None, "odd": ODD16},
-    "n_sink": {"-1": -1, "0": 0, "1000": 1000, "max": 2 ** 31 - 1},
-    "L": {"0": 0, "-3": -3, "1": 1, str(LAG_MAX): LAG_MAX, str(LAG_MAX + 1): LAG_MAX + 1},
-    "cross": {"1": 1, "7": 7},
-    "K_out": {"null": None, "odd": ODD16},
-    "V_out": {"null": None},
-    "idx": {"null": None},
-    "scores": {"null": None, "odd": ODD16},
-    "ws": {"null": None, "odd": ODD16},
-    "ws_bytes": {"short": "short"},
-}
-PROBLEM = ("dtype", "S", "D", "Hq", "n_kept", "v_stride")
-
-
-def expected(name: str, c: dict) -> int:
-    """The documented check order: validate -> n_kept == 0 short cut (compress) -> K / V / outputs (compress) ->
-    K, V, scores null and K / V alignment (score call) -> n_sink >= 0 and lag_size >= 1 -> lag_size <= 1024 ->
-    workspace."""
-    f = {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}
-    a = {**VALID, **{k: v for k, v in c.items() if k not in FIELDS}}
-    compress = name.endswith("compress")
-    if c.get("p", 0) is None:
-        return -1
-    if f["dtype"] not in (0, 1):
-        return -3
-    if f["S"] <= 0 or f["D"] % 8 or f["D"] > 256 or f["Hq"] % FIELDS["Hkv"]:
-        return -2
-    if not 0 <= f["n_kept"] <= f["S"]:
-        return -7
-    if "v_stride" in c:
-        return -4
-    if compress:
-        if f["n_kept"] == 0:
-            return 0
-        io = [a["K"], a["V"], a["K_out"], a["V_out"]]
-        if None in io:
-            return -1
-        if any(x % 16 for x in io):
-            return -4
-    else:
-        if None in (a["K"], a["V"], a["scores"]):
-            return -1
-        if a["K"] % 16 or a["V"] % 16:
-            return -4
+def _checks(f, a, compress):
+    """n_sink >= 0 and lag_size >= 1 -> lag_size <= 1024."""
     if a["n_sink"] < 0 or a["L"] < 1:
         return -7
-    if a["L"] > LAG_MAX:
-        return -2
-    if a["ws"] is None:
-        return -1
-    if a["ws"] % 16:
-        return -4
-    if a["ws_bytes"] == "short":
-        return -5
-    return -6
+    return -2 if a["L"] > LAG_MAX else 0
 
 
-def _cases(name: str) -> dict:
-    slots = ["p", *PROBLEM, *SLOTS[name].split()]
-    singles = [(s, label, v) for s in slots for label, v in CHANGES.get(s, {}).items()]
-    cases = {"valid": {}, **{f"{s}={label}": {s: v} for s, label, v in singles}}
-    cases.update({f"{s1}={l1},{s2}={l2}": {s1: v1, s2: v2}
-                  for (s1, l1, v1), (s2, l2, v2) in itertools.combinations(singles, 2) if s1 != s2})
-    return cases
-
-
-def statuses() -> dict:
-    """Every case's status. Run only in a process that sees no GPU."""
-    import importlib.util
-
-    assert torch.cuda.device_count() == 0, "the status cases pass fake device pointers: they must not see a GPU"
-    spec = importlib.util.spec_from_file_location("kvp_native", ROOT / "kvpress_b200" / "native.py")
-    nat = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(nat)
-    lib = nat.load()
-
-    def problem(c):
-        p = nat.KvpProblem()
-        for k, v in {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}.items():
-            setattr(p, k, v)
-        p.k_stride = (ctypes.c_int64 * 3)(*STRIDES)
-        p.v_stride = (ctypes.c_int64 * 3)(*c.get("v_stride", STRIDES))
-        return p
-
-    out = {}
-    for name in SLOTS:
-        for label, c in _cases(name).items():
-            pr = None if c.get("p", 0) is None else problem(c)
-            need = ctypes.c_size_t(1 << 20)
-            if pr is not None:
-                lib.kvp_workspace_bytes(ctypes.byref(pr), nat.SCORER_LAGKV, ctypes.byref(need))
-            args = [None if pr is None else ctypes.byref(pr)]
-            for slot in SLOTS[name].split():
-                v = c.get(slot, VALID[slot])
-                if slot == "ws_bytes":
-                    v = need.value - 1 if v == "short" else need.value
-                elif slot == "idx" and v is not None:
-                    v = ctypes.cast(ctypes.c_void_p(v), ctypes.POINTER(ctypes.c_int32))
-                args.append(v)
-            out[f"{name}({label})"] = getattr(lib, name)(*args)
-    return out
+ABI = abi_cases.Spec(
+    scorer=native.SCORER_LAGKV, fields=dict(Hq=2),
+    slots={"kvp_lagkv_score": "K V n_sink L cross scores ws ws_bytes stream",
+           "kvp_lagkv_compress": "K V n_sink L cross K_out V_out idx scores ws ws_bytes stream"},
+    valid=dict(K=GOOD, V=GOOD, n_sink=4, L=128, cross=0, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD, ws=GOOD,
+               ws_bytes="enough", stream=0),
+    changes={
+        "p": {"null": None},
+        "dtype": {"1": 1, "3": 3},
+        "S": {"0": 0, "1": 1},
+        "D": {"8": 8, "12": 12, "64": 64, "264": 264},
+        "Hq": {"5": 5, "8": 8},
+        "n_kept": {"-1": -1, "0": 0, "1000": 1000, "1001": 1001},
+        "v_stride": {"s100": (256000, 128000, 100)},
+        "K": {"null": None, "odd": ODD16},
+        "V": {"null": None, "odd": ODD16},
+        "n_sink": {"-1": -1, "0": 0, "1000": 1000, "max": 2 ** 31 - 1},
+        "L": {"0": 0, "-3": -3, "1": 1, str(LAG_MAX): LAG_MAX, str(LAG_MAX + 1): LAG_MAX + 1},
+        "cross": {"1": 1, "7": 7},
+        "K_out": {"null": None, "odd": ODD16},
+        "V_out": {"null": None},
+        "idx": {"null": None},
+        "scores": {"null": None, "odd": ODD16},
+        "ws": {"null": None, "odd": ODD16},
+        "ws_bytes": {"short": "short"},
+    },
+    operands={"score": (["K", "V", "scores"], ["K", "V"]), "compress": ([], [])},
+    checks=_checks)
 
 
 def test_every_status_of_the_lagkv_entry_points_follows_the_check_order():
-    env = {k: v for k, v in os.environ.items() if not k.startswith("KVP_")}
-    env["CUDA_VISIBLE_DEVICES"] = ""
-    code = "import json, tests.test_lagkv_host as m; print(json.dumps(m.statuses()))"
-    r = subprocess.run([sys.executable, *(["-s"] if sys.flags.no_user_site else []), "-c", code], cwd=ROOT, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    got = json.loads(r.stdout.strip().splitlines()[-1])
-    want = {f"{name}({label})": expected(name, c) for name in SLOTS for label, c in _cases(name).items()}
-    assert sorted(got) == sorted(want) and len(got) > 1400
-    diffs = [f"{k}: {got[k]} != {want[k]}" for k in want if got[k] != want[k]]
-    assert not diffs, f"{len(diffs)} differences, first ones:\n" + "\n".join(diffs[:30])
+    abi_cases.assert_statuses(__name__, 1400)
 
 
 def test_workspace_and_launch_count_of_the_new_scorer_id():
@@ -195,7 +93,7 @@ def test_workspace_and_launch_count_of_the_new_scorer_id():
 # --------------------------------------------------------------------------------------------------
 def test_lagkv_wrappers_pass_their_full_argument_list(rec):  # noqa: F811
     P = lambda t: t.data_ptr()  # noqa: E731
-    k, v = _kv(B=2, H=2, S=300, D=64)
+    k, v = kv(B=2, H=2, S=300, D=64)
 
     def last(name, n_kept):
         got, p, a = rec.calls[-1]
@@ -229,24 +127,7 @@ def test_lagkv_wrappers_pass_their_full_argument_list(rec):  # noqa: F811
 # --------------------------------------------------------------------------------------------------
 # the float64 definition against the unmodified reference
 # --------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def ref():
-    stored = {} if RECORD or not STORE.exists() else dict(np.load(STORE))
-    recorded = {}
-
-    def result(key: str, compute) -> dict:
-        if RECORD:
-            out = {k: np.asarray(x.detach().numpy() if torch.is_tensor(x) else x)
-                   for k, x in compute(_import_reference()).items()}
-            recorded.update({f"{key}|{k}": x for k, x in out.items()})
-            return out
-        out = {k.split("|", 1)[1]: x for k, x in stored.items() if k.split("|", 1)[0] == key}
-        assert out, f"no stored reference result for {key}"
-        return out
-
-    yield result
-    if RECORD:
-        np.savez_compressed(STORE, **recorded)
+ref = reference_store(STORE, "KVP_RECORD_LAGKV")
 
 
 # (name, S, n_sink, lag_size, planted constant channel)

@@ -3,60 +3,11 @@ against a recording stand-in for the shared library (the real library still answ
 kvp_launches_per_compress, which need no device). What is pinned here: the kvp_problem fields and strides handed to
 the C ABI for views, the pointers (views are consumed in place, small operands are made contiguous), dtype codes,
 score strides for broadcast scores, NULL for optional operands, and the n_kept == 0 short cut."""
-import contextlib
-import ctypes
-
 import pytest
 import torch
 
 from kvpress_b200 import native
-
-
-class Recorder:
-    def __init__(self, real):
-        self.real, self.calls = real, []
-
-    def __getattr__(self, name):
-        if name in ("kvp_workspace_bytes", "kvp_launches_per_compress", "kvp_status_string", "kvp_last_cuda_error",
-                    "kvp_abi_version"):
-            return getattr(self.real, name)
-
-        def fn(*args):
-            p = args[0]._obj
-            snap = {f: getattr(p, f) for f in ("B", "Hkv", "Hq", "S", "D", "n_kept", "dtype")}
-            snap["k_stride"], snap["v_stride"] = tuple(p.k_stride), tuple(p.v_stride)
-            vals = []
-            for a in args[1:]:
-                if isinstance(a, ctypes.c_void_p):
-                    vals.append(a.value or 0)
-                elif isinstance(a, ctypes.Array):
-                    vals.append(tuple(a))
-                else:
-                    vals.append(a)
-            self.calls.append((name, snap, vals))
-            return 0
-        return fn
-
-
-@pytest.fixture
-def rec(monkeypatch):
-    r = Recorder(native.load())
-    monkeypatch.setattr(native, "load", lambda: r)
-    monkeypatch.setattr(native, "_require_cuda_kv", lambda *a, **k: None)
-    monkeypatch.setattr(native, "_stream", lambda: ctypes.c_void_p(0))
-    monkeypatch.setattr(native, "_out_device", lambda keys: keys.device)
-    monkeypatch.setattr(native, "_normalise", lambda t: t if native._rows_ok(t) else t.contiguous())  # CPU stands in for CUDA
-    monkeypatch.setattr(torch.cuda, "device", lambda d: contextlib.nullcontext())
-    # the recorder accepts any shape: keep the tiny head_dim-16 inputs of these tests on the C-ABI entry points
-    from kvpress_b200 import wide_head_scores
-
-    monkeypatch.setattr(wide_head_scores, "snapkv_on_tensor_cores", lambda *a: True)
-    monkeypatch.setattr(wide_head_scores, "expected_attention_on_tensor_cores", lambda *a: True)
-    return r
-
-
-def _kv(B=2, H=3, S=50, D=64, dtype=torch.bfloat16):
-    return torch.randn(B, H, S, D).to(dtype), torch.randn(B, H, S, D).to(dtype)
+from tests.support import kv, rec  # noqa: F401  (rec: fixture)
 
 
 def test_strided_views_are_consumed_in_place(rec):
@@ -75,7 +26,7 @@ def test_strided_views_are_consumed_in_place(rec):
 
 
 def test_layouts_the_kernels_cannot_address_are_copied_once(rec):
-    k, v = _kv()
+    k, v = kv()
     kt = k.transpose(2, 3).contiguous().transpose(2, 3)            # last dim strided: rows are not contiguous
     native.knorm_compress(kt, v, 10)
     _, p, a = rec.calls[-1]
@@ -86,10 +37,10 @@ def test_layouts_the_kernels_cannot_address_are_copied_once(rec):
 
 
 def test_dtype_codes_single_row_and_empty_selection(rec):
-    k, v = _kv(dtype=torch.float16)
+    k, v = kv(dtype=torch.float16)
     native.knorm_compress(k, v, 5)
     assert rec.calls[-1][1]["dtype"] == 1
-    k1, v1 = _kv(S=1)
+    k1, v1 = kv(S=1)
     native.streaming_compress(k1, v1, 1, 4)
     assert rec.calls[-1][1]["k_stride"][2] == 64                   # S == 1: the row stride stays addressable
     n = len(rec.calls)
@@ -100,7 +51,7 @@ def test_dtype_codes_single_row_and_empty_selection(rec):
 
 
 def test_scorer_operands(rec):
-    k, v = _kv(B=2, H=2, S=200, D=128)
+    k, v = kv(B=2, H=2, S=200, D=128)
     q = torch.randn(2, 8, 16, 128).to(torch.bfloat16)
     native.snapkv_compress(k, v, q.transpose(1, 2).contiguous().transpose(1, 2), 16, 5, 100)
     name, p, a = rec.calls[-1]
@@ -119,7 +70,7 @@ def test_scorer_operands(rec):
 
 
 def test_generic_scores_and_rerotation_operands(rec):
-    k, v = _kv(B=2, H=3, S=40, D=64)
+    k, v = kv(B=2, H=3, S=40, D=64)
     row = torch.rand(40).to(torch.bfloat16)                         # already in the cache dtype: stays a broadcast view
     native.scores_compress(row.expand(2, 3, 40), k, v, 10)          # broadcast scores: zero batch/head strides
     name, p, a = rec.calls[-1]
@@ -237,7 +188,7 @@ def test_every_wrapper_passes_its_full_argument_list(rec, monkeypatch):
         return a[:-3]
 
     P = lambda t: t.data_ptr()  # noqa: E731
-    k, v = _kv(B=2, H=2, S=64, D=64)
+    k, v = kv(B=2, H=2, S=64, D=64)
 
     sc = native.knorm_score(k)
     assert last("kvp_knorm_score") == [P(k), P(sc)]

@@ -14,164 +14,61 @@ To re-record them from a checkout of the reference (located as in oracle/build_r
     KVP_RECORD_NON_CAUSAL_ATTENTION=1 python -m pytest tests/test_non_causal_attention_host.py
 """
 import ctypes
-import itertools
-import json
-import os
-import subprocess
-import sys
 from pathlib import Path
 
-import numpy as np
 import pytest
 import torch
 from transformers import DynamicCache
 
 from kvpress_b200 import NonCausalAttnPress, native
-from tests import cpu_backend, non_causal_attention_backend as NB
-from tests.test_native_marshalling import _kv, rec  # noqa: F401  (fixture)
-from tests.test_reference_differential import _import_reference, _ordered_signature
-from tests.tiny_models import tiny_llama, tiny_qwen3
+from tests import abi_cases, cpu_backend, non_causal_attention_backend as NB
+from tests.abi_cases import GOOD, ODD16
+from tests.support import TO_INT32, kv, ordered_signature, rec, reference_store  # noqa: F401  (rec: fixture)
+from tests.tiny_models import distinct_ids, tiny_llama, tiny_model
 
-ROOT = Path(__file__).resolve().parent.parent
-STORE = ROOT / "tests" / "golden" / "non_causal_attention_reference.npz"
-RECORD = os.environ.get("KVP_RECORD_NON_CAUSAL_ATTENTION") == "1"
+STORE = Path(__file__).resolve().parent / "golden" / "non_causal_attention_reference.npz"
 
 # --------------------------------------------------------------------------------------------------
 # C ABI statuses
 # --------------------------------------------------------------------------------------------------
-GOOD, ODD16 = 0x10000, 0x1000C  # aligned; 4-byte but not 16-byte aligned
-FIELDS = dict(B=1, Hkv=2, Hq=4, S=1000, D=128, n_kept=500, dtype=0)
-STRIDES = (256000, 128000, 128)
-VALID = dict(K=GOOD, V=GOOD, q=GOOD, cs=256, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD, ws=GOOD, ws_bytes="enough",
-             stream=0)
-SLOTS = {
-    "kvp_non_causal_attention_score": "K V q cs scores ws ws_bytes stream",
-    "kvp_non_causal_attention_compress": "K V q cs K_out V_out idx scores ws ws_bytes stream",
-}
-CHANGES = {  # slot -> {label: value}
-    "p": {"null": None},
-    "dtype": {"3": 3},
-    "S": {"0": 0},
-    "D": {"12": 12, "64": 64, "96": 96},
-    "Hq": {"5": 5, "32": 32},
-    "n_kept": {"-1": -1, "0": 0, "1000": 1000},
-    "v_stride": {"s100": (256000, 128000, 100)},
-    "K": {"null": None, "odd": ODD16},
-    "V": {"null": None, "odd": ODD16},
-    "q": {"null": None, "odd": ODD16},
-    "cs": {"0": 0, "-1": -1, "1": 1, "128": 128, "512": 512},
-    "K_out": {"null": None},
-    "V_out": {"null": None, "odd": ODD16},
-    "idx": {"null": None},
-    "scores": {"null": None},
-    "ws": {"null": None, "odd": ODD16},
-    "ws_bytes": {"short": "short"},
-}
-PROBLEM = ("dtype", "S", "D", "Hq", "n_kept", "v_stride")
-
-
-def expected(name: str, c: dict) -> int:
-    """The documented check order: validate -> n_kept == 0 short cut (compress) -> K / V / outputs (compress) ->
-    null / alignment of q (and K, V, scores for the score call) -> chunk_size >= 1 -> shape instantiated -> workspace."""
-    f = {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}
-    a = {**VALID, **{k: v for k, v in c.items() if k not in FIELDS}}
-    compress = name.endswith("compress")
-    if c.get("p", 0) is None:
-        return -1
-    if f["dtype"] not in (0, 1):
-        return -3
-    if f["S"] <= 0 or f["D"] % 8 or f["Hq"] % FIELDS["Hkv"]:
-        return -2
-    if not 0 <= f["n_kept"] <= f["S"]:
-        return -7
-    if "v_stride" in c:
-        return -4
-    if compress:
-        if f["n_kept"] == 0:
-            return 0
-        io = [a["K"], a["V"], a["K_out"], a["V_out"]]
-        if None in io:
-            return -1
-        if any(x % 16 for x in io):
-            return -4
-        nulls, aligned = [a["q"]], [a["q"]]
-    else:
-        nulls, aligned = [a["K"], a["V"], a["q"], a["scores"]], [a["K"], a["V"], a["q"]]
-    if None in nulls:
-        return -1
-    if any(x % 16 for x in aligned):
-        return -4
+def _checks(f, a, compress):
+    """chunk_size >= 1 -> shape instantiated."""
     if a["cs"] < 1:
         return -7
-    if f["D"] not in (64, 128) or a["cs"] not in (128, 256) or not 1 <= f["Hq"] // FIELDS["Hkv"] <= 8:
-        return -2
-    if a["ws"] is None:
-        return -1
-    if a["ws"] % 16:
-        return -4
-    if a["ws_bytes"] == "short":
-        return -5
-    return -6
+    return -2 if f["D"] not in (64, 128) or a["cs"] not in (128, 256) or not 1 <= f["Hq"] // f["Hkv"] <= 8 else 0
 
 
-def _cases(name: str) -> dict:
-    slots = ["p", *PROBLEM, *SLOTS[name].split()]
-    singles = [(s, label, v) for s in slots for label, v in CHANGES.get(s, {}).items()]
-    cases = {"valid": {}, **{f"{s}={label}": {s: v} for s, label, v in singles}}
-    cases.update({f"{s1}={l1},{s2}={l2}": {s1: v1, s2: v2}
-                  for (s1, l1, v1), (s2, l2, v2) in itertools.combinations(singles, 2) if s1 != s2})
-    return cases
-
-
-def statuses() -> dict:
-    """Every case's status. Run only in a process that sees no GPU."""
-    import importlib.util
-
-    assert torch.cuda.device_count() == 0, "the status cases pass fake device pointers: they must not see a GPU"
-    spec = importlib.util.spec_from_file_location("kvp_native", ROOT / "kvpress_b200" / "native.py")
-    nat = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(nat)
-    lib = nat.load()
-
-    def problem(c):
-        p = nat.KvpProblem()
-        for k, v in {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}.items():
-            setattr(p, k, v)
-        p.k_stride = (ctypes.c_int64 * 3)(*STRIDES)
-        p.v_stride = (ctypes.c_int64 * 3)(*c.get("v_stride", STRIDES))
-        return p
-
-    out = {}
-    for name in SLOTS:
-        for label, c in _cases(name).items():
-            pr = None if c.get("p", 0) is None else problem(c)
-            need = ctypes.c_size_t(1 << 20)
-            if pr is not None:
-                lib.kvp_workspace_bytes(ctypes.byref(pr), nat.SCORER_NON_CAUSAL_ATTENTION, ctypes.byref(need))
-            args = [None if pr is None else ctypes.byref(pr)]
-            for slot in SLOTS[name].split():
-                v = c.get(slot, VALID[slot])
-                if slot == "ws_bytes":
-                    v = need.value - 1 if v == "short" else need.value
-                elif slot == "idx" and v is not None:
-                    v = ctypes.cast(ctypes.c_void_p(v), ctypes.POINTER(ctypes.c_int32))
-                args.append(v)
-            out[f"{name}({label})"] = getattr(lib, name)(*args)
-    return out
+ABI = abi_cases.Spec(
+    scorer=native.SCORER_NON_CAUSAL_ATTENTION,
+    slots={"kvp_non_causal_attention_score": "K V q cs scores ws ws_bytes stream",
+           "kvp_non_causal_attention_compress": "K V q cs K_out V_out idx scores ws ws_bytes stream"},
+    valid=dict(K=GOOD, V=GOOD, q=GOOD, cs=256, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD, ws=GOOD,
+               ws_bytes="enough", stream=0),
+    changes={
+        "p": {"null": None},
+        "dtype": {"3": 3},
+        "S": {"0": 0},
+        "D": {"12": 12, "64": 64, "96": 96},
+        "Hq": {"5": 5, "32": 32},
+        "n_kept": {"-1": -1, "0": 0, "1000": 1000},
+        "v_stride": {"s100": (256000, 128000, 100)},
+        "K": {"null": None, "odd": ODD16},
+        "V": {"null": None, "odd": ODD16},
+        "q": {"null": None, "odd": ODD16},
+        "cs": {"0": 0, "-1": -1, "1": 1, "128": 128, "512": 512},
+        "K_out": {"null": None},
+        "V_out": {"null": None, "odd": ODD16},
+        "idx": {"null": None},
+        "scores": {"null": None},
+        "ws": {"null": None, "odd": ODD16},
+        "ws_bytes": {"short": "short"},
+    },
+    operands={"score": (["K", "V", "q", "scores"], ["K", "V", "q"]), "compress": (["q"], ["q"])},
+    checks=_checks)
 
 
 def test_every_status_of_the_non_causal_attention_entry_points_follows_the_check_order():
-    env = {k: v for k, v in os.environ.items() if not k.startswith("KVP_")}
-    env["CUDA_VISIBLE_DEVICES"] = ""
-    code = "import json, tests.test_non_causal_attention_host as m; print(json.dumps(m.statuses()))"
-    r = subprocess.run([sys.executable, *(["-s"] if sys.flags.no_user_site else []), "-c", code], cwd=ROOT, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    got = json.loads(r.stdout.strip().splitlines()[-1])
-    want = {f"{name}({label})": expected(name, c) for name in SLOTS for label, c in _cases(name).items()}
-    assert sorted(got) == sorted(want) and len(got) > 800
-    diffs = [f"{k}: {got[k]} != {want[k]}" for k in want if got[k] != want[k]]
-    assert not diffs, f"{len(diffs)} differences, first ones:\n" + "\n".join(diffs[:30])
+    abi_cases.assert_statuses(__name__, 800)
 
 
 def test_workspace_and_launch_count_of_the_new_scorer_id():
@@ -207,7 +104,7 @@ def test_non_causal_attention_wrappers_pass_their_full_argument_list(rec, monkey
 
     monkeypatch.setattr(native, "_workspace", spy)
     P = lambda t: t.data_ptr()  # noqa: E731
-    k, v = _kv(B=2, H=2, S=64, D=64)
+    k, v = kv(B=2, H=2, S=64, D=64)
     q = torch.randn(2, 8, 64, 64).to(torch.bfloat16)
 
     def last(name, n_kept):
@@ -242,25 +139,7 @@ def test_non_causal_attention_wrappers_pass_their_full_argument_list(rec, monkey
 # --------------------------------------------------------------------------------------------------
 # the float64 definition and the press against the unmodified reference
 # --------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def ref():
-    stored = {} if RECORD or not STORE.exists() else dict(np.load(STORE))
-    recorded = {}
-
-    def result(key: str, compute) -> dict:
-        if RECORD:
-            out = {k: np.asarray(x.detach().numpy() if torch.is_tensor(x) else x)
-                   for k, x in compute(_import_reference()).items()}
-            out = {k: x.astype(np.int32) if x.dtype == np.int64 else x for k, x in out.items()}
-            recorded.update({f"{key}|{k}": x for k, x in out.items()})
-            return out
-        out = {k.split("|", 1)[1]: x for k, x in stored.items() if k.split("|", 1)[0] == key}
-        assert out, f"no stored reference result for {key}"
-        return out
-
-    yield result
-    if RECORD:
-        np.savez_compressed(STORE, **recorded)
+ref = reference_store(STORE, "KVP_RECORD_NON_CAUSAL_ATTENTION", TO_INT32)
 
 
 # (S, chunk_size, negative last chunk): one chunk, several, padded by 1 or more, not padded, a single position
@@ -327,14 +206,9 @@ def test_float64_definition_is_the_reference(ref, S, cs, negative):
         assert torch.allclose(z, z_ref, rtol=0, atol=1e-5 * float(z_ref.abs().max()))
 
 
-def _ids(n, seed=5):
-    g = torch.Generator().manual_seed(seed)
-    return torch.stack([torch.randperm(250, generator=g)[:n] + 2 for _ in range(2)])
-
-
 def _kept_rows(cache) -> list:
     """Per layer, the ordered signature of every retained (K, V) row of every head."""
-    return [_ordered_signature(la.keys, la.values) for la in cache.layers]
+    return [ordered_signature(la.keys, la.values) for la in cache.layers]
 
 
 def _shared_fraction(got: torch.Tensor, want: torch.Tensor) -> float:
@@ -357,12 +231,10 @@ def test_press_keeps_the_reference_rows(monkeypatch, ref, ratio, family, cs, n):
     cache lengths are equal."""
     cpu_backend.install(monkeypatch)
     NB.install(monkeypatch)
-    ids = _ids(n)
+    ids = distinct_ids(n, seed=5)
 
     def model():
-        m = (tiny_llama if family == "llama" else tiny_qwen3)(dtype=torch.bfloat16)
-        m.config._attn_implementation = "sdpa"
-        return m
+        return tiny_model(family, dtype=torch.bfloat16)
 
     def reference(kvpress):
         m, cache = model(), DynamicCache()

@@ -14,11 +14,7 @@ oracle/build_ref.py):  KVP_RECORD_OBSERVED_ATTENTION=1 python -m pytest tests/te
 """
 import ctypes
 import itertools
-import json
 import math
-import os
-import subprocess
-import sys
 from pathlib import Path
 
 import numpy as np
@@ -27,156 +23,66 @@ import torch
 from transformers import DynamicCache
 
 from kvpress_b200 import DecodingPress, ObservedAttentionPress, native
-from tests import cpu_backend, observed_attention_backend
-from tests.test_native_marshalling import _kv, rec  # noqa: F401  (fixture)
-from tests.test_reference_differential import _import_reference, _rows_signature, close
-from tests.tiny_models import tiny_llama, tiny_qwen3
+from tests import abi_cases, cpu_backend, observed_attention_backend
+from tests.abi_cases import GOOD, ODD16
+from tests.support import TO_32BIT, close, kv, rec, reference_store, rows_signature  # noqa: F401  (rec: fixture)
+from tests.tiny_models import distinct_ids, tiny_model
 
-ROOT = Path(__file__).resolve().parent.parent
-STORE = ROOT / "tests" / "golden" / "observed_attention_reference.npz"
-RECORD = os.environ.get("KVP_RECORD_OBSERVED_ATTENTION") == "1"
+STORE = Path(__file__).resolve().parent / "golden" / "observed_attention_reference.npz"
 
 # --------------------------------------------------------------------------------------------------
 # C ABI statuses
 # --------------------------------------------------------------------------------------------------
-GOOD, ODD16 = 0x10000, 0x1000C  # aligned; 4-byte but not 16-byte aligned
-FIELDS = dict(B=1, Hkv=2, Hq=4, S=1000, D=128, n_kept=500, dtype=0)
-STRIDES = (256000, 128000, 128)
-VALID = dict(K=GOOD, V=GOOD, q=GOOD, n_q=1000, scaling=0.125, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD, ws=GOOD,
-             ws_bytes="enough", stream=0)
-SLOTS = {
-    "kvp_observed_attention_score": "K q n_q scaling scores ws ws_bytes stream",
-    "kvp_observed_attention_compress": "K V q n_q scaling K_out V_out idx scores ws ws_bytes stream",
-}
-CHANGES = {  # slot -> {label: value}
-    "p": {"null": None},
-    "dtype": {"3": 3},
-    "S": {"0": 0},
-    "D": {"12": 12, "64": 64},
-    "Hq": {"5": 5},
-    "n_kept": {"-1": -1, "0": 0, "1000": 1000},
-    "k_stride": {"s100": (256000, 128000, 100)},
-    "K": {"null": None, "odd": ODD16},
-    "V": {"null": None, "odd": ODD16},
-    "q": {"null": None, "odd": ODD16},
-    "n_q": {"0": 0, "-1": -1, "1": 1, "999": 999, "1001": 1001},
-    "scaling": {"0": 0.0, "-1": -1.0, "inf": math.inf, "nan": math.nan, "1": 1.0},
-    "K_out": {"null": None},
-    "V_out": {"null": None, "odd": ODD16},
-    "idx": {"null": None},
-    "scores": {"null": None},
-    "ws": {"null": None, "odd": ODD16},
-    "ws_bytes": {"short": "short"},
-}
-PROBLEM = ("dtype", "S", "D", "Hq", "n_kept", "k_stride")
-
-
 def _align256(n: int) -> int:
     return (n + 255) // 256 * 256
 
 
-def expected(name: str, c: dict) -> int:
-    """The documented check order: validate -> n_kept == 0 short cut (compress) -> K / V / outputs (compress) ->
-    null / alignment of q (and K, scores for the score call) -> n_q -> scaling -> workspace."""
-    f = {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}
-    a = {**VALID, **{k: v for k, v in c.items() if k not in FIELDS}}
-    compress = name.endswith("compress")
-    if c.get("p", 0) is None:
-        return -1
-    if f["dtype"] not in (0, 1):
-        return -3
-    if f["S"] <= 0 or f["D"] % 8 or f["Hq"] % FIELDS["Hkv"]:
-        return -2
-    if not 0 <= f["n_kept"] <= f["S"]:
-        return -7
-    if "k_stride" in c:
-        return -4
-    if compress:
-        if f["n_kept"] == 0:
-            return 0
-        io = [a["K"], a["V"], a["K_out"], a["V_out"]]
-        if None in io:
-            return -1
-        if any(x % 16 for x in io):
-            return -4
-        nulls, aligned = [a["q"]], [a["q"]]
-    else:
-        nulls, aligned = [a["K"], a["q"], a["scores"]], [a["K"], a["q"]]
-    if None in nulls:
-        return -1
-    if any(x % 16 for x in aligned):
-        return -4
+def _checks(f, a, compress):
+    """n_q -> scaling."""
     if not 1 <= a["n_q"] <= f["S"]:
         return -7
-    if not (math.isfinite(a["scaling"]) and a["scaling"] > 0):
-        return -7
-    if a["ws"] is None:
-        return -1
-    if a["ws"] % 16:
-        return -4
-    if a["ws_bytes"] == "short":
-        # one byte short of the size for n_q = S; the per-row normalisers of fewer rows may still fit
-        qrows = lambda n: _align256(4 * f["B"] * f["Hq"] * n)  # noqa: E731
-        return -5 if qrows(a["n_q"]) == qrows(f["S"]) else -6
-    return -6
+    return 0 if math.isfinite(a["scaling"]) and a["scaling"] > 0 else -7
 
 
-def _cases(name: str) -> dict:
-    slots = ["p", *PROBLEM, *SLOTS[name].split()]
-    singles = [(s, label, v) for s in slots for label, v in CHANGES.get(s, {}).items()]
-    cases = {"valid": {}, **{f"{s}={label}": {s: v} for s, label, v in singles}}
-    cases.update({f"{s1}={l1},{s2}={l2}": {s1: v1, s2: v2}
-                  for (s1, l1, v1), (s2, l2, v2) in itertools.combinations(singles, 2) if s1 != s2})
-    return cases
+def _short(f, a):
+    """One byte short of the size for n_q = S: the per-row normalisers of fewer rows may still fit."""
+    qrows = lambda n: _align256(4 * f["B"] * f["Hq"] * n)  # noqa: E731
+    return -5 if qrows(a["n_q"]) == qrows(f["S"]) else -6
 
 
-def statuses() -> dict:
-    """Every case's status. Run only in a process that sees no GPU."""
-    import importlib.util
-
-    assert torch.cuda.device_count() == 0, "the status cases pass fake device pointers: they must not see a GPU"
-    spec = importlib.util.spec_from_file_location("kvp_native", ROOT / "kvpress_b200" / "native.py")
-    nat = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(nat)
-    lib = nat.load()
-
-    def problem(c):
-        p = nat.KvpProblem()
-        for k, v in {**FIELDS, **{k: v for k, v in c.items() if k in FIELDS}}.items():
-            setattr(p, k, v)
-        p.k_stride = (ctypes.c_int64 * 3)(*c.get("k_stride", STRIDES))
-        p.v_stride = (ctypes.c_int64 * 3)(*STRIDES)
-        return p
-
-    need = ctypes.c_size_t(0)
-    assert lib.kvp_workspace_bytes(ctypes.byref(problem({})), nat.SCORER_OBSERVED_ATTENTION, ctypes.byref(need)) == 0
-    out = {}
-    for name in SLOTS:
-        for label, c in _cases(name).items():
-            args = [None if c.get("p", 0) is None else ctypes.byref(problem(c))]
-            for slot in SLOTS[name].split():
-                v = c.get(slot, VALID[slot])
-                if slot == "ws_bytes":
-                    v = need.value - 1 if v == "short" else need.value
-                elif slot == "idx" and v is not None:
-                    v = ctypes.cast(ctypes.c_void_p(v), ctypes.POINTER(ctypes.c_int32))
-                args.append(v)
-            out[f"{name}({label})"] = getattr(lib, name)(*args)
-    return out
+ABI = abi_cases.Spec(
+    scorer=native.SCORER_OBSERVED_ATTENTION,
+    slots={"kvp_observed_attention_score": "K q n_q scaling scores ws ws_bytes stream",
+           "kvp_observed_attention_compress": "K V q n_q scaling K_out V_out idx scores ws ws_bytes stream"},
+    valid=dict(K=GOOD, V=GOOD, q=GOOD, n_q=1000, scaling=0.125, K_out=GOOD, V_out=GOOD, idx=GOOD, scores=GOOD,
+               ws=GOOD, ws_bytes="enough", stream=0),
+    changes={
+        "p": {"null": None},
+        "dtype": {"3": 3},
+        "S": {"0": 0},
+        "D": {"12": 12, "64": 64},
+        "Hq": {"5": 5},
+        "n_kept": {"-1": -1, "0": 0, "1000": 1000},
+        "k_stride": {"s100": (256000, 128000, 100)},
+        "K": {"null": None, "odd": ODD16},
+        "V": {"null": None, "odd": ODD16},
+        "q": {"null": None, "odd": ODD16},
+        "n_q": {"0": 0, "-1": -1, "1": 1, "999": 999, "1001": 1001},
+        "scaling": {"0": 0.0, "-1": -1.0, "inf": math.inf, "nan": math.nan, "1": 1.0},
+        "K_out": {"null": None},
+        "V_out": {"null": None, "odd": ODD16},
+        "idx": {"null": None},
+        "scores": {"null": None},
+        "ws": {"null": None, "odd": ODD16},
+        "ws_bytes": {"short": "short"},
+    },
+    problem=("dtype", "S", "D", "Hq", "n_kept", "k_stride"),
+    operands={"score": (["K", "q", "scores"], ["K", "q"]), "compress": (["q"], ["q"])},
+    checks=_checks, short=_short)
 
 
 def test_every_status_of_the_observed_attention_entry_points_follows_the_check_order():
-    env = {k: v for k, v in os.environ.items() if not k.startswith("KVP_")}
-    env["CUDA_VISIBLE_DEVICES"] = ""
-    code = "import json, tests.test_observed_attention_host as m; print(json.dumps(m.statuses()))"
-    r = subprocess.run([sys.executable, *(["-s"] if sys.flags.no_user_site else []), "-c", code], cwd=ROOT, env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-4000:]
-    got = json.loads(r.stdout.strip().splitlines()[-1])
-    want = {f"{name}({label})": expected(name, c) for name in SLOTS for label, c in _cases(name).items()}
-    assert sorted(got) == sorted(want) and len(got) > 900
-    diffs = [f"{k}: {got[k]} != {want[k]}" for k in want if got[k] != want[k]]
-    assert not diffs, f"{len(diffs)} differences, first ones:\n" + "\n".join(diffs[:30])
+    abi_cases.assert_statuses(__name__, 900)
 
 
 def test_workspace_and_launch_count_of_the_new_scorer_id():
@@ -210,7 +116,7 @@ def test_observed_attention_wrappers_pass_their_full_argument_list(rec, monkeypa
 
     monkeypatch.setattr(native, "_workspace", spy)
     P = lambda t: t.data_ptr()  # noqa: E731
-    k, v = _kv(B=2, H=2, S=64, D=64)
+    k, v = kv(B=2, H=2, S=64, D=64)
     q = torch.randn(2, 8, 40, 64).to(torch.bfloat16)
 
     def last(name, n_kept):
@@ -294,41 +200,11 @@ def test_observed_attention_partition_is_balanced_and_complete(sm):
 # --------------------------------------------------------------------------------------------------
 # the press against the unmodified reference (CPU stand-ins)
 # --------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def ref():
-    stored = {} if RECORD or not STORE.exists() else dict(np.load(STORE))
-    recorded = {}
-
-    def result(key: str, compute) -> dict:
-        if RECORD:
-            out = {k: np.asarray(x.detach().numpy() if torch.is_tensor(x) else x)
-                   for k, x in compute(_import_reference()).items()}
-            out = {k: x.astype(np.float32) if x.dtype == np.float64 else x.astype(np.int32) if x.dtype == np.int64
-                   else x for k, x in out.items()}
-            recorded.update({f"{key}|{k}": x for k, x in out.items()})
-            return out
-        out = {k.split("|", 1)[1]: x for k, x in stored.items() if k.split("|", 1)[0] == key}
-        assert out, f"no stored reference result for {key}"
-        return out
-
-    yield result
-    if RECORD:
-        np.savez_compressed(STORE, **recorded)
-
-
-def _ids(n=160, seed=5):
-    g = torch.Generator().manual_seed(seed)
-    return torch.stack([torch.randperm(250, generator=g)[:n] + 2 for _ in range(2)])
-
-
-def _model(family, attn):
-    m = tiny_llama() if family == "llama" else tiny_qwen3()
-    m.config._attn_implementation = attn
-    return m
+ref = reference_store(STORE, "KVP_RECORD_OBSERVED_ATTENTION", TO_32BIT)
 
 
 def _signatures(cache) -> dict:
-    return {"len": cache.get_seq_length(), **{f"sig{i}": _rows_signature(la.keys, la.values)
+    return {"len": cache.get_seq_length(), **{f"sig{i}": rows_signature(la.keys, la.values)
                                                for i, la in enumerate(cache.layers)}}
 
 
@@ -337,10 +213,10 @@ def _signatures(cache) -> dict:
 def test_observed_attention_keeps_the_reference_rows(monkeypatch, ref, ratio, family):
     cpu_backend.install(monkeypatch)
     observed_attention_backend.install(monkeypatch)
-    ids = _ids()
+    ids = distinct_ids(160, seed=5)
 
     def reference(kvpress):
-        model, cache = _model(family, "eager"), DynamicCache()
+        model, cache = tiny_model(family, "eager"), DynamicCache()
         with kvpress.ObservedAttentionPress(compression_ratio=ratio)(model):
             model.model(input_ids=ids, past_key_values=cache, cache_position=torch.arange(ids.shape[1]))
         return _signatures(cache)
@@ -348,12 +224,12 @@ def test_observed_attention_keeps_the_reference_rows(monkeypatch, ref, ratio, fa
     want = ref(f"observed/{ratio}/{family}", reference)
     # same attention implementation as the reference, so that later layers see bit-equal hidden states; the press
     # ignores the eager weights it is handed
-    model, ours = _model(family, "eager"), DynamicCache()
+    model, ours = tiny_model(family, "eager"), DynamicCache()
     with ObservedAttentionPress(compression_ratio=ratio)(model):
         model.model(input_ids=ids, past_key_values=ours)
     assert ours.get_seq_length() == int(want["len"]) == int(ids.shape[1] * (1 - ratio))
     for i, la in enumerate(ours.layers):
-        close(_rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
+        close(rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
 
 
 def test_decoding_press_over_observed_attention_matches_the_reference(monkeypatch, ref):
@@ -363,7 +239,7 @@ def test_decoding_press_over_observed_attention_matches_the_reference(monkeypatc
     divisors see different rows (ours keep position order)."""
     cpu_backend.install(monkeypatch)
     observed_attention_backend.install(monkeypatch)
-    ids = _ids(120)
+    ids = distinct_ids(120, seed=5)
     steps = [torch.tensor([[10 + t], [40 + t]]) for t in range(7)]
 
     def drive(model, cache, **fw):
@@ -376,23 +252,23 @@ def test_decoding_press_over_observed_attention_matches_the_reference(monkeypatc
         return lens
 
     def reference(kvpress):
-        model, cache = _model("llama", "eager"), DynamicCache()
+        model, cache = tiny_model("llama", "eager"), DynamicCache()
         with kvpress.DecodingPress(kvpress.ObservedAttentionPress(), compression_interval=4, target_size=96)(model):
             lens = drive(model, cache, cache_position=torch.arange(ids.shape[1]))
         return {"lens": np.array(lens), **_signatures(cache)}
 
     want = ref("decoding/observed", reference)
-    model, cache = _model("llama", "eager"), DynamicCache()
+    model, cache = tiny_model("llama", "eager"), DynamicCache()
     with DecodingPress(ObservedAttentionPress(), compression_interval=4, target_size=96)(model):
         lens = drive(model, cache)
     assert lens == [int(x) for x in want["lens"]] and cache.get_seq_length() == int(want["len"])
     for i, la in enumerate(cache.layers):
-        close(_rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
+        close(rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
 
 
 def test_press_refuses_a_pruned_cache_and_a_narrow_sliding_window(monkeypatch):
     observed_attention_backend.install(monkeypatch)
-    model = _model("qwen3", "sdpa")
+    model = tiny_model("qwen3", "sdpa")
     attn = model.model.layers[0].self_attn
     S, n_q = 12, 20
     keys = torch.randn(1, 2, S, 16)

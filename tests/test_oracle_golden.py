@@ -7,6 +7,7 @@ import torch
 
 from oracle import press_oracle as O
 from tests.conftest import GOLDEN_DIR, REFERENCE_DIR, assert_gemm_prologue, ulp16_diff
+from tests.support import rerotation_cases
 
 
 def test_knorm_scores_match_reference(golden):
@@ -113,25 +114,11 @@ def test_ulp_helper():
 
 
 # ---- KeyRerotationPress (SURVEY §8f row 1) ------------------------------------------------------------
-def _rerotation_cases():
-    """Per case: the regenerated inputs (checked against the stored checksum) and a getter of the stored arrays; the
-    reference's re-rotated outputs are stored as SHA-256 digests (make_golden.digest16)."""
-    from tests.golden.make_golden import RERO_CASES, rerotation_inputs, tensor_checksum
-
-    z = np.load(GOLDEN_DIR / "rerotation.npz")
-    for (tag, B, H, S, D, dtype, theta), row in zip(RERO_CASES, z["cases"]):
-        assert row.tolist() == [B, H, S, D, int(dtype == torch.float16)]
-        inputs = rerotation_inputs(B, H, S, D, dtype, theta)
-        assert (tensor_checksum(*inputs[:2], inputs[3]) == z[f"{tag}_checksum"]).all(), "RNG no longer reproduces"
-        get = lambda k, tag=tag: z[f"{tag}_{k}"]  # noqa: E731
-        yield tag, int(S), [float(r) for r in z["ratios"]], inputs, get
-
-
 def test_rerotation_matches_reference_bit_exact():
     """The oracle's rerotate_keys / key_rerotation_compress against KeyRerotationPress.compress outputs."""
     from tests.golden.make_golden import digest16
 
-    for tag, S, ratios, (keys, values, inv_freq, scores), get in _rerotation_cases():
+    for tag, S, ratios, (keys, values, inv_freq, scores), get in rerotation_cases():
         for i, r in enumerate(ratios):
             n_kept = O.kept_count(S, r)
             k2, v2, idx = O.key_rerotation_compress(scores, keys, values, n_kept, inv_freq)

@@ -7,9 +7,6 @@ the reference (located as in oracle/build_ref.py):  KVP_RECORD_REFERENCE=1 pytho
 The stored values come from another host's float32 CPU kernels: values compare with a tolerance of a few float32
 rounding steps (a different retained row differs by orders of magnitude more); counts, lengths and masks exactly."""
 import json
-import os
-import sys
-import types
 from pathlib import Path
 
 import numpy as np
@@ -19,77 +16,20 @@ from transformers import DynamicCache
 
 from kvpress_b200 import ExpectedAttentionPress, KeyDiffPress, KnormPress, SnapKVPress, StreamingLLMPress
 from tests import cpu_backend
-from tests.tiny_models import tiny_llama, tiny_qwen3
+from tests.support import TO_32BIT, close, ordered_signature, reference_store, rows_signature
+from tests.tiny_models import distinct_ids, tiny_llama, tiny_qwen3
 
 STORE = Path(__file__).resolve().parent / "golden" / "reference_differential.npz"
-RECORD = os.environ.get("KVP_RECORD_REFERENCE") == "1"
-_recorded: dict = {}
-
-
-def _import_reference():
-    from oracle.build_ref import REFERENCE
-
-    path = str(REFERENCE)
-    assert (REFERENCE / "kvpress").is_dir(), "recording needs a reference checkout (oracle/build_ref.py)"
-    sys.modules.setdefault("fire", types.ModuleType("fire"))
-    if path not in sys.path:
-        sys.path.insert(0, path)
-    import kvpress
-
-    return kvpress
-
-
-@pytest.fixture(scope="module")
-def ref():
-    """Runs `compute(kvpress)` on the reference when recording; otherwise returns the stored results of `key`."""
-    stored = {} if RECORD else dict(np.load(STORE))
-
-    def result(key: str, compute) -> dict:
-        if RECORD:
-            out = {k: np.asarray(v.detach().numpy() if torch.is_tensor(v) else v) for k, v in compute(_import_reference()).items()}
-            # stored compactly: float32 is well inside the comparison tolerance, positions fit int32
-            out = {k: v.astype(np.float32) if v.dtype == np.float64 else v.astype(np.int32) if v.dtype == np.int64 else v
-                   for k, v in out.items()}
-            _recorded.update({f"{key}|{k}": v for k, v in out.items()})
-            return out
-        out = {k.split("|", 1)[1]: v for k, v in stored.items() if k.split("|", 1)[0] == key}
-        assert out, f"no stored reference result for {key}"
-        return out
-
-    yield result
-    if RECORD:
-        old = dict(np.load(STORE)) if STORE.exists() else {}
-        old.update(_recorded)
-        np.savez_compressed(STORE, **old)
-
-
-def close(got, want, what=""):
-    """Same values up to float32 rounding of another host (see the module docstring)."""
-    got, want = (torch.as_tensor(x.detach() if torch.is_tensor(x) else np.asarray(x), dtype=torch.float64)
-                 for x in (got, want))
-    assert got.shape == want.shape, (what, got.shape, want.shape)
-    assert torch.allclose(got, want, rtol=1e-5, atol=1e-6), (what, float((got - want).abs().max()))
+ref = reference_store(STORE, "KVP_RECORD_REFERENCE", TO_32BIT, merge=True)
 
 
 def _signatures(cache) -> dict:
-    return {f"sig{i}": _rows_signature(la.keys, la.values) for i, la in enumerate(cache.layers)}
+    return {f"sig{i}": rows_signature(la.keys, la.values) for i, la in enumerate(cache.layers)}
 
 
 def _assert_signatures(cache, want: dict):
     for i, la in enumerate(cache.layers):
-        close(_rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
-
-
-def _ordered_signature(keys, values):
-    """Signature of every retained (K, V) row of every head, in cache order: a seeded random projection."""
-    g = torch.Generator().manual_seed(0)
-    w = torch.randn(keys.shape[-1], generator=g, dtype=torch.float64)
-    return keys.double() @ w + 3.0 * (values.double() @ w)
-
-
-def _rows_signature(keys, values):
-    """Order-independent signature of the retained (K, V) rows of every head."""
-    return _ordered_signature(keys, values).sort(-1).values
+        close(rows_signature(la.keys, la.values), want[f"sig{i}"], f"layer {i}")
 
 
 CASES = [
@@ -108,10 +48,7 @@ CASES = [
 def test_same_rows_as_reference(monkeypatch, ref, name, ref_cls, our_cls, kw, ratio, family):
     cpu_backend.install(monkeypatch)
     model = tiny_llama() if family == "llama" else tiny_qwen3()
-    # distinct tokens per sequence: a repeated token gives layer-0 keys of exactly equal norm (RoPE keeps
-    # norms), i.e. exact score ties that torch.topk and the kernels may legitimately break differently
-    g = torch.Generator().manual_seed(5)
-    ids = torch.stack([torch.randperm(250, generator=g)[:160] + 2 for _ in range(2)])
+    ids = distinct_ids(160, seed=5)  # distinct tokens: no exactly tied layer-0 key norms
     S = ids.shape[1]
 
     def reference(kvpress):
@@ -122,7 +59,7 @@ def test_same_rows_as_reference(monkeypatch, ref, name, ref_cls, our_cls, kw, ra
         out = {"len": theirs.get_seq_length()}
         for i, lt in enumerate(theirs.layers):
             out[f"norms{i}"] = lt.keys.norm(dim=-1).sort(-1).values
-            out[f"sig{i}"] = _rows_signature(lt.keys, lt.values)
+            out[f"sig{i}"] = rows_signature(lt.keys, lt.values)
         return out
 
     want = ref(f"same_rows/{name}/{ratio}/{family}", reference)
@@ -137,7 +74,7 @@ def test_same_rows_as_reference(monkeypatch, ref, name, ref_cls, our_cls, kw, ra
             # torch.topk and by the lowest-position rule. The multiset of kept scores must still agree.
             close(lo.keys.norm(dim=-1).sort(-1).values, want[f"norms{i}"], f"layer {i}")
         else:
-            close(_rows_signature(lo.keys, lo.values), want[f"sig{i}"], f"layer {i}")
+            close(rows_signature(lo.keys, lo.values), want[f"sig{i}"], f"layer {i}")
 
 
 @pytest.mark.parametrize("inner", ["streaming", "snapkv"])
@@ -149,8 +86,7 @@ def test_key_rerotation_same_cache_as_reference(monkeypatch, ref, inner, family)
 
     cpu_backend.install(monkeypatch)
     model = tiny_llama() if family == "llama" else tiny_qwen3()
-    g = torch.Generator().manual_seed(7)
-    ids = torch.stack([torch.randperm(250, generator=g)[:160] + 2 for _ in range(2)])
+    ids = distinct_ids(160, seed=7)
     S, ratio = ids.shape[1], 0.4
     _, ref_cls, our_cls, kw = next(c for c in CASES if c[0] == inner)
 
@@ -160,7 +96,7 @@ def test_key_rerotation_same_cache_as_reference(monkeypatch, ref, inner, family)
             model.model(input_ids=ids, past_key_values=theirs, cache_position=torch.arange(S))
         out = {"len": theirs.get_seq_length()}
         for i, lt in enumerate(theirs.layers):
-            out[f"keys{i}"], out[f"rows{i}"] = _ordered_signature(lt.keys, lt.keys), _ordered_signature(lt.keys, lt.values)
+            out[f"keys{i}"], out[f"rows{i}"] = ordered_signature(lt.keys, lt.keys), ordered_signature(lt.keys, lt.values)
         return out
 
     want = ref(f"rerotation/{inner}/{family}", reference)
@@ -172,8 +108,8 @@ def test_key_rerotation_same_cache_as_reference(monkeypatch, ref, inner, family)
 
     assert ours.get_seq_length() == int(want["len"]) == int(S * (1 - ratio))
     for i, lo in enumerate(ours.layers):   # row by row, re-rotated keys included
-        close(_ordered_signature(lo.keys, lo.keys), want[f"keys{i}"], f"keys {i}")
-        close(_ordered_signature(lo.keys, lo.values), want[f"rows{i}"], f"rows {i}")
+        close(ordered_signature(lo.keys, lo.keys), want[f"keys{i}"], f"keys {i}")
+        close(ordered_signature(lo.keys, lo.values), want[f"rows{i}"], f"rows {i}")
 
 
 def _prefill(press, model, ids, reference=False):
@@ -192,11 +128,6 @@ def _reference_prefill(make_press, model, ids):
     return compute
 
 
-def _distinct_ids(seed, n=160, batch=2):
-    g = torch.Generator().manual_seed(seed)
-    return torch.stack([torch.randperm(250, generator=g)[:n] + 2 for _ in range(batch)])
-
-
 def _assert_same_rows(ours, want):
     assert [la.keys.shape[2] for la in ours.layers] == list(want["lens"])
     _assert_signatures(ours, want)
@@ -210,7 +141,7 @@ def test_pyramidkv_same_rows_and_budgets_as_reference(monkeypatch, ref, ratio, b
 
     cpu_backend.install(monkeypatch)
     model = tiny_llama(layers=4)
-    ids = _distinct_ids(11)
+    ids = distinct_ids(160, seed=11)
     kw = dict(compression_ratio=ratio, window_size=16, kernel_size=5, beta=beta)
     from types import SimpleNamespace
     grid = [(q_len, r, b, layer) for q_len in (100, 777, 4096, 131072) for r in (0.1, 0.5, 0.75, 0.95)
@@ -240,7 +171,7 @@ def test_chunk_press_same_rows_as_reference(monkeypatch, ref, inner, n_tokens, c
 
     cpu_backend.install(monkeypatch)
     model = tiny_llama()
-    ids = _distinct_ids(12, n=n_tokens)
+    ids = distinct_ids(n_tokens, seed=12)
     _, ref_cls, our_cls, kw = next(c for c in CASES if c[0] == inner)
     if inner == "snapkv":
         kw = {"window_size": 8, "kernel_size": 3}
@@ -256,7 +187,7 @@ def test_composed_and_per_layer_wrappers_same_rows_as_reference(monkeypatch, ref
 
     cpu_backend.install(monkeypatch)
     model = tiny_llama()
-    ids = _distinct_ids(13)
+    ids = distinct_ids(160, seed=13)
     # second press = Knorm: its scores do not depend on the ROW ORDER the first press leaves behind (the reference
     # emits top-k order, this package ascending positions; index-based scorers such as SnapKV's window or
     # StreamingLLM's sinks would read a different "last w rows" from the reference's permuted cache)
@@ -291,7 +222,7 @@ def test_random_press_same_rows_as_reference_on_cpu(monkeypatch, ref):
 
     cpu_backend.install(monkeypatch)
     model = tiny_llama()
-    ids = _distinct_ids(14)
+    ids = distinct_ids(160, seed=14)
     want = ref("random", _reference_prefill(lambda m: m.RandomPress(0.5, seed=3), model, ids))
     _assert_same_rows(_prefill(RandomPress(0.5, seed=3), model, ids), want)
 
@@ -305,7 +236,7 @@ def test_adakv_masks_the_same_keys_as_reference(monkeypatch, ref, inner, alpha):
 
     cpu_backend.install(monkeypatch)
     model = tiny_llama()
-    ids = _distinct_ids(21)
+    ids = distinct_ids(160, seed=21)
     S = ids.shape[1]
     _, ref_cls, our_cls, kw = next(c for c in CASES if c[0] == inner)
     attns = [layer.self_attn for layer in model.model.layers]
@@ -354,7 +285,7 @@ def test_chunkkv_press_same_rows_as_reference(monkeypatch, ref, inner, n_tokens,
         pytest.skip("window scorers need more tokens than their window")
     cpu_backend.install(monkeypatch)
     model = tiny_llama()
-    ids = _distinct_ids(31, n=n_tokens)
+    ids = distinct_ids(n_tokens, seed=31)
     _, ref_cls, our_cls, kw = next(c for c in CASES if c[0] == inner)
     if inner == "snapkv":
         kw = {"window_size": 8, "kernel_size": 3}
@@ -363,7 +294,7 @@ def test_chunkkv_press_same_rows_as_reference(monkeypatch, ref, inner, n_tokens,
                          ids, reference=True)
         out = {"len": cache.get_seq_length(), "lens": [la.keys.shape[2] for la in cache.layers], **_signatures(cache)}
         for i, lt in enumerate(cache.layers):
-            out[f"rows{i}"] = _ordered_signature(lt.keys, lt.values)
+            out[f"rows{i}"] = ordered_signature(lt.keys, lt.values)
         return out
 
     want = ref(f"chunkkv/{inner}/{n_tokens}/{chunk}", reference)
@@ -373,7 +304,7 @@ def test_chunkkv_press_same_rows_as_reference(monkeypatch, ref, inner, n_tokens,
         _assert_same_rows(ours, want)
         return
     for i, lo in enumerate(ours.layers):               # both emit position order: caches are equal row by row
-        close(_ordered_signature(lo.keys, lo.values), want[f"rows{i}"], f"rows {i}")
+        close(ordered_signature(lo.keys, lo.values), want[f"rows{i}"], f"rows {i}")
 
 
 @pytest.mark.parametrize("inner", ["knorm", "keydiff"])
@@ -385,7 +316,7 @@ def test_block_press_same_rows_as_reference(monkeypatch, ref, inner, block_size)
 
     cpu_backend.install(monkeypatch)
     model = tiny_llama()
-    ids = _distinct_ids(32)
+    ids = distinct_ids(160, seed=32)
     _, ref_cls, our_cls, kw = next(c for c in CASES if c[0] == inner)
     want = ref(f"block/{inner}/{block_size}", _reference_prefill(
         lambda m: m.BlockPress(ref_cls(m)(compression_ratio=0.5, **kw), block_size=block_size), model, ids))
@@ -409,7 +340,7 @@ def test_expected_attention_stats_press_same_rows_and_folder_layout_as_reference
     model = tiny_llama()
     cfg = model.config
     L, Hq, D = cfg.num_hidden_layers, cfg.num_attention_heads, cfg.head_dim
-    batches = [_distinct_ids(40 + i, n=120, batch=1) for i in range(3)]
+    batches = [distinct_ids(120, seed=40 + i, batch=1) for i in range(3)]
     stats = collect_query_statistics(model, batches, n_sink=4)
     # independent restatement of the reference's collect_queries arithmetic
     from kvpress_b200.utils import get_prerope_query_states
@@ -432,7 +363,7 @@ def test_expected_attention_stats_press_same_rows_and_folder_layout_as_reference
     # folder layout: ours -> the reference's loader and writer (recorded: the folder the reference writes back);
     # that folder -> our loader; our folder has the reference's layout (same config, same tensor names and shapes)
     stats.save_pretrained(str(tmp_path / "ours"))
-    ids = _distinct_ids(50)
+    ids = distinct_ids(160, seed=50)
 
     def reference(kvpress):
         from kvpress.presses.expected_attention_with_stats import ExpectedAttentionStats as RefStats
@@ -556,7 +487,7 @@ def test_decoding_press_with_stats_press_matches_reference(monkeypatch, ref, tmp
     model = tiny_llama()
     import kvpress_b200
 
-    stats = collect_query_statistics(model, [_distinct_ids(60 + i, n=100, batch=1) for i in range(2)], n_sink=4)
+    stats = collect_query_statistics(model, [distinct_ids(100, seed=60 + i, batch=1) for i in range(2)], n_sink=4)
     stats.save_pretrained(str(tmp_path / "stats"))
     context, question = words(60, seed=8), words(5, seed=9)
     kw = dict(compression_interval=7, target_size=40, hidden_states_buffer_size=256)

@@ -28,6 +28,20 @@ def tiny_qwen3(dtype=torch.float32, device="cpu", head_dim=16, layers=2, heads=4
     return model
 
 
+def tiny_model(family="llama", attn="sdpa", **kw):
+    """tiny_llama / tiny_qwen3 (`kw` as they take it) with the attention implementation `attn`."""
+    model = (tiny_llama if family == "llama" else tiny_qwen3)(**kw)
+    model.config._attn_implementation = attn
+    return model
+
+
+def distinct_ids(n, seed, batch=2, device="cpu"):
+    """`batch` prompts of n distinct token ids: a repeated token gives layer-0 keys of exactly equal norm (RoPE keeps
+    norms), i.e. exact score ties that torch.topk and the kernels may legitimately break differently."""
+    g = torch.Generator().manual_seed(seed)
+    return torch.stack([torch.randperm(250, generator=g)[:n] + 2 for _ in range(batch)]).to(device)
+
+
 def word_tokenizer():
     vocab = {f"w{i}": i for i in range(2, VOCAB - 1)}
     vocab.update({"<pad>": 0, "<s>": 1, "</s>": VOCAB - 1, "<unk>": VOCAB})
