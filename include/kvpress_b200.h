@@ -18,6 +18,7 @@
  *     kvp_non_causal_attention_* <- kvpress/presses/non_causal_attention_press.py (Compactor's attention half)
  *     kvp_lagkv_*              <- kvpress/presses/lagkv_press.py (lag-relative K / V statistics, from K and V only)
  *     kvp_cur_*                <- kvpress/presses/cur_press.py (approximate K / V leverage scores, from K and V only)
+ *     kvp_merging_*            <- kvpress/presses/merging_press.py (evicted values folded into their nearest kept row)
  *     kvp_scores_compress      <- scorer_press.py:93-100 for an arbitrary score tensor
  *                                 (what wrapper presses / user ScorerPress subclasses need)
  *
@@ -79,8 +80,10 @@ typedef enum kvp_scorer {
     KVP_SCORER_OBSERVED_ATTENTION = 7,
     KVP_SCORER_NON_CAUSAL_ATTENTION = 8,
     KVP_SCORER_LAGKV = 9,
-    /* 10 is not assigned: kvp_launches_per_compress answers KVP_ERR_BAD_ARGUMENT for it, as for any unknown id */
-    KVP_SCORER_CUR = 11
+    /* 10 and 12 are not assigned: kvp_launches_per_compress answers KVP_ERR_BAD_ARGUMENT for them, as for any unknown
+     * id */
+    KVP_SCORER_CUR = 11,
+    KVP_SCORER_MERGING = 13 /* kvp_merging_*: the selection of the caller's scores, then the merge */
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -310,6 +313,52 @@ int kvp_cur_score(const kvp_problem* p, const void* K, const void* V, int32_t nu
 int kvp_cur_compress(const kvp_problem* p, const void* K, const void* V, int32_t num_sinks, int32_t leverage_type,
                      int32_t local_window_size, const float* G, int32_t r, void* K_out, void* V_out, int32_t* idx_out,
                      void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+
+/* ---- MergingPress (kvpress/presses/merging_press.py) ----------------------------------------------------------------
+ * Keeps the same rows as hard eviction, but first folds every evicted value into the kept row whose key is most
+ * cosine-similar. Keys are only gathered, so the press is safe under RoPE. Per row (b, kv head j):
+ *   - kept: the n_kept kept positions, ascending and distinct, numbered by kept slot t; ev: the other n_evict = S - n_kept
+ *     positions, ascending, numbered by evicted slot e.
+ *   - sim(e, t) = (K[e].K[t]) / (max(|K[e]|, 1e-6) max(|K[t]|, 1e-6)), from the raw 16-bit keys: exact products, fp32
+ *     accumulation, fp32 norms.
+ *   - target(e) is the kept slot with the largest sim; exact ties go to the lowest slot (the lowest position). A NaN
+ *     similarity wins the max, as in torch.max: the first NaN column is the target. max_sim(e) = sim(e, target(e)).
+ *   - The gate: ok(e) = max_sim(e) >= similarity_threshold. If merge_fraction < 1: thr = torch.quantile over the row's
+ *     n_evict entries of max_sim with the non-ok entries at -inf, at q = 1 - merge_fraction, and ok &= max_sim >= thr.
+ *     torch's arithmetic is reproduced exactly: q rounded to fp32, rank = q (n_evict - 1) in fp32, the order statistics
+ *     at trunc(rank) and ceil(rank), and torch.lerp's two-branch formula (weight below 0.5: below + w (above - below),
+ *     else above - (above - below)(1 - w), each one fused multiply-add). Two -inf order statistics give thr = NaN, and
+ *     no entry of that row merges (q = 0.25 over [-inf, -inf, 0.2, 0.5, 0.9]).
+ *   - w(e) = clamp(max_sim, min=0) ok |V[e]| / (|V[e]| + |V[target]| + 1e-6), in this order in fp32 (|V| in fp32).
+ *   - acc_v(t) = sum of w(e) V[e] and acc_w(t) = sum of w(e) over the e with target(e) = t, both fp32, each product
+ *     rounded, in ASCENDING e (the order of the reference's CPU scatter_add_). Where acc_w > 0:
+ *     V_out[t] = (V[t] + acc_v) / (1 + acc_w), rounded once to the cache dtype; everywhere else V[t] bit for bit.
+ * NaN / inf: a NaN or inf key makes its similarities NaN (inf / inf), so a NaN or inf evicted key targets slot 0 and a
+ * NaN or inf kept key is the target of every evicted row whose earlier columns are numbers. A NaN max_sim never passes
+ * the gate but gives a NaN weight (clamp keeps NaN, NaN * 0 = NaN): its target's acc_w is NaN, and that row is left
+ * unmerged. So does an inf or NaN evicted value, whose norm makes its weight NaN, as in the reference.
+ * A zero key has similarity 0 with every column, so it targets slot 0 and passes a threshold of 0.
+ * Outputs: target_out (int32) and sim_out (fp32), both nullable, [B, Hkv, n_evict] contiguous: target and max_sim by
+ * evicted slot, target in kept-slot numbering. Two calls give bitwise-equal outputs, and a row's outputs do not depend
+ * on the batch it is in.
+ * kvp_merging_compress: the selection of kvp_scores_compress on `scores` (K_out, V_out, idx_out as there), then the merge
+ *   rewrites the n_kept rows of V_out. kvp_workspace_bytes(KVP_SCORER_MERGING) sizes its workspace; a compress takes 7
+ *   launches (memset, keys, select+compact, prologue, argmax, plan, merge), 6 when nothing is evicted.
+ * kvp_merging_merge: kept_idx int32 [B, Hkv, n_kept] contiguous, ascending and distinct in [0, S) (not checked);
+ *   V_out contiguous [B, Hkv, n_kept, D] gets the merged kept rows. Same workspace; 4 launches; K_out is not written.
+ * similarity_threshold in [0, 1] and merge_fraction in (0, 1], else KVP_ERR_BAD_ARGUMENT (NaN included). Every head_dim
+ * the problem validates. Memory beyond the workspace: none; no n_evict x n_kept tensor is formed.
+ * Check order (the first failure is returned): validate the problem -> (compress) n_kept == 0 returns KVP_OK ->
+ * K / V / K_out / V_out null and 16-byte alignment (compress) -> scores / score_stride null (compress); K, V, kept_idx,
+ * V_out null (merge) -> K, V, V_out 16-byte and kept_idx 4-byte alignment (merge) -> target_out, sim_out 4-byte alignment
+ * -> similarity_threshold -> merge_fraction -> workspace. A merge call with n_kept == 0 enqueues nothing. */
+int kvp_merging_compress(const kvp_problem* p, const void* scores, const int64_t* score_stride, const void* K,
+                         const void* V, float similarity_threshold, double merge_fraction, void* K_out, void* V_out,
+                         int32_t* idx_out, int32_t* target_out, float* sim_out, void* workspace,
+                         size_t workspace_bytes, kvp_stream_t stream);
+int kvp_merging_merge(const kvp_problem* p, const void* K, const void* V, const int32_t* kept_idx,
+                      float similarity_threshold, double merge_fraction, void* V_out, int32_t* target_out,
+                      float* sim_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

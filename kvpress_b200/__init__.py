@@ -20,6 +20,7 @@ from kvpress_b200.presses.key_rerotation_press import KeyRerotationPress
 from kvpress_b200.presses.keydiff_press import KeyDiffPress
 from kvpress_b200.presses.knorm_press import KnormPress
 from kvpress_b200.presses.lagkv_press import LagKVPress
+from kvpress_b200.presses.merging_press import MergingPress
 from kvpress_b200.presses.non_causal_attention_press import NonCausalAttnPress
 from kvpress_b200.presses.observed_attention_press import ObservedAttentionPress
 from kvpress_b200.presses.per_layer_compression_press import PerLayerCompressionPress
@@ -54,6 +55,7 @@ __all__ = [
     "NonCausalAttnPress",
     "LagKVPress",
     "CURPress",
+    "MergingPress",
     "BlockPress",
     "ChunkPress",
     "ChunkKVPress",

@@ -5,6 +5,9 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+#include <cstddef>
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace kvp {
@@ -85,6 +88,7 @@ static size_t layout(const Dims& d, int scorer, int window, void* base, Workspac
                        : scorer == KVP_SCORER_OBSERVED_ATTENTION ? observed_attention_scratch_bytes(d, window)
                        : scorer == KVP_SCORER_NON_CAUSAL_ATTENTION ? non_causal_attention_scratch_bytes(d)
                        : scorer == KVP_SCORER_CUR                  ? cur_scratch_bytes(d)
+                       : scorer == KVP_SCORER_MERGING              ? merging_scratch_bytes(d)
                                                                    : 0;
     ws->scorer = c.take<char>(ws->scorer_bytes);
     return c.bytes;
@@ -119,6 +123,8 @@ struct Io {
     void* V_out;
     int32_t* idx_out;
     const float* inv_freq;  // kvp_scores_compress_rerotate: the kept keys are re-rotated
+    // where the selection writes the kept positions when idx_out is null and a later stage reads them (MergingPress)
+    int32_t* (*kept_scratch)(const Dims&, const Workspace&) = nullptr;
 };
 
 enum class Kind {
@@ -142,11 +148,12 @@ static int prepare(Kind kind, const kvp_problem* p, int scorer, int window, cons
     return c->carve(scorer, window, workspace, workspace_bytes);
 }
 
-// prepare -> memset (unless zero == false) -> score -> selection (compress, select).
-// `score(const Call&)` enqueues the score stage and returns its cudaError_t.
-template <typename Operands, typename Score>
+// prepare -> memset (unless zero == false) -> score -> selection (compress, select) -> after (compress).
+// `score(const Call&)` enqueues the score stage and returns its cudaError_t; `after(const Call&, const int32_t* kept)`
+// enqueues a stage on the selection's output (the kept positions) and returns its cudaError_t.
+template <typename Operands, typename Score, typename After = std::nullptr_t>
 static int run(Kind kind, const kvp_problem* p, int scorer, int window, const Io& io, Operands operands, Score score,
-               void* workspace, size_t workspace_bytes, kvp_stream_t stream, bool zero = true) {
+               void* workspace, size_t workspace_bytes, kvp_stream_t stream, bool zero = true, After after = nullptr) {
     Call c;
     int rc = prepare(kind, p, scorer, window, io, operands, workspace, workspace_bytes, stream, &c);
     if (rc || (kind != Kind::score && c.d.n_kept == 0)) return rc;
@@ -156,8 +163,11 @@ static int run(Kind kind, const kvp_problem* p, int scorer, int window, const Io
     if (io.inv_freq)
         return status(launch_select_compact_rerotate(c.d, p->dtype, io.K, io.V, io.K_out, io.V_out, io.idx_out, c.ws,
                                                      io.inv_freq, c.st));
+    int32_t* idx = io.idx_out != nullptr || io.kept_scratch == nullptr ? io.idx_out : io.kept_scratch(c.d, c.ws);
     if (kind == Kind::select) c.d.ks = c.d.vs = {0, 0, 0};
-    return status(launch_select_compact(c.d, io.K, io.V, io.K_out, io.V_out, io.idx_out, c.ws, c.st));
+    if ((rc = status(launch_select_compact(c.d, io.K, io.V, io.K_out, io.V_out, idx, c.ws, c.st)))) return rc;
+    if constexpr (!std::is_same<After, std::nullptr_t>::value) return status(after(c, idx), scorer);
+    return KVP_OK;
 }
 
 static int no_operands(const Dims&) { return KVP_OK; }
@@ -256,6 +266,12 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         case KVP_SCORER_NON_CAUSAL_ATTENTION: *launches_out = 6; break;
         case KVP_SCORER_LAGKV: *launches_out = 3; break;  // memset, scores + keys, select+compact
         case KVP_SCORER_CUR: *launches_out = 4; break;  // memset, unit sums, finalize, select+compact
+        // memset, keys, select+compact, prologue, argmax (none when nothing is evicted), plan, merge
+        case KVP_SCORER_MERGING: {
+            Dims d;
+            *launches_out = validate(p, &d, false) == KVP_OK && p->n_kept == p->S ? 6 : 7;
+            break;
+        }
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -642,6 +658,52 @@ int kvp_scores_compress_rerotate(const kvp_problem* p, const void* scores, const
     };
     return run(Kind::compress, p, KVP_SCORER_GENERIC, 0, {K, V, K_out, V_out, idx_out, inv_freq}, operands,
                keys_from(p, scores, score_stride), workspace, workspace_bytes, stream);
+}
+
+// ---- Merging -------------------------------------------------------------------------------------------------------
+// The argument checks both entry points share, after their null / alignment checks. NaN fails every comparison.
+static int merging_args(float similarity_threshold, double merge_fraction) {
+    if (!(similarity_threshold >= 0.f && similarity_threshold <= 1.f)) return KVP_ERR_BAD_ARGUMENT;
+    return (merge_fraction > 0.0 && merge_fraction <= 1.0) ? KVP_OK : KVP_ERR_BAD_ARGUMENT;
+}
+
+static bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+
+int kvp_merging_compress(const kvp_problem* p, const void* scores, const int64_t* score_stride, const void* K,
+                         const void* V, float similarity_threshold, double merge_fraction, void* K_out, void* V_out,
+                         int32_t* idx_out, int32_t* target_out, float* sim_out, void* workspace,
+                         size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims&) -> int {
+        if (!scores || !score_stride) return KVP_ERR_NULL_POINTER;
+        if (!aligned4(target_out) || !aligned4(sim_out)) return KVP_ERR_BAD_STRIDE;
+        return merging_args(similarity_threshold, merge_fraction);
+    };
+    // the merge rewrites the kept rows of V_out from V and the kept positions
+    auto merge = [&](const Call& c, const int32_t* kept) {
+        return launch_merging(c.d, p->dtype, K, V, kept, similarity_threshold, merge_fraction, V_out, target_out,
+                              sim_out, c.ws, c.st);
+    };
+    const Io io = {K, V, K_out, V_out, idx_out, nullptr, merging_scratch_kept};
+    return run(Kind::compress, p, KVP_SCORER_MERGING, 0, io, operands, keys_from(p, scores, score_stride), workspace,
+               workspace_bytes, stream, true, merge);
+}
+
+int kvp_merging_merge(const kvp_problem* p, const void* K, const void* V, const int32_t* kept_idx,
+                      float similarity_threshold, double merge_fraction, void* V_out, int32_t* target_out,
+                      float* sim_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims&) -> int {
+        if (!K || !V || !kept_idx || !V_out) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(K) || !aligned16(V) || !aligned16(V_out) || !aligned4(kept_idx) || !aligned4(target_out) ||
+            !aligned4(sim_out))
+            return KVP_ERR_BAD_STRIDE;
+        return merging_args(similarity_threshold, merge_fraction);
+    };
+    auto merge = [&](const Call& c) {
+        return launch_merging(c.d, p->dtype, K, V, kept_idx, similarity_threshold, merge_fraction, V_out, target_out,
+                              sim_out, c.ws, c.st);
+    };
+    // no selection: nothing to clear
+    return run(Kind::score, p, KVP_SCORER_MERGING, 0, {}, operands, merge, workspace, workspace_bytes, stream, false);
 }
 
 }  // extern "C"

@@ -47,7 +47,7 @@ struct Workspace {
                          // zero = row not scanned yet
     int R;
     void* scorer;        // scorer-specific scratch (SnapKV / ExpectedAttention / KeyDiff / CriticalKV /
-                         // ObservedAttention / NonCausalAttention / CUR; LagKV needs none)
+                         // ObservedAttention / NonCausalAttention / CUR / Merging; LagKV needs none)
     size_t scorer_bytes;
     int S_pad;
     int n_tiles;
@@ -365,5 +365,10 @@ size_t cur_scratch_bytes(const Dims& d);
 cudaError_t launch_cur_score(const Dims& d, int dtype, const void* K, const void* V, int num_sinks, int leverage_type,
                              int window, const float* G, int r, const Workspace& ws, void* scores_out,
                              cudaStream_t st);
+size_t merging_scratch_bytes(const Dims& d);
+int32_t* merging_scratch_kept(const Dims& d, const Workspace& ws);
+cudaError_t launch_merging(const Dims& d, int dtype, const void* K, const void* V, const int32_t* kept, float threshold,
+                           double merge_fraction, void* V_out, int32_t* target_out, float* sim_out, const Workspace& ws,
+                           cudaStream_t st);
 
 }  // namespace kvp

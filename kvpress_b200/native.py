@@ -21,6 +21,7 @@ _LIB_PATH = Path(__file__).resolve().parent / _LIB_NAME
 (SCORER_GENERIC, SCORER_KNORM, SCORER_STREAMING, SCORER_SNAPKV, SCORER_EXPECTED_ATTENTION, SCORER_KEYDIFF,
  SCORER_CRITICALKV, SCORER_OBSERVED_ATTENTION, SCORER_NON_CAUSAL_ATTENTION, SCORER_LAGKV) = range(10)
 SCORER_CUR = 11  # KVP_SCORER_CUR; id 10 is not assigned
+SCORER_MERGING = 13  # KVP_SCORER_MERGING; id 12 is not assigned
 LAG_MAX = 1024  # the largest lag_size the LagKV kernel scores (kLagMax in csrc/common.cuh)
 CUR_WINDOW_MAX = 1024  # the largest local_window_size the CUR kernel scores (kCurWindowMax in csrc/common.cuh)
 CUR_RANK_MAX = 32  # the most projection columns the CUR kernel scores (kCurRankMax)
@@ -92,6 +93,9 @@ SIGNATURES = {
     "kvp_lagkv_compress": (ctypes.c_int, [_PP, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _SZ, _P]),
     "kvp_cur_score": (ctypes.c_int, [_PP, _P, _P, _I, _I, _I, _P, _I, _P, _P, _SZ, _P]),
     "kvp_cur_compress": (ctypes.c_int, [_PP, _P, _P, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_merging_compress": (
+        ctypes.c_int, [_PP, _P, _PI64, _P, _P, ctypes.c_float, ctypes.c_double, _P, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_merging_merge": (ctypes.c_int, [_PP, _P, _P, _P, ctypes.c_float, ctypes.c_double, _P, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -696,3 +700,64 @@ def cur_compress(keys, values, num_sinks: int, leverage_type: str, local_window_
     keys, values = _normalise(keys), _normalise(values)
     inputs = _cur_inputs(keys, values, num_sinks, leverage_type, local_window_size, G)
     return _compress("kvp_cur_compress", SCORER_CUR, keys, values, n_kept, inputs, return_indices, return_scores)
+
+
+# --------------------------------------------------------------------------------------------------
+# Merging (MergingPress: evicted values folded into their most cosine-similar kept row)
+# --------------------------------------------------------------------------------------------------
+def _merging_gate(similarity_threshold: float, merge_fraction: float) -> tuple:
+    if not 0.0 <= similarity_threshold <= 1.0:
+        raise ValueError(f"similarity_threshold must be in [0, 1], got {similarity_threshold}")
+    if not 0.0 < merge_fraction <= 1.0:
+        raise ValueError(f"merge_fraction must be in (0, 1], got {merge_fraction}")
+    return float(similarity_threshold), float(merge_fraction)
+
+
+def _merge_plan(keys: torch.Tensor, dev, n_evict: int, return_plan: bool):
+    """target_out / sim_out of a merging call: int32 and float32 [B, Hkv, n_evict], or None."""
+    if not return_plan:
+        return None, None
+    shape = (*keys.shape[:2], n_evict)
+    return (torch.empty(shape, dtype=torch.int32, device=dev), torch.empty(shape, dtype=torch.float32, device=dev))
+
+
+def merging_compress(scores: torch.Tensor, keys, values, similarity_threshold: float, merge_fraction: float,
+                     n_kept: int, return_indices: bool = False, return_plan: bool = False):
+    """MergingPress.compress (include/kvpress_b200.h, kvp_merging_compress): the n_kept best `scores` of every row are
+    kept, as scores_compress keeps them, and every evicted value is first folded into the kept row whose key is most
+    cosine-similar. Returns (k_out, v_out, idx, target, sim): idx with return_indices, and with return_plan the merge
+    plan (target in kept-slot numbering, int32, and max_sim, float32, [B, Hkv, S - n_kept]); None otherwise."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    scores, sstride = _caller_scores(scores, keys)
+    thr, frac = _merging_gate(similarity_threshold, merge_fraction)
+    B, H, S, D = keys.shape
+    dev = keys.device
+    k_out = torch.empty((B, H, n_kept, D), dtype=keys.dtype, device=dev)
+    v_out = torch.empty_like(k_out)
+    idx = torch.empty((B, H, n_kept), dtype=torch.int32, device=dev) if return_indices else None
+    target, sim = _merge_plan(keys, dev, S - n_kept, return_plan)
+    if n_kept > 0:
+        _enqueue("kvp_merging_compress", dev, make_problem(keys, values, n_kept), scores, sstride, keys, values, thr,
+                 frac, k_out, v_out, idx, target, sim, scorer=SCORER_MERGING)
+    return k_out, v_out, idx, target, sim
+
+
+def merging_merge(keys, values, kept_idx: torch.Tensor, similarity_threshold: float, merge_fraction: float,
+                  return_plan: bool = False):
+    """The merge alone (include/kvpress_b200.h, kvp_merging_merge) on caller kept positions kept_idx [B, Hkv, n_kept]
+    (ascending and distinct; cast to int32): the merged kept value rows [B, Hkv, n_kept, D], then the merge plan as in
+    merging_compress. Returns (v_out, target, sim)."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    thr, frac = _merging_gate(similarity_threshold, merge_fraction)
+    B, H, S, D = keys.shape
+    if kept_idx.dim() != 3 or tuple(kept_idx.shape[:2]) != (B, H) or kept_idx.shape[2] > S or kept_idx.device != keys.device:
+        raise RuntimeError(f"kept_idx must be [B, Hkv, n_kept <= {S}] on the cache device, got {tuple(kept_idx.shape)}")
+    kept_idx = kept_idx.to(torch.int32).contiguous()
+    n_kept = kept_idx.shape[2]
+    v_out = torch.empty((B, H, n_kept, D), dtype=values.dtype, device=keys.device)
+    target, sim = _merge_plan(keys, keys.device, S - n_kept, return_plan)
+    _enqueue("kvp_merging_merge", keys.device, make_problem(keys, values, n_kept), keys, values, kept_idx, thr, frac,
+             v_out, target, sim, scorer=SCORER_MERGING)
+    return v_out, target, sim
