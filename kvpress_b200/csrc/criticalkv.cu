@@ -81,9 +81,7 @@ criticalkv_kernel(const __grid_constant__ CUtensorMap mapV, const __grid_constan
                   int G, int S, int R, int n_tiles, int n_chunks, int n_workers, float eps) {
     using L = CkvSmem<D>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    // dynamic shared memory is only guaranteed 16-B aligned: round up to 1024 B for the swizzle
-    unsigned char* smem = reinterpret_cast<unsigned char*>(
-        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_v = smem + L::kVOff;
     unsigned char* s_w = smem + L::kWOff;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
@@ -225,23 +223,11 @@ static cudaError_t launch_criticalkv_t(const Dims& d, const void* V, const void*
     cudaError_t e = ensure_dynamic_smem(kern, smem, smem_set);
     if (e != cudaSuccess) return e;
     CUtensorMap mapV, mapW;
-    {
-        const uint64_t row_b = (uint64_t)d.vs.s * 2;
-        const uint64_t h_b = d.H > 1 ? (uint64_t)d.vs.h * 2 : row_b * (uint64_t)d.S;
-        const uint64_t b_b = d.B > 1 ? (uint64_t)d.vs.b * 2 : h_b * (uint64_t)d.H;
-        const uint64_t dims[4] = {(uint64_t)D, (uint64_t)d.S, (uint64_t)d.H, (uint64_t)d.B};
-        const uint64_t str[4] = {0, row_b, h_b, b_b};
-        const uint32_t box[4] = {64, (uint32_t)kCkvRows, 1, 1};
-        if ((e = make_tmap_16bit(&mapV, V, 4, dims, str, box)) != cudaSuccess) return e;
-    }
-    {
-        // Wo [hidden, wo_stride] as stored; rows past `hidden` read as zero and add nothing
-        const uint64_t row_b = (uint64_t)wo_stride * 2;
-        const uint64_t dims[3] = {(uint64_t)d.Hq * D, (uint64_t)hidden, 1};
-        const uint64_t str[3] = {0, row_b, row_b * (uint64_t)hidden};
-        const uint32_t box[3] = {64, (uint32_t)kCkvN, 1};
-        if ((e = make_tmap_16bit(&mapW, wo, 3, dims, str, box)) != cudaSuccess) return e;
-    }
+    if ((e = make_tmap_cache(&mapV, V, d, d.vs, kCkvRows)) != cudaSuccess) return e;
+    // Wo [hidden, wo_stride] as stored; rows past `hidden` read as zero and add nothing
+    if ((e = make_tmap_rows(&mapW, wo, (uint64_t)d.Hq * D, hidden, wo_stride, 1, (uint64_t)wo_stride * hidden,
+                            kCkvN)) != cudaSuccess)
+        return e;
     kern<<<n_workers, kCkvThreads, smem, st>>>(mapV, mapW, static_cast<const uint16_t*>(base), sb, sh,
                                                 static_cast<uint16_t*>(scores_out), d.H, d.Hq / d.H, d.S, d.R,
                                                 n_tiles, n_chunks, n_workers, eps);

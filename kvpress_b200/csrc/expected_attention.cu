@@ -579,21 +579,8 @@ static cudaError_t launch_ea_logits_t(const Dims& d, const void* K, const void* 
 
     CUtensorMap mapK, mapCov;
     cudaError_t e;
-    {
-        const uint64_t row_b = (uint64_t)d.ks.s * 2;
-        const uint64_t h_b = d.H > 1 ? (uint64_t)d.ks.h * 2 : row_b * (uint64_t)d.S;
-        const uint64_t b_b = d.B > 1 ? (uint64_t)d.ks.b * 2 : h_b * (uint64_t)d.H;
-        const uint64_t dims[4] = {(uint64_t)D, (uint64_t)d.S, (uint64_t)d.H, (uint64_t)d.B};
-        const uint64_t str[4] = {0, row_b, h_b, b_b};
-        const uint32_t box[4] = {64, (uint32_t)kEaTile, 1, 1};
-        if ((e = make_tmap_16bit(&mapK, K, 4, dims, str, box)) != cudaSuccess) return e;
-    }
-    {
-        const uint64_t dims[3] = {(uint64_t)D, (uint64_t)D, (uint64_t)d.B * d.Hq};
-        const uint64_t str[3] = {0, (uint64_t)D * 2, (uint64_t)D * D * 2};
-        const uint32_t box[3] = {64, (uint32_t)D, 1};
-        if ((e = make_tmap_16bit(&mapCov, cov, 3, dims, str, box)) != cudaSuccess) return e;
-    }
+    if ((e = make_tmap_cache(&mapK, K, d, d.ks, kEaTile)) != cudaSuccess) return e;
+    if ((e = make_tmap_rows(&mapCov, cov, D, D, D, (uint64_t)d.B * d.Hq, (uint64_t)D * D, D)) != cudaSuccess) return e;
     const int smem = L::kTotal + 1024;
     auto kern = ea_logits_kernel<T, D, GR>;
     static PerDeviceOnce smem_set;  // one per <T, D, GR> instantiation of this launcher

@@ -162,8 +162,7 @@ merging_argmax_kernel(const __grid_constant__ CUtensorMap mapE, const __grid_con
                       int n_kept, int n_evict, int R, MgScratch sc) {
     using L = SnSmem<DP, 128>;  // resident: 128 evicted rows; ring: 128 kept rows per stage
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>(
-        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_a = smem + L::kQOff;
     unsigned char* s_stage = smem + L::kStageOff;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
@@ -602,16 +601,11 @@ static cudaError_t launch_mg_argmax(const Dims& d, const MgScratch& sc, int S_pa
     const int grid = std::min(device_sm_count(), n_items);
     CUtensorMap mapE, mapT;
     cudaError_t e;
-    const uint64_t str[3] = {0, (uint64_t)DP * 2, (uint64_t)S_pad * DP * 2};
-    const uint32_t box[3] = {64, 128, 1};
-    {
-        const uint64_t dims[3] = {(uint64_t)DP, (uint64_t)n_evict, (uint64_t)d.R};
-        if ((e = make_tmap_16bit(&mapE, sc.keys + (size_t)d.n_kept * DP, 3, dims, str, box)) != cudaSuccess) return e;
-    }
-    {
-        const uint64_t dims[3] = {(uint64_t)DP, (uint64_t)d.n_kept, (uint64_t)d.R};
-        if ((e = make_tmap_16bit(&mapT, sc.keys, 3, dims, str, box)) != cudaSuccess) return e;
-    }
+    const uint64_t head_stride = (uint64_t)S_pad * DP;
+    if ((e = make_tmap_rows(&mapE, sc.keys + (size_t)d.n_kept * DP, DP, n_evict, DP, d.R, head_stride, 128)) !=
+        cudaSuccess)
+        return e;
+    if ((e = make_tmap_rows(&mapT, sc.keys, DP, d.n_kept, DP, d.R, head_stride, 128)) != cudaSuccess) return e;
     const int smem = L::kTotal + 1024;
     auto k = merging_argmax_kernel<T, DP>;
     static PerDeviceOnce smem_set;  // one per <T, DP> instantiation of this launcher

@@ -90,8 +90,7 @@ obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                  int S, int n_q, int qpos, int R, int n_blocks, float c, ObsScratch sc) {
     using L = SnSmem<D, NQP>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>(
-        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_q = smem + L::kQOff;
     unsigned char* s_stage = smem + L::kStageOff;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
@@ -169,41 +168,7 @@ obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                     for (int hh = 0; hh < 2; ++hh) {
                         const int r = mb * 64 + w4 * 16 + (lane >> 2) + 8 * hh;  // resident row
                         const int limit = off + p0 + r % qpos;                  // last visible key position
-                        // the running max is kept in raw units (q.k); c > 0 keeps the order and folds the scale into
-                        // one FFMA per element: exp2(fma(y, c, -m c))
-                        float v[32];
-#pragma unroll
-                        for (int jj = 0; jj < 16; ++jj) {
-                            v[2 * jj] = acc[4 * jj + 2 * hh];
-                            v[2 * jj + 1] = acc[4 * jj + 2 * hh + 1];
-                            if (!interior) {
-                                const int pos = key0 + 8 * jj;
-                                if (pos > limit || pos >= S) v[2 * jj] = -INFINITY;
-                                if (pos + 1 > limit || pos + 1 >= S) v[2 * jj + 1] = -INFINITY;
-                            }
-                        }
-                        float m16[16];
-#pragma unroll
-                        for (int jj = 0; jj < 16; ++jj) m16[jj] = fmaxf(v[jj], v[jj + 16]);
-#pragma unroll
-                        for (int jj = 0; jj < 8; ++jj) m16[jj] = fmaxf(m16[jj], m16[jj + 8]);
-#pragma unroll
-                        for (int jj = 0; jj < 4; ++jj) m16[jj] = fmaxf(m16[jj], m16[jj + 4]);
-                        const float m = run_m[i][hh];
-                        const float m_new = fmaxf(m, fmaxf(fmaxf(m16[0], m16[2]), fmaxf(m16[1], m16[3])));
-                        if (m_new > -INFINITY) {
-                            const float neg = -m_new * c;
-                            float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;  // four independent sum chains
-#pragma unroll
-                            for (int jj = 0; jj < 32; jj += 4) {
-                                a0 += fast_exp2(fmaf(v[jj], c, neg));
-                                a1 += fast_exp2(fmaf(v[jj + 1], c, neg));
-                                a2 += fast_exp2(fmaf(v[jj + 2], c, neg));
-                                a3 += fast_exp2(fmaf(v[jj + 3], c, neg));
-                            }
-                            run_z[i][hh] = run_z[i][hh] * fast_exp2((m - m_new) * c) + ((a0 + a1) + (a2 + a3));
-                            run_m[i][hh] = m_new;
-                        }
+                        online_row_update(acc, hh, c, interior, key0, limit, S, run_m[i][hh], run_z[i][hh]);
                     }
                 }
                 __syncwarp();
@@ -215,14 +180,7 @@ obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
 #pragma unroll
                 for (int hh = 0; hh < 2; ++hh) {
                     float m = run_m[i][hh], z = run_z[i][hh];
-#pragma unroll
-                    for (int o = 1; o <= 2; o <<= 1) {  // the four threads of a row
-                        const float m2 = __shfl_xor_sync(0xFFFFFFFFu, m, o);
-                        const float z2 = __shfl_xor_sync(0xFFFFFFFFu, z, o);
-                        const float mn = fmaxf(m, m2);
-                        z = (mn == -INFINITY) ? 0.f : z * fast_exp2((m - mn) * c) + z2 * fast_exp2((m2 - mn) * c);
-                        m = mn;
-                    }
+                    quad_merge(m, z, c);
                     const int r = (2 * i + cw) * 64 + w4 * 16 + (lane >> 2) + 8 * hh;
                     const int g = r / qpos, pos = p0 + r % qpos;
                     if (qd == 0 && g < G && pos < n_q)
@@ -244,8 +202,7 @@ obs_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                   int S, int n_q, int R, int n_ktiles, float c, ObsScratch sc, int S_pad) {
     using L = ObsColSmem<D>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>(
-        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_k = smem + L::kKOff;
     unsigned char* s_stage = smem + L::kStageOff;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
@@ -356,11 +313,7 @@ obs_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
             // every MMA on the K tile has completed: hand it back to the producer
             __syncwarp();
             if (lane == 0) umma::mbar_arrive(k_empty);
-#pragma unroll
-            for (int o = 1; o <= 2; o <<= 1) {
-                tot0 += __shfl_xor_sync(0xFFFFFFFFu, tot0, o);
-                tot1 += __shfl_xor_sync(0xFFFFFFFFu, tot1, o);
-            }
+            quad_sum(tot0, tot1);
             if (qd == 0 && key < S) sc.colsum[(size_t)row * S_pad + key] = tot0;
             if (qd == 0 && key + 8 < S) sc.colsum[(size_t)row * S_pad + key + 8] = tot1;
         }
@@ -409,24 +362,11 @@ static cudaError_t launch_obs_t(const Dims& d, const void* K, const void* q, int
 
     CUtensorMap mapK, mapQ1, mapQ2;
     cudaError_t e;
-    {
-        const uint64_t row_b = (uint64_t)d.ks.s * 2;
-        const uint64_t h_b = d.H > 1 ? (uint64_t)d.ks.h * 2 : row_b * (uint64_t)d.S;
-        const uint64_t b_b = d.B > 1 ? (uint64_t)d.ks.b * 2 : h_b * (uint64_t)d.H;
-        const uint64_t dims[4] = {(uint64_t)D, (uint64_t)d.S, (uint64_t)d.H, (uint64_t)d.B};
-        const uint64_t str[4] = {0, row_b, h_b, b_b};
-        const uint32_t box[4] = {64, (uint32_t)kSnTile, 1, 1};
-        if ((e = make_tmap_16bit(&mapK, K, 4, dims, str, box)) != cudaSuccess) return e;
-    }
-    {
-        // q [B Hq, n_q, D] contiguous: rows past n_q of a head read as zero
-        const uint64_t dims[3] = {(uint64_t)D, (uint64_t)n_q, (uint64_t)d.B * d.Hq};
-        const uint64_t str[3] = {0, (uint64_t)D * 2, (uint64_t)n_q * D * 2};
-        const uint32_t box1[3] = {64, (uint32_t)qpos, 1};
-        const uint32_t box2[3] = {64, (uint32_t)kSnTile, 1};
-        if ((e = make_tmap_16bit(&mapQ1, q, 3, dims, str, box1)) != cudaSuccess) return e;
-        if ((e = make_tmap_16bit(&mapQ2, q, 3, dims, str, box2)) != cudaSuccess) return e;
-    }
+    if ((e = make_tmap_cache(&mapK, K, d, d.ks, kSnTile)) != cudaSuccess) return e;
+    // q [B Hq, n_q, D] contiguous: rows past n_q of a head read as zero
+    const uint64_t n_heads = (uint64_t)d.B * d.Hq, head_stride = (uint64_t)n_q * D;
+    if ((e = make_tmap_rows(&mapQ1, q, D, n_q, D, n_heads, head_stride, qpos)) != cudaSuccess) return e;
+    if ((e = make_tmap_rows(&mapQ2, q, D, n_q, D, n_heads, head_stride, kSnTile)) != cudaSuccess) return e;
     const int smem1 = L1::kTotal + 1024, smem2 = L2::kTotal + 1024;
     auto k1 = obs_stats_kernel<T, D, NQP>;
     auto k2 = obs_colsum_kernel<T, D>;

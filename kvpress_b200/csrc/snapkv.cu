@@ -85,8 +85,7 @@ snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                   SnapScratch sc) {
     using L = SnSmem<D, NQP>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>(
-        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_q = smem + L::kQOff;
     unsigned char* s_stage = smem + L::kStageOff;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
@@ -155,41 +154,7 @@ snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                     for (int hh = 0; hh < 2; ++hh) {
                         const int r = mb * 64 + w4 * 16 + (lane >> 2) + 8 * hh;  // query row
                         const int limit = (S - window) + (r % window);          // last visible key position
-                        // running max is kept in RAW logit units (q.k); c > 0 so the order is the same and the
-                        // scale folds into one FFMA per element: exp2(fma(y, c, -m*c))
-                        float v[32];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                            v[2 * j] = acc[4 * j + 2 * hh];
-                            v[2 * j + 1] = acc[4 * j + 2 * hh + 1];
-                            if (!interior) {
-                                const int pos = key0 + 8 * j;
-                                if (pos > limit || pos >= S) v[2 * j] = -INFINITY;
-                                if (pos + 1 > limit || pos + 1 >= S) v[2 * j + 1] = -INFINITY;
-                            }
-                        }
-                        float m16[16];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) m16[j] = fmaxf(v[j], v[j + 16]);
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) m16[j] = fmaxf(m16[j], m16[j + 8]);
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) m16[j] = fmaxf(m16[j], m16[j + 4]);
-                        const float m = run_m[i][hh];
-                        const float m_new = fmaxf(m, fmaxf(fmaxf(m16[0], m16[2]), fmaxf(m16[1], m16[3])));
-                        if (m_new > -INFINITY) {
-                            const float neg = -m_new * c;
-                            float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;  // four independent sum chains
-#pragma unroll
-                            for (int j = 0; j < 32; j += 4) {
-                                a0 += fast_exp2(fmaf(v[j], c, neg));
-                                a1 += fast_exp2(fmaf(v[j + 1], c, neg));
-                                a2 += fast_exp2(fmaf(v[j + 2], c, neg));
-                                a3 += fast_exp2(fmaf(v[j + 3], c, neg));
-                            }
-                            run_z[i][hh] = run_z[i][hh] * fast_exp2((m - m_new) * c) + ((a0 + a1) + (a2 + a3));
-                            run_m[i][hh] = m_new;
-                        }
+                        online_row_update(acc, hh, c, interior, key0, limit, S, run_m[i][hh], run_z[i][hh]);
                     }
                 }
                 __syncwarp();
@@ -201,14 +166,7 @@ snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
 #pragma unroll
                 for (int hh = 0; hh < 2; ++hh) {
                     float m = run_m[i][hh], z = run_z[i][hh];
-#pragma unroll
-                    for (int off = 1; off <= 2; off <<= 1) {  // the four threads of a row
-                        const float m2 = __shfl_xor_sync(0xFFFFFFFFu, m, off);
-                        const float z2 = __shfl_xor_sync(0xFFFFFFFFu, z, off);
-                        const float mn = fmaxf(m, m2);
-                        z = (mn == -INFINITY) ? 0.f : z * fast_exp2((m - mn) * c) + z2 * fast_exp2((m2 - mn) * c);
-                        m = mn;
-                    }
+                    quad_merge(m, z, c);
                     const int r = (2 * i + cw) * 64 + w4 * 16 + (lane >> 2) + 8 * hh;
                     if (qd == 0 && r < NQ)
                         sc.partial[((size_t)row * NQ + r) * n_parts + part] = make_float2(m * c, z);  // (max in log2 units, sum)
@@ -229,8 +187,7 @@ snap_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_consta
                    SnapScratch sc, int S_pad) {
     using L = SnSmem<D, NQP>;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    unsigned char* smem = reinterpret_cast<unsigned char*>(
-        (reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_q = smem + L::kQOff;
     unsigned char* s_stage = smem + L::kStageOff;
     float* s_cb = reinterpret_cast<float*>(smem + L::kCbOff);
@@ -306,25 +263,11 @@ snap_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_consta
                     if (nc * 128 >= NQ) break;  // warpgroup-uniform
                     float acc[64];
                     snap_mma<T, D>(acc, kb, kSnTile * 128, umma::smem_u32(s_q + nc * 128 * 128), L::kQPanel);
-                    float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float2 cb = *reinterpret_cast<const float2*>(&s_cb[nc * 128 + 8 * j + 2 * qd]);
-                        a0 += fast_exp2(fmaf(acc[4 * j], c, cb.x));
-                        a1 += fast_exp2(fmaf(acc[4 * j + 1], c, cb.y));
-                        a2 += fast_exp2(fmaf(acc[4 * j + 2], c, cb.x));
-                        a3 += fast_exp2(fmaf(acc[4 * j + 3], c, cb.y));
-                    }
-                    tot0 += a0 + a1;
-                    tot1 += a2 + a3;
+                    colsum_tile(acc, s_cb + nc * 128, qd, c, tot0, tot1);
                 }
                 __syncwarp();
                 if (lane == 0) umma::mbar_arrive(&k_empty[stage]);
-#pragma unroll
-                for (int off = 1; off <= 2; off <<= 1) {
-                    tot0 += __shfl_xor_sync(0xFFFFFFFFu, tot0, off);
-                    tot1 += __shfl_xor_sync(0xFFFFFFFFu, tot1, off);
-                }
+                quad_sum(tot0, tot1);
                 const int pos = t * kSnTile + cw * 64 + w4 * 16 + (lane >> 2);
                 if (qd == 0 && pos < S - window) sc.colsum[(size_t)row * S_pad + pos] = tot0;
                 if (qd == 0 && pos + 8 < S - window) sc.colsum[(size_t)row * S_pad + pos + 8] = tot1;
@@ -411,30 +354,15 @@ static cudaError_t launch_snap_t(const Dims& d, int dtype, const void* K, const 
     const int n_parts = ctas_per_row;  // one (max, sum) per query row and CTA of the row
 
     CUtensorMap mapK, mapQ;
-    {
-        const uint64_t row_b = (uint64_t)d.ks.s * 2;
-        const uint64_t h_b = d.H > 1 ? (uint64_t)d.ks.h * 2 : row_b * (uint64_t)d.S;
-        const uint64_t b_b = d.B > 1 ? (uint64_t)d.ks.b * 2 : h_b * (uint64_t)d.H;
-        const uint64_t dims[4] = {(uint64_t)D, (uint64_t)d.S, (uint64_t)d.H, (uint64_t)d.B};
-        const uint64_t str[4] = {0, row_b, h_b, b_b};
-        const uint32_t box[4] = {64, (uint32_t)kSnTile, 1, 1};
-        cudaError_t e = make_tmap_16bit(&mapK, K, 4, dims, str, box);
-        if (e != cudaSuccess) return e;
-    }
-    {
-        const uint64_t rows = (uint64_t)d.B * d.Hq * window;
-        const uint64_t dims[3] = {(uint64_t)D, rows, 1};
-        const uint64_t str[3] = {0, (uint64_t)D * 2, rows * D * 2};
-        const uint32_t box[3] = {64, (uint32_t)(NQP < 256 ? NQP : 256), 1};
-        cudaError_t e = make_tmap_16bit(&mapQ, q_window, 3, dims, str, box);
-        if (e != cudaSuccess) return e;
-    }
+    cudaError_t e;
+    if ((e = make_tmap_cache(&mapK, K, d, d.ks, kSnTile)) != cudaSuccess) return e;
+    const uint64_t rows = (uint64_t)d.B * d.Hq * window;
+    if ((e = make_tmap_rows(&mapQ, q_window, D, rows, D, 1, rows * D, NQP < 256 ? NQP : 256)) != cudaSuccess) return e;
     const int smem = L::kTotal + 1024;
     auto k1 = snap_stats_kernel<T, D, NQP>;
     auto k2 = snap_colsum_kernel<T, D, NQP>;
     static PerDeviceOnce smem_set1, smem_set2;  // one pair per <T, D, NQP> instantiation of this launcher
-    cudaError_t e = ensure_dynamic_smem(k1, smem, smem_set1);
-    if (e != cudaSuccess) return e;
+    if ((e = ensure_dynamic_smem(k1, smem, smem_set1)) != cudaSuccess) return e;
     e = ensure_dynamic_smem(k2, smem, smem_set2);
     if (e != cudaSuccess) return e;
 

@@ -52,4 +52,22 @@ cudaError_t make_tmap_16bit(CUtensorMap* map, const void* base, int rank, const 
     return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
+cudaError_t make_tmap_cache(CUtensorMap* map, const void* base, const Dims& d, const Strides3& s, uint32_t box_rows) {
+    const uint64_t row_b = (uint64_t)s.s * 2;
+    const uint64_t h_b = d.H > 1 ? (uint64_t)s.h * 2 : row_b * (uint64_t)d.S;
+    const uint64_t b_b = d.B > 1 ? (uint64_t)s.b * 2 : h_b * (uint64_t)d.H;
+    const uint64_t dims[4] = {(uint64_t)d.D, (uint64_t)d.S, (uint64_t)d.H, (uint64_t)d.B};
+    const uint64_t str[4] = {0, row_b, h_b, b_b};
+    const uint32_t box[4] = {64, box_rows, 1, 1};
+    return make_tmap_16bit(map, base, 4, dims, str, box);
+}
+
+cudaError_t make_tmap_rows(CUtensorMap* map, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride,
+                           uint64_t heads, uint64_t head_stride, uint32_t box_rows) {
+    const uint64_t dims[3] = {cols, rows, heads};
+    const uint64_t str[3] = {0, row_stride * 2, head_stride * 2};
+    const uint32_t box[3] = {64, box_rows, 1};
+    return make_tmap_16bit(map, base, 3, dims, str, box);
+}
+
 }  // namespace kvp

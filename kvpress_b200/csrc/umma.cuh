@@ -13,6 +13,11 @@ namespace umma {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);
 }
+// Dynamic shared memory is only guaranteed 16-B aligned: round up to the 1024 B a SWIZZLE_128B panel needs (the
+// launchers request 1024 B more than the layout uses).
+__device__ __forceinline__ unsigned char* smem_align_1024(unsigned char* smem_raw) {
+    return reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+}
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
 }
@@ -218,5 +223,14 @@ kvp_encode_tiled_fn get_encode_tiled();
 // out-of-bounds elements read as zero. dims/strides innermost-first; strides[0] is implicit.
 cudaError_t make_tmap_16bit(CUtensorMap* map, const void* base, int rank, const uint64_t* dims,
                             const uint64_t* strides_bytes, const uint32_t* box);
+struct Dims;
+struct Strides3;
+// rank-4 map of a [B, H, S, D] cache with element strides s (a cache's stride of a size-1 dim may be anything, so
+// H == 1 and B == 1 take the dense one); a box is 64 columns x box_rows positions of one (b, h).
+cudaError_t make_tmap_cache(CUtensorMap* map, const void* base, const Dims& d, const Strides3& s, uint32_t box_rows);
+// rank-3 map of `heads` matrices [rows x cols], element strides row_stride and head_stride; a box is 64 columns x
+// box_rows rows of one head.
+cudaError_t make_tmap_rows(CUtensorMap* map, const void* base, uint64_t cols, uint64_t rows, uint64_t row_stride,
+                           uint64_t heads, uint64_t head_stride, uint32_t box_rows);
 
 }  // namespace kvp
