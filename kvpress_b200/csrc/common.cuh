@@ -4,7 +4,10 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "../../include/kvpress_b200.h"
 
@@ -71,6 +74,17 @@ __host__ __device__ __forceinline__ uint16_t key16_to_bits(uint16_t key) {
     return (key & 0x8000u) ? (uint16_t)(key & 0x7FFFu) : (uint16_t)(~key);
 }
 
+// ---- float -> order-preserving uint32 image, and back --------------------------------------------
+// Unsigned comparison of images is the float order, with -0 below +0 and NaNs outside +-inf by their sign bit; zero
+// (the value counters are cleared to) is below every image of a number, so atomicMax on it works from a cleared slot.
+__device__ __forceinline__ uint32_t ordered_f32(float f) {
+    const uint32_t u = __float_as_uint(f);
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float ordered_f32_to_float(uint32_t k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+}
+
 template <typename T>
 struct F16Traits;
 template <>
@@ -102,6 +116,31 @@ struct F16Traits<__half> {
     static constexpr uint16_t kInfBits = 0x7C00u;
     static constexpr int kMmaFormat = 0;  // F16
 };
+
+// ---- host: the two dispatches every launcher shares -------------------------------------------------------------
+// Calls f with a value of the cache's 16-bit type (KVP_BF16 or KVP_F16; api.cu rejects any other dtype).
+template <typename F>
+static inline decltype(auto) with_dtype(int dtype, F&& f) {
+    if (dtype == KVP_BF16) return f(__nv_bfloat16{});
+    return f(__half{});
+}
+
+// Lanes that cover one cache row with 16-byte loads (8 elements per lane), as instantiated by the CUDA-core score
+// kernels: a row of D <= 256 elements takes the first entry >= D / 8. The tests read this list.
+constexpr int kLanesPerRow[] = {4, 8, 16, 32};
+constexpr int kNumLanesPerRow = sizeof(kLanesPerRow) / sizeof(kLanesPerRow[0]);
+
+// Calls f with std::integral_constant<int, LPR> of the lane count of head_dim D.
+template <int I = 0, typename F>
+static inline void with_lanes_per_row(int D, F&& f) {
+    constexpr int lpr = kLanesPerRow[I];
+    if constexpr (I + 1 == kNumLanesPerRow) {
+        f(std::integral_constant<int, lpr>{});
+    } else {
+        if (D / 8 <= lpr) f(std::integral_constant<int, lpr>{});
+        else with_lanes_per_row<I + 1>(D, f);
+    }
+}
 
 // ---- cache-hinted 128-bit global accesses ---------------------------------------------------
 // 128-bit accesses take an explicit createpolicy handle through .L2::cache_hint.
@@ -210,17 +249,22 @@ __device__ __forceinline__ void flush_row_hist(const uint32_t* shist, int row, c
     }
 }
 
+// Adds each lane's bin (256: none) to the shared histogram. The atomics are warp-aggregated with match.any so heavily
+// tied scores (bf16 norms take ~100 distinct values) do not serialise on one address. Every lane of the warp calls it.
+__device__ __forceinline__ void warp_hist_add(uint32_t* shist, unsigned bin) {
+    const unsigned peers = __match_any_sync(0xFFFFFFFFu, bin);
+    if (bin < 256u && (threadIdx.x & 31) == (__ffs(peers) - 1)) atomicAdd(&shist[bin], __popc(peers));
+}
+
 // Common tail of every score kernel: KPT keys (and optionally scores) per thread staged in shared
 // memory for a chunk of KPT*blockDim positions starting at s_begin -> coalesced global writes + row
-// histogram of (key >> 8). Shared-memory atomics are warp-aggregated with match.any so heavily tied
-// scores (bf16 norms take ~100 distinct values) do not serialise on one address.
+// histogram of (key >> 8).
 // Call with all threads of a 256-thread CTA after a __syncthreads(); shist must be zeroed.
 template <int KPT, bool kFlushHist = true>
 __device__ __forceinline__ void flush_chunk_keys(const uint16_t* skeys, const uint16_t* sscores,
                                                  uint32_t* shist, int row, int s_begin, int S,
                                                  const Workspace& ws, uint16_t* scores_out) {
     const int tid = threadIdx.x;
-    const int lane = tid & 31;
     const int s0 = s_begin + tid * KPT;
     uint16_t k[KPT];
 #pragma unroll
@@ -246,14 +290,83 @@ __device__ __forceinline__ void flush_chunk_keys(const uint16_t* skeys, const ui
             if (s0 + i < S) dst[i] = sscores[tid * KPT + i];
     }
 #pragma unroll
-    for (int i = 0; i < KPT; ++i) {
-        const unsigned bin = ((s0 + i) < S) ? (unsigned)(k[i] >> 8) : 256u;
-        const unsigned peers = __match_any_sync(0xFFFFFFFFu, bin);
-        if (bin < 256u && lane == (__ffs(peers) - 1)) atomicAdd(&shist[bin], __popc(peers));
-    }
+    for (int i = 0; i < KPT; ++i) warp_hist_add(shist, ((s0 + i) < S) ? (unsigned)(k[i] >> 8) : 256u);
     if (kFlushHist) {
         __syncthreads();
         flush_row_hist(shist, row, ws);
+    }
+}
+
+// ---- the end of every score stage ------------------------------------------------------------------------------
+// What the select + compact stage reads: each score rounded once to the cache dtype, its ordered key in ws.keys and
+// the histogram of the key's high byte in ws.hist_hi.
+
+// The one rounding: fp32 values as the presses define them, fp64 where a press evaluates its score in double.
+template <typename T>
+__device__ __forceinline__ uint16_t round_once(float v) {
+    return F16Traits<T>::from_float(v);
+}
+template <typename T>
+__device__ __forceinline__ uint16_t round_once(double v) {
+    if constexpr (std::is_same<T, __nv_bfloat16>::value) return __bfloat16_as_ushort(__double2bfloat16(v));
+    else return __half_as_ushort(__double2half(v));
+}
+
+// A score tile of a 256-thread CTA: thread tid owns positions s = s_begin + tid * KPT + i, i < KPT. Below S, a
+// position in [forced_lo, forced_hi) is forced (key kForcedKey, score 0); any other gets value(i, s) rounded once and
+// its ordered key. Both are staged in skeys / sscores (KPT * 256 each), then the keys, the scores (scores_out may be
+// null) and the histogram go out through flush_chunk_keys; shist must be zeroed. Unless max_valid is null, raises
+// *max_valid to the largest rounded score of the thread's unforced positions (see publish_max_valid).
+template <typename T, int KPT, bool kFlushHist = true, typename Value>
+__device__ __forceinline__ void score_tile_epilogue(uint16_t* skeys, uint16_t* sscores, uint32_t* shist, int row,
+                                                    int s_begin, int S, int forced_lo, int forced_hi,
+                                                    const Workspace& ws, uint16_t* scores_out, float* max_valid,
+                                                    Value value) {
+    const int tid = threadIdx.x;
+#pragma unroll
+    for (int i = 0; i < KPT; ++i) {
+        const int s = s_begin + tid * KPT + i;
+        uint16_t bits = 0, key = 0;
+        if (s < S) {
+            if (s >= forced_lo && s < forced_hi) {
+                key = kForcedKey;
+            } else {
+                bits = round_once<T>(value(i, s));
+                key = ordered_key16(bits, F16Traits<T>::kInfBits);
+                if (max_valid) *max_valid = fmaxf(*max_valid, F16Traits<T>::to_float(bits));
+            }
+        }
+        skeys[tid * KPT + i] = key;
+        sscores[tid * KPT + i] = bits;
+    }
+    __syncthreads();
+    flush_chunk_keys<KPT, kFlushHist>(skeys, sscores, shist, row, s_begin, S, ws, scores_out);
+}
+
+// Score kernels that stage their own keys (one position per thread): keys, scores and histogram for a compress
+// call (want_keys), the scores alone for a score-only call. Call after a __syncthreads().
+__device__ __forceinline__ void flush_or_store_scores(const uint16_t* skeys, const uint16_t* sscores, uint32_t* shist,
+                                                      int row, int s_begin, int S, const Workspace& ws,
+                                                      uint16_t* scores_out, bool want_keys) {
+    const int tid = threadIdx.x;
+    if (want_keys) flush_chunk_keys<1>(skeys, sscores, shist, row, s_begin, S, ws, scores_out);
+    else if (s_begin + tid < S) scores_out[(size_t)row * S + s_begin + tid] = sscores[tid];
+}
+
+// Raises counters[kCounterMaxSlot] to the CTA's largest valid score m (-inf: none), for the reference's max + 1
+// sentinel that fill_sentinel_kernel writes. Call with all threads of a 256-thread CTA; the CTA's shared histogram may
+// be flushed after it returns.
+__device__ __forceinline__ void publish_max_valid(float m, const Workspace& ws) {
+    __shared__ float s_max[kTileThreads / 32];
+    const int tid = threadIdx.x;
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, off));
+    if ((tid & 31) == 0) s_max[tid >> 5] = m;
+    __syncthreads();
+    if (tid == 0) {
+        m = s_max[0];
+        for (int w = 1; w < kTileThreads / 32; ++w) m = fmaxf(m, s_max[w]);
+        if (m > -INFINITY) atomicMax(&ws.counters[kCounterMaxSlot(ws.R)], ordered_f32(m));
     }
 }
 

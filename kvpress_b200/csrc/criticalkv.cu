@@ -249,18 +249,16 @@ cudaError_t launch_criticalkv_score(const Dims& d, int dtype, const void* V, con
         if ((e = launch_select_compact(ds, nullptr, nullptr, nullptr, nullptr, sc.first, ws, st)) != cudaSuccess)
             return e;
     }
-    const bool bf16 = dtype == KVP_BF16;
-    if (d.D == 128)
-        e = bf16 ? launch_criticalkv_t<__nv_bfloat16, 128>(d, V, base, sb, sh, wo, hidden, wo_stride, eps, scores_out, st)
-                 : launch_criticalkv_t<__half, 128>(d, V, base, sb, sh, wo, hidden, wo_stride, eps, scores_out, st);
-    else
-        e = bf16 ? launch_criticalkv_t<__nv_bfloat16, 64>(d, V, base, sb, sh, wo, hidden, wo_stride, eps, scores_out, st)
-                 : launch_criticalkv_t<__half, 64>(d, V, base, sb, sh, wo, hidden, wo_stride, eps, scores_out, st);
+    e = with_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        if (d.D == 128) return launch_criticalkv_t<T, 128>(d, V, base, sb, sh, wo, hidden, wo_stride, eps, scores_out, st);
+        return launch_criticalkv_t<T, 64>(d, V, base, sb, sh, wo, hidden, wo_stride, eps, scores_out, st);
+    });
     if (e != cudaSuccess || n_first == 0) return e;
     const long long n = (long long)d.R * n_first;
     const int blocks = (int)(n < 256 * 1024 ? (n + 255) / 256 : 1024);
     criticalkv_force_kernel<<<blocks, 256, 0, st>>>(static_cast<uint16_t*>(scores_out), d.S, sc.first, n_first, d.R,
-                                                    bf16 ? (uint16_t)0x7F7Fu : (uint16_t)0x7BFFu);
+                                                    dtype == KVP_BF16 ? (uint16_t)0x7F7Fu : (uint16_t)0x7BFFu);
     return cudaPeekAtLastError();
 }
 

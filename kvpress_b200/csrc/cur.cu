@@ -211,17 +211,9 @@ cur_finalize_kernel(int S, int n_units, int num_sinks, CurScratch sc, Workspace 
     double t = 0.0;
     for (int i = tid; i < n_units; i += kTileThreads) t += sc.partials[(size_t)row * sc.part_stride + i];
     const double total = cur_block_sum(t, red);
-    const int s = tile * kTile + tid;
-    uint16_t bits = 0, key = 0;
-    if (s < S) {
-        const float value = s < num_sinks ? 1.f : (float)((double)sc.u[(size_t)row * S + s] / total);
-        bits = F16Traits<T>::from_float(value);
-        key = ordered_key16(bits, F16Traits<T>::kInfBits);
-    }
-    skeys[tid] = key;
-    sscores[tid] = bits;
-    __syncthreads();
-    flush_chunk_keys<1>(skeys, sscores, shist, row, tile * kTile, S, ws, scores_out);
+    score_tile_epilogue<T, 1>(skeys, sscores, shist, row, tile * kTile, S, 0, 0, ws, scores_out, nullptr, [&](int, int s) {
+        return s < num_sinks ? 1.f : (float)((double)sc.u[(size_t)row * S + s] / total);
+    });
 }
 
 template <typename T>
@@ -232,13 +224,7 @@ static cudaError_t launch_cur_t(const CurArgs& a, const Dims& d, int num_sinks, 
     if (a.r > 0) {
         cur_unit_kernel<T, 4, true><<<grid, kCurThreads, (size_t)a.D * kCurGCols * sizeof(float), st>>>(a);
     } else {
-        const int nvec = a.D / 8;
-#define KVP_CUR(LPR) cur_unit_kernel<T, LPR, false><<<grid, kCurThreads, 0, st>>>(a)
-        if (nvec <= 4) KVP_CUR(4);
-        else if (nvec <= 8) KVP_CUR(8);
-        else if (nvec <= 16) KVP_CUR(16);
-        else KVP_CUR(32);
-#undef KVP_CUR
+        with_lanes_per_row(a.D, [&](auto lpr) { cur_unit_kernel<T, lpr, false><<<grid, kCurThreads, 0, st>>>(a); });
     }
     cudaError_t e = cudaPeekAtLastError();
     if (e != cudaSuccess) return e;
@@ -271,8 +257,7 @@ cudaError_t launch_cur_score(const Dims& d, int dtype, const void* K, const void
     a.u = sc.u;
     a.partials = sc.partials;
     a.part_stride = sc.part_stride;
-    if (dtype == KVP_BF16) return launch_cur_t<__nv_bfloat16>(a, d, num_sinks, sc, ws, scores_out, st);
-    return launch_cur_t<__half>(a, d, num_sinks, sc, ws, scores_out, st);
+    return with_dtype(dtype, [&](auto t) { return launch_cur_t<decltype(t)>(a, d, num_sinks, sc, ws, scores_out, st); });
 }
 
 }  // namespace kvp

@@ -438,7 +438,6 @@ ea_finalize_kernel(int G, int S, int n_sink, int use_vnorm, float eps, int n_par
     __shared__ uint16_t sscores[kEaFinalPos];
     __shared__ uint32_t shist[256];
     __shared__ float s_m[8], s_iz[8];
-    __shared__ float s_max[8];
     const int chunk = blockIdx.x, row = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     shist[tid] = 0;
     pdl_launch_dependents();  // the select+compact kernel behind this one may start to take residency
@@ -477,52 +476,22 @@ ea_finalize_kernel(int G, int S, int n_sink, int use_vnorm, float eps, int n_par
         }
     }
     __syncthreads();
-    float fmax_valid = -INFINITY;
     const float vn[4] = {vn4.x, vn4.y, vn4.z, vn4.w};
+    float fmax_valid = -INFINITY;
+    score_tile_epilogue<T, KPT, false>(
+        skeys, sscores, shist, row, chunk * kEaFinalPos, S, 0, n_sink, ws, scores_out, &fmax_valid, [&](int i, int) {
+            float p = 0.f;
 #pragma unroll
-    for (int i = 0; i < KPT; ++i) {
-        const int s = s0 + i;
-        uint16_t bits = 0, key = 0;
-        if (s < S) {
-            if (s < n_sink) {
-                key = kForcedKey;
-            } else {
-                float p = 0.f;
-#pragma unroll
-                for (int g = 0; g < 8; ++g) {
-                    if (g < G) {
-                        const float l = (i == 0) ? lg[g].x : (i == 1) ? lg[g].y : (i == 2) ? lg[g].z : lg[g].w;
-                        p += __expf(l - s_m[g]) * s_iz[g];
-                    }
+            for (int g = 0; g < 8; ++g) {
+                if (g < G) {
+                    const float l = (i == 0) ? lg[g].x : (i == 1) ? lg[g].y : (i == 2) ? lg[g].z : lg[g].w;
+                    p += __expf(l - s_m[g]) * s_iz[g];
                 }
-                p *= (1.0f / (float)G);
-                const float score = use_vnorm ? (p + eps) * vn[i] : p;
-                bits = F16Traits<T>::from_float(score);
-                key = ordered_key16(bits, F16Traits<T>::kInfBits);
-                fmax_valid = fmaxf(fmax_valid, F16Traits<T>::to_float(bits));
             }
-        }
-        skeys[tid * KPT + i] = key;
-        sscores[tid * KPT + i] = bits;
-    }
-    __syncthreads();
-    flush_chunk_keys<KPT, false>(skeys, sscores, shist, row, chunk * kEaFinalPos, S, ws, scores_out);
-    // max over valid scores of the whole tensor (for the reference's max+1 sentinel)
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1)
-        fmax_valid = fmaxf(fmax_valid, __shfl_xor_sync(0xFFFFFFFFu, fmax_valid, off));
-    if (lane == 0) s_max[warp] = fmax_valid;
-    __syncthreads();
-    if (tid == 0) {
-        float m = s_max[0];
-        for (int w = 1; w < 8; ++w) m = fmaxf(m, s_max[w]);
-        if (m > -INFINITY) {
-            // order-preserving float -> uint so atomicMax works (counters are zero-initialised)
-            const uint32_t u = __float_as_uint(m);
-            const uint32_t ord = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-            atomicMax(&ws.counters[kCounterMaxSlot(ws.R)], ord);
-        }
-    }
+            p *= (1.0f / (float)G);
+            return use_vnorm ? (p + eps) * vn[i] : p;
+        });
+    publish_max_valid(fmax_valid, ws);
     flush_row_hist(shist, row, ws);
 }
 
@@ -533,8 +502,7 @@ __global__ void fill_sentinel_kernel(uint16_t* __restrict__ scores_out, int R, i
                                      const uint32_t* __restrict__ max_slot) {
     const uint32_t ord = *max_slot;
     pdl_launch_dependents();  // the select+compact kernel behind this one may start to take residency
-    const uint32_t u = (ord & 0x80000000u) ? (ord & 0x7FFFFFFFu) : ~ord;
-    const float sentinel = __uint_as_float(u) + 1.0f;
+    const float sentinel = ordered_f32_to_float(ord) + 1.0f;
     const uint16_t bits = F16Traits<T>::from_float(sentinel);
     const int width = hi - lo;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < R * width; i += gridDim.x * blockDim.x)
@@ -547,10 +515,9 @@ cudaError_t launch_fill_sentinel(int dtype, void* scores_out, int R, int S, int 
     const uint32_t* slot = ws.counters + kCounterMaxSlot(R);
     int blocks = (R * (hi - lo) + 255) / 256;
     if (blocks > 1024) blocks = 1024;
-    if (dtype == KVP_BF16)
-        fill_sentinel_kernel<__nv_bfloat16><<<blocks, 256, 0, st>>>(static_cast<uint16_t*>(scores_out), R, S, lo, hi, slot);
-    else
-        fill_sentinel_kernel<__half><<<blocks, 256, 0, st>>>(static_cast<uint16_t*>(scores_out), R, S, lo, hi, slot);
+    with_dtype(dtype, [&](auto t) {
+        fill_sentinel_kernel<decltype(t)><<<blocks, 256, 0, st>>>(static_cast<uint16_t*>(scores_out), R, S, lo, hi, slot);
+    });
     return cudaPeekAtLastError();
 }
 
@@ -597,7 +564,6 @@ static cudaError_t launch_ea_t(const Dims& d, int dtype, const void* K, const vo
                                const Workspace& ws, void* scores_out, cudaStream_t st) {
     const int G = d.Hq / d.H;
     if (G > 8) return cudaErrorNotSupported;
-    const int nvec = d.D / 8;
     const EaScratch sc = carve_ea(d, ws.scorer);
     int n_parts = 0;
     cudaError_t e = cudaSuccess;
@@ -621,16 +587,11 @@ static cudaError_t launch_ea_t(const Dims& d, int dtype, const void* K, const vo
     } else {
         n_parts = (d.S + kScoreChunkGeneric - 1) / kScoreChunkGeneric;
         dim3 grid(n_parts, d.R);
-#define KVP_EA_MU(LPR)                                                                                   \
-    ea_mu_logits_kernel<T, LPR><<<grid, 256, 0, st>>>(static_cast<const T*>(K), d.ks,                      \
-                                                      static_cast<const T*>(mu), static_cast<const T*>(V), \
-                                                      d.vs, use_vnorm, d.H, d.Hq, G, d.S, d.D, n_sink,     \
-                                                      n_parts, sc, ws.S_pad)
-        if (nvec <= 4) KVP_EA_MU(4);
-        else if (nvec <= 8) KVP_EA_MU(8);
-        else if (nvec <= 16) KVP_EA_MU(16);
-        else KVP_EA_MU(32);
-#undef KVP_EA_MU
+        with_lanes_per_row(d.D, [&](auto lpr) {
+            ea_mu_logits_kernel<T, lpr><<<grid, 256, 0, st>>>(static_cast<const T*>(K), d.ks, static_cast<const T*>(mu),
+                                                              static_cast<const T*>(V), d.vs, use_vnorm, d.H, d.Hq, G,
+                                                              d.S, d.D, n_sink, n_parts, sc, ws.S_pad);
+        });
         e = cudaPeekAtLastError();
     }
     if (e != cudaSuccess) return e;
@@ -647,9 +608,9 @@ cudaError_t launch_ea_score(const Dims& d, int dtype, const void* K, const void*
                             const void* cov, float eps, int n_sink, int use_vnorm,
                             const Workspace& ws, void* scores_out, cudaStream_t st) {
     // keys + histogram are always produced; a score-only call skips the select stage
-    if (dtype == KVP_BF16)
-        return launch_ea_t<__nv_bfloat16>(d, dtype, K, V, mu, cov, eps, n_sink, use_vnorm, ws, scores_out, st);
-    return launch_ea_t<__half>(d, dtype, K, V, mu, cov, eps, n_sink, use_vnorm, ws, scores_out, st);
+    return with_dtype(dtype, [&](auto t) {
+        return launch_ea_t<decltype(t)>(d, dtype, K, V, mu, cov, eps, n_sink, use_vnorm, ws, scores_out, st);
+    });
 }
 
 }  // namespace kvp

@@ -234,12 +234,7 @@ keydiff_score_kernel(const T* __restrict__ K, Strides3 ks, int H, int S, int D, 
         }
     }
     __syncthreads();
-    const int s_begin = chunk * kScoreChunk;
-    if (want_keys) {
-        flush_chunk_keys<1>(skeys, sscores, shist, row, s_begin, S, ws, scores_out);
-    } else if (s_begin + tid < S) {
-        scores_out[(size_t)row * S + s_begin + tid] = sscores[tid];
-    }
+    flush_or_store_scores(skeys, sscores, shist, row, chunk * kScoreChunk, S, ws, scores_out, want_keys);
 }
 
 template <typename T>
@@ -249,34 +244,25 @@ static cudaError_t launch_keydiff_t(const Dims& d, const void* K, const Workspac
     const KeyDiffScratch sc = carve_keydiff(d, ws.scorer);
     const int n_chunks = (d.S + kScoreChunk - 1) / kScoreChunk;
     dim3 grid(n_chunks, d.R);
-    const int nvec = d.D / 8;
     const T* Kp = static_cast<const T*>(K);
     uint16_t* so = static_cast<uint16_t*>(scores_out);
-#define KVP_KD_ANCHOR(LPR) \
-    keydiff_anchor_kernel<T, LPR><<<grid, kTileThreads, 0, st>>>(Kp, d.ks, d.H, d.S, d.D, n_chunks, sc)
-#define KVP_KD_SCORE(LPR) \
-    keydiff_score_kernel<T, LPR><<<grid, kTileThreads, 0, st>>>(Kp, d.ks, d.H, d.S, d.D, sc, ws, so, want_keys ? 1 : 0)
-    if (nvec <= 4) KVP_KD_ANCHOR(4);
-    else if (nvec <= 8) KVP_KD_ANCHOR(8);
-    else if (nvec <= 16) KVP_KD_ANCHOR(16);
-    else KVP_KD_ANCHOR(32);
-    cudaError_t e = cudaPeekAtLastError();
-    if (e != cudaSuccess) return e;
-    keydiff_merge_kernel<<<d.R, kKdMergeThreads, 0, st>>>(d.S, d.D, n_chunks, sc);
-    if ((e = cudaPeekAtLastError()) != cudaSuccess) return e;
-    if (nvec <= 4) KVP_KD_SCORE(4);
-    else if (nvec <= 8) KVP_KD_SCORE(8);
-    else if (nvec <= 16) KVP_KD_SCORE(16);
-    else KVP_KD_SCORE(32);
-#undef KVP_KD_ANCHOR
-#undef KVP_KD_SCORE
-    return cudaPeekAtLastError();
+    cudaError_t e = cudaSuccess;
+    // one lane count for both passes
+    with_lanes_per_row(d.D, [&](auto lpr) {
+        keydiff_anchor_kernel<T, lpr><<<grid, kTileThreads, 0, st>>>(Kp, d.ks, d.H, d.S, d.D, n_chunks, sc);
+        if ((e = cudaPeekAtLastError()) != cudaSuccess) return;
+        keydiff_merge_kernel<<<d.R, kKdMergeThreads, 0, st>>>(d.S, d.D, n_chunks, sc);
+        if ((e = cudaPeekAtLastError()) != cudaSuccess) return;
+        keydiff_score_kernel<T, lpr><<<grid, kTileThreads, 0, st>>>(Kp, d.ks, d.H, d.S, d.D, sc, ws, so,
+                                                                    want_keys ? 1 : 0);
+        e = cudaPeekAtLastError();
+    });
+    return e;
 }
 
 cudaError_t launch_keydiff_score(const Dims& d, int dtype, const void* K, const Workspace& ws,
                                  void* scores_out, bool want_keys, cudaStream_t st) {
-    if (dtype == KVP_BF16) return launch_keydiff_t<__nv_bfloat16>(d, K, ws, scores_out, want_keys, st);
-    return launch_keydiff_t<__half>(d, K, ws, scores_out, want_keys, st);
+    return with_dtype(dtype, [&](auto t) { return launch_keydiff_t<decltype(t)>(d, K, ws, scores_out, want_keys, st); });
 }
 
 }  // namespace kvp

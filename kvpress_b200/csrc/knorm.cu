@@ -30,19 +30,13 @@ knorm_score_kernel(const T* __restrict__ K, Strides3 ks, int H, int S, int D, Wo
     else if (row >= keep_from_row) knorm_score_chunk<T, LPR, 1>(K, ks, row / H, row % H, chunk, S, D, skeys, sscores);
     else knorm_score_chunk<T, LPR, 2>(K, ks, row / H, row % H, chunk, S, D, skeys, sscores);
     __syncthreads();
-    const int s_begin = chunk * kScoreChunk;
-    if (want_keys) {
-        flush_chunk_keys<1>(skeys, sscores, shist, row, s_begin, S, ws, scores_out);
-    } else if (s_begin + tid < S) {  // score-only call
-        scores_out[(size_t)row * S + s_begin + tid] = sscores[tid];
-    }
+    flush_or_store_scores(skeys, sscores, shist, row, chunk * kScoreChunk, S, ws, scores_out, want_keys);
 }
 
 template <typename T>
 static cudaError_t launch_knorm_t(const Dims& d, const void* K, const Workspace& ws,
                                   void* scores_out, bool want_keys, cudaStream_t st) {
     dim3 grid((d.S + kScoreChunk - 1) / kScoreChunk, d.R);
-    const int nvec = d.D / 8;
     const T* Kp = static_cast<const T*>(K);
     uint16_t* so = static_cast<uint16_t*>(scores_out);
     // rows whose K (row_bytes each) fits kKeepBytes of L2 at the end of the pass are kept for the compaction stage
@@ -57,22 +51,18 @@ static cudaError_t launch_knorm_t(const Dims& d, const void* K, const Workspace&
         keep_from_row = d.R - (int)n_keep;  // n_keep == 0: everything evict_first except nothing kept
         if (n_keep == 0) keep_from_row = -1;
     }
-#define KVP_LAUNCH_KNORM(LPR)                                                                   \
-    knorm_score_kernel<T, LPR><<<grid, kTileThreads, 0, st>>>(Kp, d.ks, d.H, d.S, d.D, ws, so, \
-                                                              want_keys ? 1 : 0, keep_from_row)
-    if (nvec <= 4) KVP_LAUNCH_KNORM(4);
-    else if (nvec <= 8) KVP_LAUNCH_KNORM(8);
-    else if (nvec <= 16) KVP_LAUNCH_KNORM(16);
-    else KVP_LAUNCH_KNORM(32);
-#undef KVP_LAUNCH_KNORM
+    with_lanes_per_row(d.D, [&](auto lpr) {
+        knorm_score_kernel<T, lpr><<<grid, kTileThreads, 0, st>>>(Kp, d.ks, d.H, d.S, d.D, ws, so, want_keys ? 1 : 0,
+                                                                  keep_from_row);
+    });
     return cudaPeekAtLastError();
 }
 
 cudaError_t launch_knorm_score(const Dims& d, int dtype, const void* K, const Workspace& ws,
                                void* scores_out, bool want_keys, cudaStream_t st) {
-    if (dtype == KVP_BF16)
-        return launch_knorm_t<__nv_bfloat16>(d, K, ws, scores_out, want_keys, st);
-    return launch_knorm_t<__half>(d, K, ws, scores_out, want_keys, st);
+    return with_dtype(dtype, [&](auto t) {
+        return launch_knorm_t<decltype(t)>(d, K, ws, scores_out, want_keys, st);
+    });
 }
 
 // ---- caller-supplied scores -> keys + histogram ------------------------------------------------
@@ -96,9 +86,9 @@ cudaError_t launch_keys_from_scores(const Dims& d, int dtype, const void* scores
                                     const Workspace& ws, cudaStream_t st) {
     const int n_tiles = (d.S + kTile - 1) / kTile;
     dim3 grid(n_tiles, d.R);
-    keys_from_scores_kernel<<<grid, kTileThreads, 0, st>>>(static_cast<const uint16_t*>(scores),
-                                                           sb, sh, d.H, d.S,
-                                                           dtype == KVP_BF16 ? 0x7F80u : 0x7C00u, ws);
+    const uint16_t inf_bits = with_dtype(dtype, [](auto t) { return F16Traits<decltype(t)>::kInfBits; });
+    keys_from_scores_kernel<<<grid, kTileThreads, 0, st>>>(static_cast<const uint16_t*>(scores), sb, sh, d.H, d.S,
+                                                           inf_bits, ws);
     return cudaPeekAtLastError();
 }
 

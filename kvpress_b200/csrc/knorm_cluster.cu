@@ -401,12 +401,11 @@ cudaError_t launch_knorm_cluster(const Dims& d, int dtype, const void* K, const 
                                  int32_t* idx_out, void* scores_out, cudaStream_t st) {
     ClusterPlan pl;
     if (!choose_cluster(d, &pl)) return cudaErrorNotSupported;
-    if (d.S <= kClThreads * 12)
-        return (dtype == KVP_BF16) ? launch_cluster_t<__nv_bfloat16, 12>(d, pl, K, V, K_out, V_out, idx_out, scores_out, st)
-                                   : launch_cluster_t<__half, 12>(d, pl, K, V, K_out, V_out, idx_out, scores_out, st);
-    return (dtype == KVP_BF16)
-               ? launch_cluster_t<__nv_bfloat16, kClMaxKeysPerThread>(d, pl, K, V, K_out, V_out, idx_out, scores_out, st)
-               : launch_cluster_t<__half, kClMaxKeysPerThread>(d, pl, K, V, K_out, V_out, idx_out, scores_out, st);
+    return with_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        if (d.S <= kClThreads * 12) return launch_cluster_t<T, 12>(d, pl, K, V, K_out, V_out, idx_out, scores_out, st);
+        return launch_cluster_t<T, kClMaxKeysPerThread>(d, pl, K, V, K_out, V_out, idx_out, scores_out, st);
+    });
 }
 
 }  // namespace kvp

@@ -75,11 +75,9 @@ __device__ __forceinline__ int f2o(float f) {
 }
 __device__ __forceinline__ float o2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7FFFFFFF); }
 
-// order-preserving uint image of a float, NaN above everything (the rank's comparison)
+// the rank's comparison: ordered_f32, except that every NaN sorts above everything and -0 ties with +0 (as torch.sort)
 __device__ __forceinline__ uint32_t rank_key(float f) {
-    if (isnan(f)) return 0xFFFFFFFFu;
-    const uint32_t u = __float_as_uint(f == 0.f ? 0.f : f);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    return isnan(f) ? 0xFFFFFFFFu : ordered_f32(f == 0.f ? 0.f : f);
 }
 
 // Writes one position's score (or, past S, its zero key padding) and counts its key in the CTA histogram.
@@ -100,10 +98,7 @@ __device__ __forceinline__ void emit(const LagArgs& a, int row, int s, bool vali
             a.ws.keys[(size_t)row * a.ws.S_pad + s] = 0;
         }
     }
-    if (a.want_keys) {
-        const unsigned peers = __match_any_sync(0xFFFFFFFFu, bin);
-        if (bin < 256u && (threadIdx.x & 31) == (__ffs(peers) - 1)) atomicAdd(&shist[bin], __popc(peers));
-    }
+    if (a.want_keys) warp_hist_add(shist, bin);
 }
 
 // sigma of one row: x = (v - lo) / (hi - lo) over this lane's 8 channels, mean and the two-pass unbiased std over the
@@ -361,14 +356,8 @@ __global__ void __launch_bounds__(kLagThreads, 2) lagkv_kernel(LagArgs a) {
 
 template <typename T>
 static cudaError_t launch_lagkv_t(const LagArgs& a, int R, int n_items, cudaStream_t st) {
-    const int nvec = a.D / 8;
     const dim3 grid(n_items, R);
-#define KVP_LAG(LPR) lagkv_kernel<T, LPR><<<grid, kLagThreads, 0, st>>>(a)
-    if (nvec <= 4) KVP_LAG(4);
-    else if (nvec <= 8) KVP_LAG(8);
-    else if (nvec <= 16) KVP_LAG(16);
-    else KVP_LAG(32);
-#undef KVP_LAG
+    with_lanes_per_row(a.D, [&](auto lpr) { lagkv_kernel<T, lpr><<<grid, kLagThreads, 0, st>>>(a); });
     return cudaPeekAtLastError();
 }
 
@@ -408,8 +397,7 @@ cudaError_t launch_lagkv_score(const Dims& d, int dtype, const void* K, const vo
         a.tail_start = n_sink + (P - 1) * lag_size;
         n_items = a.n_seg + a.n_fill_a + (a.fill_end - a.tail_start + kLagThreads - 1) / kLagThreads;
     }
-    if (dtype == KVP_BF16) return launch_lagkv_t<__nv_bfloat16>(a, d.R, n_items, st);
-    return launch_lagkv_t<__half>(a, d.R, n_items, st);
+    return with_dtype(dtype, [&](auto t) { return launch_lagkv_t<decltype(t)>(a, d.R, n_items, st); });
 }
 
 }  // namespace kvp

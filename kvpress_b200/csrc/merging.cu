@@ -271,13 +271,9 @@ merging_argmax_kernel(const __grid_constant__ CUtensorMap mapE, const __grid_con
 }
 
 // ---- 3. gate, weights and the stable counting sort --------------------------------------------------------------------
-__device__ __forceinline__ uint32_t mg_key32(float f) {  // order-preserving; -0 and +0 share a key
-    uint32_t u = __float_as_uint(f);
-    if (u == 0x80000000u) u = 0;
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float mg_from_key32(uint32_t k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+// ordered_f32, except that -0 and +0 share a key
+__device__ __forceinline__ uint32_t mg_key32(float f) {
+    return ordered_f32(__float_as_uint(f) == 0x80000000u ? 0.f : f);
 }
 
 struct MgPlanArgs {
@@ -432,7 +428,7 @@ __global__ void __launch_bounds__(kMgPlanThreads) merging_plan_kernel(MgPlanArgs
             __syncthreads();
             khi = bc[0] > hi ? klo : bc[1];
         }
-        const float below = mg_from_key32(klo), above = mg_from_key32(khi);
+        const float below = ordered_f32_to_float(klo), above = ordered_f32_to_float(khi);
         const float diff = above - below;  // -inf - -inf = NaN: no merge in the row, as in torch
         thr = fabsf(w) < 0.5f ? fmaf(w, diff, below) : fmaf(-diff, 1.f - w, above);
     }
@@ -640,9 +636,9 @@ static cudaError_t launch_mg_t(const Dims& d, const void* K, const void* V, cons
 cudaError_t launch_merging(const Dims& d, int dtype, const void* K, const void* V, const int32_t* kept, float threshold,
                            double merge_fraction, void* V_out, int32_t* target_out, float* sim_out, const Workspace& ws,
                            cudaStream_t st) {
-    if (dtype == KVP_BF16)
-        return launch_mg_t<__nv_bfloat16>(d, K, V, kept, threshold, merge_fraction, V_out, target_out, sim_out, ws, st);
-    return launch_mg_t<__half>(d, K, V, kept, threshold, merge_fraction, V_out, target_out, sim_out, ws, st);
+    return with_dtype(dtype, [&](auto t) {
+        return launch_mg_t<decltype(t)>(d, K, V, kept, threshold, merge_fraction, V_out, target_out, sim_out, ws, st);
+    });
 }
 
 }  // namespace kvp

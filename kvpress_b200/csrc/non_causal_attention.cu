@@ -342,12 +342,6 @@ nca_stats_kernel(int S, int R, int n_parts, NcaScratch sc) {
 }
 
 template <typename T>
-__device__ __forceinline__ uint16_t nca_round(double v) {
-    if constexpr (std::is_same<T, __nv_bfloat16>::value) return __bfloat16_as_ushort(__double2bfloat16(v));
-    else return __half_as_ushort(__double2half(v));
-}
-
-template <typename T>
 __global__ void __launch_bounds__(kTileThreads)
 nca_z_kernel(int S, NcaScratch sc, Workspace ws, uint16_t* __restrict__ scores_out) {
     __shared__ uint16_t skeys[kTile];
@@ -356,17 +350,9 @@ nca_z_kernel(int S, NcaScratch sc, Workspace ws, uint16_t* __restrict__ scores_o
     const int tile = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
     shist[tid] = 0;
     pdl_launch_dependents();  // the select+compact kernel behind this one may start to take residency
-    const int s = tile * kTile + tid;
-    uint16_t bits = 0, key = 0;
-    if (s < S) {
-        const double p = nca_pooled(sc, (size_t)row * ws.S_pad, s, S);
-        bits = nca_round<T>((p - sc.stats[0]) / sc.stats[1]);
-        key = ordered_key16(bits, F16Traits<T>::kInfBits);
-    }
-    skeys[tid] = key;
-    sscores[tid] = bits;
-    __syncthreads();
-    flush_chunk_keys<1>(skeys, sscores, shist, row, tile * kTile, S, ws, scores_out);
+    score_tile_epilogue<T, 1>(skeys, sscores, shist, row, tile * kTile, S, 0, 0, ws, scores_out, nullptr, [&](int, int s) {
+        return (nca_pooled(sc, (size_t)row * ws.S_pad, s, S) - sc.stats[0]) / sc.stats[1];
+    });
 }
 
 // ---- host launcher ------------------------------------------------------------------------------------------------
@@ -418,8 +404,7 @@ static cudaError_t launch_nca_d(const Dims& d, const void* K, const void* V, con
 
 cudaError_t launch_non_causal_attention_score(const Dims& d, int dtype, const void* K, const void* V, const void* q,
                                               int chunk_size, const Workspace& ws, void* scores_out, cudaStream_t st) {
-    if (dtype == KVP_BF16) return launch_nca_d<__nv_bfloat16>(d, K, V, q, chunk_size, ws, scores_out, st);
-    return launch_nca_d<__half>(d, K, V, q, chunk_size, ws, scores_out, st);
+    return with_dtype(dtype, [&](auto t) { return launch_nca_d<decltype(t)>(d, K, V, q, chunk_size, ws, scores_out, st); });
 }
 
 }  // namespace kvp

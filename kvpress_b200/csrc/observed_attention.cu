@@ -330,19 +330,12 @@ obs_finalize_kernel(int S, int G, ObsScratch sc, Workspace ws, uint16_t* __restr
     const int tile = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
     shist[tid] = 0;
     pdl_launch_dependents();  // the select+compact kernel behind this one may start to take residency
-    const int s = tile * kTile + tid;
-    uint16_t bits = 0, key = 0;
-    if (s < S) {
+    score_tile_epilogue<T, 1>(skeys, sscores, shist, row, tile * kTile, S, 0, 0, ws, scores_out, nullptr, [&](int, int s) {
         // the reference's divisor, S - s in the cache dtype (fp16: inf from 65520 on, so the score is exactly 0);
         // G times it is exact in fp32
         const float div = F16Traits<T>::to_float(F16Traits<T>::from_float((float)(S - s)));
-        bits = F16Traits<T>::from_float(sc.colsum[(size_t)row * ws.S_pad + s] / ((float)G * div));
-        key = ordered_key16(bits, F16Traits<T>::kInfBits);
-    }
-    skeys[tid] = key;
-    sscores[tid] = bits;
-    __syncthreads();
-    flush_chunk_keys<1>(skeys, sscores, shist, row, tile * kTile, S, ws, scores_out);
+        return sc.colsum[(size_t)row * ws.S_pad + s] / ((float)G * div);
+    });
 }
 
 // ---- host launcher ------------------------------------------------------------------------------------------------
@@ -405,8 +398,7 @@ static cudaError_t launch_obs_d(const Dims& d, const void* K, const void* q, int
 
 cudaError_t launch_observed_attention_score(const Dims& d, int dtype, const void* K, const void* q, int n_q,
                                             float scaling, const Workspace& ws, void* scores_out, cudaStream_t st) {
-    if (dtype == KVP_BF16) return launch_obs_d<__nv_bfloat16>(d, K, q, n_q, scaling, ws, scores_out, st);
-    return launch_obs_d<__half>(d, K, q, n_q, scaling, ws, scores_out, st);
+    return with_dtype(dtype, [&](auto t) { return launch_obs_d<decltype(t)>(d, K, q, n_q, scaling, ws, scores_out, st); });
 }
 
 }  // namespace kvp

@@ -542,9 +542,9 @@ cudaError_t launch_select_compact(const Dims& d, const void* K, const void* V, v
 cudaError_t launch_select_compact_rerotate(const Dims& d, int dtype, const void* K, const void* V,
                                            void* K_out, void* V_out, int32_t* idx_out,
                                            const Workspace& ws, const float* inv_freq, cudaStream_t st) {
-    if (dtype == KVP_BF16)
-        return launch_select_compact_t<__nv_bfloat16>(d, K, V, K_out, V_out, idx_out, ws, inv_freq, st);
-    return launch_select_compact_t<__half>(d, K, V, K_out, V_out, idx_out, ws, inv_freq, st);
+    return with_dtype(dtype, [&](auto t) {
+        return launch_select_compact_t<decltype(t)>(d, K, V, K_out, V_out, idx_out, ws, inv_freq, st);
+    });
 }
 
 // ---- KnormPress: score + select + compact in ONE persistent kernel ---------------------------------
@@ -708,31 +708,24 @@ static cudaError_t launch_knorm_fused_t(const Dims& d, const void* K, const void
     const int k_last = knob_klast >= 0 ? knob_klast : (big_rows ? 1 : 0);
     const long long total = fused_total_items(fq);
     if (total > 0x7FFFFFFFll) return cudaErrorNotSupported;
-    const int nvec = d.D / 8;
-#define KVP_LAUNCH_FUSED(LPR)                                                                         \
-    do {                                                                                              \
-        auto kern = knorm_fused_kernel<T, LPR>;                                                       \
-        static PerDeviceInt occupancy;                                                                \
-        const int grid = persistent_grid(kern, kTileThreads, (int)total, occupancy);                  \
-        kern<<<grid, kTileThreads, 0, st>>>(static_cast<const T*>(K), static_cast<const T*>(V), d.ks,  \
-                                            d.vs, static_cast<char*>(K_out), static_cast<char*>(V_out), \
-                                            idx_out, static_cast<uint16_t*>(scores_out), d.H, d.S, d.D, \
-                                            d.n_kept, ws, fq, k_last);                                \
-    } while (0)
-    if (nvec <= 4) KVP_LAUNCH_FUSED(4);
-    else if (nvec <= 8) KVP_LAUNCH_FUSED(8);
-    else if (nvec <= 16) KVP_LAUNCH_FUSED(16);
-    else KVP_LAUNCH_FUSED(32);
-#undef KVP_LAUNCH_FUSED
+    with_lanes_per_row(d.D, [&](auto lpr) {
+        auto kern = knorm_fused_kernel<T, lpr>;
+        static PerDeviceInt occupancy;  // one per <T, LPR> instantiation of this lambda
+        const int grid = persistent_grid(kern, kTileThreads, (int)total, occupancy);
+        kern<<<grid, kTileThreads, 0, st>>>(static_cast<const T*>(K), static_cast<const T*>(V), d.ks, d.vs,
+                                            static_cast<char*>(K_out), static_cast<char*>(V_out), idx_out,
+                                            static_cast<uint16_t*>(scores_out), d.H, d.S, d.D, d.n_kept, ws, fq,
+                                            k_last);
+    });
     return cudaPeekAtLastError();
 }
 
 cudaError_t launch_knorm_fused(const Dims& d, int dtype, const void* K, const void* V, void* K_out,
                                void* V_out, int32_t* idx_out, void* scores_out, const Workspace& ws,
                                cudaStream_t st) {
-    if (dtype == KVP_BF16)
-        return launch_knorm_fused_t<__nv_bfloat16>(d, K, V, K_out, V_out, idx_out, scores_out, ws, st);
-    return launch_knorm_fused_t<__half>(d, K, V, K_out, V_out, idx_out, scores_out, ws, st);
+    return with_dtype(dtype, [&](auto t) {
+        return launch_knorm_fused_t<decltype(t)>(d, K, V, K_out, V_out, idx_out, scores_out, ws, st);
+    });
 }
 
 // ---- StreamingLLM: the answer is two ranges, no scores needed --------------------------------
@@ -795,12 +788,9 @@ cudaError_t launch_streaming_score(const Dims& d, int dtype, int n_sink, void* s
     const int lo = n_sink, hi = (n_sink + n_pruned < d.S) ? n_sink + n_pruned : d.S;
     int blocks = (int)((total + 255) / 256);
     if (blocks > 132 * 8) blocks = 132 * 8;
-    if (dtype == KVP_BF16)
-        streaming_score_kernel<__nv_bfloat16>
-            <<<blocks, 256, 0, st>>>(static_cast<uint16_t*>(scores_out), d.S, lo, hi, total);
-    else
-        streaming_score_kernel<__half>
-            <<<blocks, 256, 0, st>>>(static_cast<uint16_t*>(scores_out), d.S, lo, hi, total);
+    with_dtype(dtype, [&](auto t) {
+        streaming_score_kernel<decltype(t)><<<blocks, 256, 0, st>>>(static_cast<uint16_t*>(scores_out), d.S, lo, hi, total);
+    });
     return cudaPeekAtLastError();
 }
 

@@ -285,8 +285,7 @@ snap_finalize_kernel(int S, int window, int kernel_size, float inv_gw, SnapScrat
     __shared__ uint16_t skeys[kTile];
     __shared__ uint16_t sscores[kTile];
     __shared__ uint32_t shist[256];
-    __shared__ float s_max[8];
-    const int tile = blockIdx.x, row = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tile = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
     shist[tid] = 0;
     pdl_launch_dependents();  // the select+compact kernel behind this one may start to take residency
     const int n_scored = S - window;
@@ -294,43 +293,19 @@ snap_finalize_kernel(int S, int window, int kernel_size, float inv_gw, SnapScrat
     for (int sub = 0; sub < kFinalizeTiles; ++sub) {
         const int t = tile * kFinalizeTiles + sub;
         if (t >= ws.n_tiles) break;
-        const int s = t * kTile + tid;
-        uint16_t bits = 0, key = 0;
-        if (s < S) {
-            if (s >= n_scored) {
-                key = kForcedKey;
-            } else {
-                const int half = kernel_size >> 1;
-                float acc = 0.f;
-                for (int o = -half; o <= half; ++o) {
-                    const int j = s + o;
-                    if (j >= 0 && j < n_scored) acc += sc.colsum[(size_t)row * ws.S_pad + j];
-                }
-                const float score = acc * inv_gw / (float)kernel_size;  // count_include_pad: always / kernel
-                bits = F16Traits<T>::from_float(score);
-                key = ordered_key16(bits, F16Traits<T>::kInfBits);
-                fmax_valid = fmaxf(fmax_valid, F16Traits<T>::to_float(bits));
+        if (sub > 0) __syncthreads();  // the previous tile's keys and scores are out of skeys / sscores
+        score_tile_epilogue<T, 1, false>(skeys, sscores, shist, row, t * kTile, S, n_scored, S, ws, scores_out,
+                                         &fmax_valid, [&](int, int s) {
+            const int half = kernel_size >> 1;
+            float acc = 0.f;
+            for (int o = -half; o <= half; ++o) {
+                const int j = s + o;
+                if (j >= 0 && j < n_scored) acc += sc.colsum[(size_t)row * ws.S_pad + j];
             }
-        }
-        __syncthreads();
-        skeys[tid] = key;
-        sscores[tid] = bits;
-        __syncthreads();
-        flush_chunk_keys<1, false>(skeys, sscores, shist, row, t * kTile, S, ws, scores_out);
+            return acc * inv_gw / (float)kernel_size;  // count_include_pad: always / kernel
+        });
     }
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1)
-        fmax_valid = fmaxf(fmax_valid, __shfl_xor_sync(0xFFFFFFFFu, fmax_valid, off));
-    if (lane == 0) s_max[warp] = fmax_valid;
-    __syncthreads();
-    if (tid == 0) {
-        float m = s_max[0];
-        for (int w = 1; w < 8; ++w) m = fmaxf(m, s_max[w]);
-        if (m > -INFINITY) {
-            const uint32_t u = __float_as_uint(m);
-            atomicMax(&ws.counters[kCounterMaxSlot(ws.R)], (u & 0x80000000u) ? ~u : (u | 0x80000000u));
-        }
-    }
+    publish_max_valid(fmax_valid, ws);
     flush_row_hist(shist, row, ws);
 }
 
@@ -404,9 +379,9 @@ static cudaError_t launch_snap_d(const Dims& d, int dtype, const void* K, const 
 
 cudaError_t launch_snapkv_score(const Dims& d, int dtype, const void* K, const void* q_window, int window,
                                 int kernel_size, const Workspace& ws, void* scores_out, cudaStream_t st) {
-    if (dtype == KVP_BF16)
-        return launch_snap_d<__nv_bfloat16>(d, dtype, K, q_window, window, kernel_size, ws, scores_out, st);
-    return launch_snap_d<__half>(d, dtype, K, q_window, window, kernel_size, ws, scores_out, st);
+    return with_dtype(dtype, [&](auto t) {
+        return launch_snap_d<decltype(t)>(d, dtype, K, q_window, window, kernel_size, ws, scores_out, st);
+    });
 }
 
 }  // namespace kvp

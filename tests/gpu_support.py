@@ -1,6 +1,8 @@
 """Helpers shared by the GPU tests: the library, the float64 references and input generators of the scorers, and the
 bars their kernels are held to (each bar is described in the module docstring of the test file that states it)."""
 import math
+import re
+from pathlib import Path
 
 import torch
 import torch.nn.functional as F
@@ -372,10 +374,15 @@ MERGE_THREADS = 1024  # kKdMergeThreads
 CHUNK = 256  # kScoreChunk: positions per anchor / score CTA
 
 
-def kd_lanes(D: int) -> int:
-    """LPR of keydiff_anchor_kernel / keydiff_score_kernel: lanes per key row"""
-    nvec = D // 8
-    return 4 if nvec <= 4 else 8 if nvec <= 8 else 16 if nvec <= 16 else 32
+# kLanesPerRow of csrc/common.cuh: the lanes-per-row counts the CUDA-core score kernels are instantiated for
+LANES_PER_ROW = tuple(int(x) for x in re.search(
+    r"constexpr int kLanesPerRow\[\] = \{([\d, ]+)\};",
+    (Path(__file__).resolve().parent.parent / "kvpress_b200" / "csrc" / "common.cuh").read_text()).group(1).split(","))
+
+
+def lanes_per_row(D: int) -> int:
+    """The LPR with_lanes_per_row picks for head_dim D: the first kLanesPerRow entry >= D / 8, else the last."""
+    return next((lpr for lpr in LANES_PER_ROW if D // 8 <= lpr), LANES_PER_ROW[-1])
 
 
 def kd_dpad(D: int) -> int:
@@ -393,7 +400,7 @@ def kd_chunks(S: int) -> int:
 
 def kd_chain(S: int, D: int) -> int:
     """L: the longest addition chain of an anchor component (see the module docstring)"""
-    lpr, G = kd_lanes(D), kd_groups(D)
+    lpr, G = lanes_per_row(D), kd_groups(D)
     return lpr + int(math.log2(32 // lpr)) + 8 + (kd_chunks(S) + 4 * G - 1) // (4 * G) + 3 + 2 + G + 1
 
 

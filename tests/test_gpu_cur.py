@@ -20,7 +20,6 @@ below are of non-negative terms, so relative errors carry through them as their 
   rounded to fp32 once: E_s = 1.01 z (rho_u(s) + max_t rho_u(t) + 2 u).
 """
 import math
-import re
 from pathlib import Path
 
 import pytest
@@ -30,8 +29,8 @@ from transformers import DynamicCache
 from oracle import press_oracle as O
 from tests import cur_backend as CB
 from tests.conftest import ulp16_diff
-from tests.gpu_support import (assert_compress, gpu_ids, lagkv_inputs, _masked, _name, _native, _prefill, same16,
-                               _shared, tiny_gpu_llama, ulp_at)
+from tests.gpu_support import (assert_compress, gpu_ids, lagkv_inputs, LANES_PER_ROW, lanes_per_row, _masked, _name,
+                               _native, _prefill, same16, _shared, tiny_gpu_llama, ulp_at)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
@@ -133,18 +132,12 @@ HEAD_DIMS = (8, 16, 40, 64, 72, 96, 128, 200, 256)
 SWEEP = [(dt, D) for dt in (torch.bfloat16, torch.float16) for D in HEAD_DIMS]
 
 
-def _lpr(D: int) -> int:
-    nvec = D // 8
-    return 4 if nvec <= 4 else 8 if nvec <= 8 else 16 if nvec <= 16 else 32
-
-
-def test_sweep_reaches_every_instantiation():
+def test_sweep_reaches_every_lanes_per_row_instantiation():
     """csrc/cur.cu instantiates <dtype, lanes per row> for 4, 8, 16 and 32 lanes, plus one projected kernel per dtype;
     HEAD_DIMS reaches each, with and without idle lanes."""
     src = (ROOT / "kvpress_b200" / "csrc" / "cur.cu").read_text()
-    lprs = {int(x) for x in re.findall(r"KVP_CUR\((\d+)\);", src)}
-    assert lprs == {4, 8, 16, 32} == {_lpr(D) for D in HEAD_DIMS}
-    assert {D // 8 == _lpr(D) for D in HEAD_DIMS} == {True, False}
+    assert set(LANES_PER_ROW) == {lanes_per_row(D) for D in HEAD_DIMS}
+    assert {D // 8 == lanes_per_row(D) for D in HEAD_DIMS} == {True, False}
     assert "cur_unit_kernel<T, 4, true>" in src
 
 

@@ -64,7 +64,8 @@ import torch
 from oracle import press_oracle as O
 from tests.conftest import ulp16_diff
 from tests.gpu_support import (assert_compress, assert_e_small, assert_keydiff_vs_ref, assert_rerotated, _bits, CHUNK,
-                               _gather, kd_chain, kd_chunks, kd_dpad, kd_groups, kd_lanes, keydiff_error_bound,
+                               _gather, kd_chain, kd_chunks, kd_dpad, kd_groups, LANES_PER_ROW, lanes_per_row,
+                               keydiff_error_bound,
                                keydiff_ref64, _layout, LAYOUTS, MERGE_THREADS, _name, _native, rope_inv_freq, _same)
 
 gpu = pytest.mark.gpu
@@ -111,25 +112,12 @@ def n_kept_values(S: int):
 # ---------------------------------------------------------------------------------------------------
 # CPU: the sweeps reach every instantiation the sources build
 # ---------------------------------------------------------------------------------------------------
-def test_sweep_reaches_every_keydiff_and_rerotation_instantiation():
+def test_sweeps_reach_every_dispatched_keydiff_and_rerotation_instantiation():
     """The KeyDiff sweep runs every <T, LPR> of the anchor and score kernels, each LPR with and without idle lanes,
     every d_pad of the merge and, at G = 32, 8 and 4, n_chunks on both sides of G and 4G and past 8G; the rerotation
     sweep runs both <T> of the rerotating compaction with 1 to 8 and 16 vectors per half row, odd counts included."""
     kd = (CSRC / "keydiff.cu").read_text()
-    dispatch = {}
-    for macro in ("KVP_KD_ANCHOR", "KVP_KD_SCORE"):
-        bounded = [(int(n), int(l)) for n, l in re.findall(rf"if \(nvec <= (\d+)\) {macro}\((\d+)\);", kd)]
-        last = [int(l) for l in re.findall(rf"else {macro}\((\d+)\);", kd)]
-        assert len(bounded) == 3 and len(last) == 1, macro
-        dispatch[macro] = bounded + [(None, last[0])]
-    assert dispatch["KVP_KD_ANCHOR"] == dispatch["KVP_KD_SCORE"]
-    # the restated dispatch agrees with the launcher on both sides of every bound
-    bounded = dispatch["KVP_KD_ANCHOR"]
-    for i, (nvec, lpr) in enumerate(bounded):
-        if nvec is not None:
-            assert kd_lanes(8 * nvec) == lpr and kd_lanes(8 * (nvec + 1)) == bounded[i + 1][1]
-    lprs = {lpr for _, lpr in bounded}
-    assert lprs == {4, 8, 16, 32}
+    lprs = set(LANES_PER_ROW)  # one with_lanes_per_row call launches both passes
     m = re.search(r"d_pad = \(D <= (\d+)\) \? (\d+) : \(D <= (\d+)\) \? (\d+) : \(D <= (\d+)\) \? (\d+) : (\d+);", kd)
     bounds = [int(x) for x in m.groups()]
     pads = {bounds[1], bounds[3], bounds[5], bounds[6]}
@@ -138,9 +126,9 @@ def test_sweep_reaches_every_keydiff_and_rerotation_instantiation():
     assert int(re.search(r"constexpr int kScoreChunk = (\d+);", (CSRC / "knorm_chunk.cuh").read_text()).group(1)) == CHUNK
 
     built = {(n, lpr) for n in ("bf16", "fp16") for lpr in lprs}
-    assert {(_name(dt), kd_lanes(D)) for dt, D in KD_SWEEP} == built
+    assert {(_name(dt), lanes_per_row(D)) for dt, D in KD_SWEEP} == built
     for lpr in lprs:  # idle lanes: fewer 8-element pieces per row than lanes
-        assert {D // 8 < lpr for _, D in KD_SWEEP if kd_lanes(D) == lpr} == {True, False}
+        assert {D // 8 < lpr for _, D in KD_SWEEP if lanes_per_row(D) == lpr} == {True, False}
     assert {kd_dpad(D) for _, D in KD_SWEEP} == pads
     assert all(any(kd_dpad(D) == p and D < p for _, D in KD_SWEEP) for p in pads)
     for G in (32, 8, 4):
@@ -150,8 +138,7 @@ def test_sweep_reaches_every_keydiff_and_rerotation_instantiation():
 
     sc = (CSRC / "select_compact.cu").read_text()
     rerot = re.search(r"cudaError_t launch_select_compact_rerotate\(.*?\n}", sc, re.S).group(0)
-    types = set(re.findall(r"launch_select_compact_t<(__nv_bfloat16|__half)>\(", rerot))
-    assert types == {"__nv_bfloat16", "__half"}
+    assert "with_dtype(dtype" in rerot and "launch_select_compact_t<decltype(t)>(" in rerot  # both <T>
     assert "copy_rows_k_rerotated<TR>(" in sc
     want = {(n, hv) for n in ("bf16", "fp16") for hv in (*range(1, 9), 16)}  # head_dim 16 .. 128, and 256
     assert {(_name(dt), D // 16) for dt, D in RR_SWEEP} == want
@@ -235,7 +222,7 @@ def test_keydiff_instantiations(dtype, D):
     B, H, S = 2, 3, 3001
     for kind in ("isotropic", "offset"):
         k, v = kd_inputs(B, H, S, D, dtype, kind, 10 * D + (kind == "offset"))
-        run_keydiff(k, v, f"keydiff {_name(dtype)} D={D} LPR={kd_lanes(D)} d_pad={kd_dpad(D)} {kind}")
+        run_keydiff(k, v, f"keydiff {_name(dtype)} D={D} LPR={lanes_per_row(D)} d_pad={kd_dpad(D)} {kind}")
 
 
 @gpu
@@ -274,7 +261,7 @@ def planted_unit_keys(B, H, S, D, dtype, seed):
     gen = torch.Generator(device=DEV).manual_seed(seed)
     s = torch.arange(S, device=DEV)
     loc = s % CHUNK
-    rpw = 32 // kd_lanes(D)
+    rpw = 32 // lanes_per_row(D)
     p = loc % 32
     j = ((s // CHUNK) * 3 + (loc // 32) * 5 + (p % rpw) * 7 + (p // rpw) * 11) % (D - 1) + 1
     orth = s % 16 == 0

@@ -44,8 +44,8 @@ import torch
 from oracle import press_oracle as O
 from tests.conftest import ulp16_diff
 from tests.abi_cases import PYTHON, child_env
-from tests.gpu_support import (assert_compress, assert_vs_ref64, _bits, _gather, knorm_ref64, _layout, LAYOUTS, _name,
-                               _native, _same)
+from tests.gpu_support import (assert_compress, assert_vs_ref64, _bits, _gather, knorm_ref64, LANES_PER_ROW,
+                               lanes_per_row, _layout, LAYOUTS, _name, _native, _same)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
@@ -81,11 +81,6 @@ def cluster_size(S: int) -> int:
     while C > 1 and (S + C - 1) // C < 64:
         C >>= 1
     return C
-
-
-def lanes_per_row(D: int) -> int:
-    nvec = D // 8
-    return 4 if nvec <= 4 else 8 if nvec <= 8 else 16 if nvec <= 16 else 32
 
 
 def knorm_dispatch(B: int, H: int, S: int, D: int, dtype) -> Dispatch:
@@ -208,22 +203,28 @@ def test_knorm_dispatch_matches_launch_count():
     assert not wrong, f"(shape, library path, restated path): {wrong}"
 
 
+def test_lanes_per_row_follows_common():
+    """lanes_per_row restates with_lanes_per_row over kLanesPerRow: ascending power-of-two lane counts of one warp, the
+    last covering the widest head_dim (256); every head_dim takes the first count >= D / 8 and each count is taken."""
+    assert LANES_PER_ROW == (4, 8, 16, 32)  # the instantiations the sweeps' head_dims are chosen for
+    assert 8 * LANES_PER_ROW[-1] >= 256
+    for D in range(8, 257, 8):
+        assert lanes_per_row(D) == min(lpr for lpr in LANES_PER_ROW if D // 8 <= lpr)
+    assert {lanes_per_row(D) for D in range(8, 257, 8)} == set(LANES_PER_ROW)
+
+
 def _built_instantiations():
     """{(path, dtype, LPR or KPT)} the sources instantiate."""
-    fused = re.findall(r"KVP_LAUNCH_FUSED\((\d+)\);", (CSRC / "select_compact.cu").read_text())
-    score = re.findall(r"KVP_LAUNCH_KNORM\((\d+)\);", (CSRC / "knorm.cu").read_text())
     cl_src = (CSRC / "knorm_cluster.cu").read_text()
     max_kpt = re.search(r"constexpr int kClMaxKeysPerThread = (\d+);", cl_src).group(1)
-    cluster = re.findall(r"launch_cluster_t<(__nv_bfloat16|__half), (12|kClMaxKeysPerThread)>\(", cl_src)
+    cluster = re.findall(r"launch_cluster_t<T, (12|kClMaxKeysPerThread)>\(", cl_src)  # T: both, through with_dtype
     assert int(max_kpt) == CL_MAX_KPT
-    dt = {"__nv_bfloat16": "bf16", "__half": "fp16"}
-    built = {("fused", n, int(x)) for x in fused for n in ("bf16", "fp16")}
-    built |= {("two_kernels", n, int(x)) for x in score for n in ("bf16", "fp16")}
-    built |= {("cluster", dt[t], int(max_kpt if k == "kClMaxKeysPerThread" else k)) for t, k in cluster}
+    built = {(path, n, lpr) for path in ("fused", "two_kernels") for n in ("bf16", "fp16") for lpr in LANES_PER_ROW}
+    built |= {("cluster", n, int(max_kpt if k == "kClMaxKeysPerThread" else k)) for k in cluster for n in ("bf16", "fp16")}
     return built
 
 
-def test_knorm_sweep_reaches_every_instantiation_and_regime():
+def test_knorm_sweep_reaches_every_dispatched_instantiation_and_regime():
     """The shape sweep runs every <T, LPR> of the fused and score kernels and every <T, KPT> of the cluster kernel, the
     fused queue at lag 2, at lag 1 with R >= 2 and at lag 1 clipped to R = 1, and the cluster kernel with 1, 2, 4 and 8
     CTAs, with and without V staged in shared memory."""

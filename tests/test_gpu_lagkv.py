@@ -26,8 +26,6 @@ E_s, derived from the kernel's operations (first order; the final factor 1.01 co
 - c = (a_k + a_v) * 0.5: E_s = 1.01 ((|da_k| + |da_v|) / 2 + u c).
 """
 import math
-import re
-from pathlib import Path
 
 import pytest
 import torch
@@ -36,14 +34,13 @@ from transformers import DynamicCache
 from oracle import press_oracle as O
 from tests import lagkv_backend as LB
 from tests.conftest import ulp16_diff
-from tests.gpu_support import (assert_compress, gpu_ids, lagkv_inputs, _masked, _name, _native, _prefill, same16,
-                               _shared, tiny_gpu_llama, ulp_at)
+from tests.gpu_support import (assert_compress, gpu_ids, lagkv_inputs, LANES_PER_ROW, lanes_per_row, _masked, _name,
+                               _native, _prefill, same16, _shared, tiny_gpu_llama, ulp_at)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
 U = 2.0 ** -24
 LAG_MAX = 1024
-ROOT = Path(__file__).resolve().parent.parent
 
 
 # --------------------------------------------------------------------------------------------------
@@ -176,20 +173,11 @@ HEAD_DIMS = (8, 16, 40, 64, 72, 96, 128, 200, 256)
 SWEEP = [(dt, D, cross) for dt in (torch.bfloat16, torch.float16) for D in HEAD_DIMS for cross in (False, True)]
 
 
-def _lpr(D: int) -> int:
-    nvec = D // 8
-    return 4 if nvec <= 4 else 8 if nvec <= 8 else 16 if nvec <= 16 else 32
-
-
-def test_sweep_reaches_every_instantiation():
+def test_sweep_reaches_every_lanes_per_row_instantiation():
     """CPU: the lanes-per-row instantiations of lagkv.cu, per dtype, are all reached by SWEEP."""
-    src = (ROOT / "kvpress_b200" / "csrc" / "lagkv.cu").read_text()
-    lprs = {int(x) for x in re.findall(r"KVP_LAG\((\d+)\);", src)}
-    assert lprs == {4, 8, 16, 32}
-    assert "launch_lagkv_t<__nv_bfloat16>" in src and "launch_lagkv_t<__half>" in src
-    reached = {(_name(dt), _lpr(D), cross) for dt, D, cross in SWEEP}
-    assert reached == {(n, lpr, cross) for n in ("bf16", "fp16") for lpr in lprs for cross in (False, True)}
-    assert {_lpr(D) for D in HEAD_DIMS if D // 8 < _lpr(D)} == {4, 8, 16, 32}  # idle lanes in every instantiation
+    reached = {(_name(dt), lanes_per_row(D), cross) for dt, D, cross in SWEEP}
+    assert reached == {(n, lpr, cross) for n in ("bf16", "fp16") for lpr in LANES_PER_ROW for cross in (False, True)}
+    assert {lanes_per_row(D) for D in HEAD_DIMS if D // 8 < lanes_per_row(D)} == set(LANES_PER_ROW)  # idle lanes
 
 
 @gpu
