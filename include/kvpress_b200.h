@@ -106,7 +106,8 @@ const char* kvp_status_string(int status);
 /* Last CUDA error string recorded on this host thread by a failed call (never NULL). */
 const char* kvp_last_cuda_error(void);
 
-/* Bytes of scratch a *_compress / *_score call of this scorer needs (256-byte aligned). */
+/* Bytes of scratch a *_compress / *_score call of this scorer needs (256-byte aligned), whatever its other arguments:
+ * every SnapKV window, ObservedAttention n_q, CUR window / rank, ... the call accepts. */
 int kvp_workspace_bytes(const kvp_problem* p, int scorer, size_t* bytes_out);
 
 /* Debugging aid. The persistent select / compact kernels wait on each other with BOUNDED spins; a wait that

@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <cstddef>
 #include <type_traits>
 
@@ -60,9 +61,13 @@ static int validate(const kvp_problem* p, Dims* d, bool need_kv_strides = true) 
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
-// The window kvp_workspace_bytes / kvp_workspace_check size a scorer's scratch for: the largest a call may pass (SnapKV's
-// supported windows, ObservedAttention's n_q = S).
-static int largest_window(const Dims& d, int scorer) { return scorer == KVP_SCORER_OBSERVED_ATTENTION ? d.S : 256; }
+// The window kvp_workspace_bytes / kvp_workspace_check size a scorer's scratch for: the largest a call may pass.
+// ObservedAttention: n_q = S. SnapKV: the most query rows G * window <= kSnapMaxRows with window < S (at least 1, so
+// that a group too wide for any window still reaches the launcher's unsupported-shape status).
+static int largest_window(const Dims& d, int scorer) {
+    if (scorer == KVP_SCORER_OBSERVED_ATTENTION) return d.S;
+    return std::max(1, std::min(kSnapMaxRows / (d.Hq / d.H), d.S - 1));
+}
 
 // The workspace of a call: sized when `base` is null, carved otherwise. `window` is SnapKV's window, or the query rows
 // n_q of ObservedAttention. Returns the total bytes and, in *zeroed, the

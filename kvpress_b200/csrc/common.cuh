@@ -23,6 +23,7 @@ constexpr int kScoreChunkGeneric = 256;   // positions per CTA of the plain stre
 constexpr int kLagMax = 1024;              // largest LagKV lag_size (partition length) the kernel scores
 constexpr int kCurWindowMax = 1024;        // largest CUR local_window_size the kernel scores
 constexpr int kCurRankMax = 32;            // most columns of a CUR projection G the kernel scores
+constexpr int kSnapMaxRows = 512;          // most query rows G * window per kv head the SnapKV kernels score
 // counters[] layout: [0] ticket, [1, 1+R) refine done, [1+R, 1+2R) row ready, then the slot below:
 // order-preserving uint image of the largest valid score (for the reference's max+1 sentinel);
 // [2+2R, 2+3R) score items done per row (fused Knorm kernel)

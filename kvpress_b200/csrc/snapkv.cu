@@ -20,6 +20,7 @@
 // Both MMA kernels are persistent (one CTA per SM), warp-specialised: one TMA producer thread and two consumer
 // warpgroups that issue wgmma and reduce their register accumulators; while one warpgroup reduces, the other's
 // MMAs run.
+#include <algorithm>
 #include <type_traits>
 
 #include "qk_tiles.cuh"
@@ -33,13 +34,16 @@ struct SnapScratch {
     float* colsum;    // [R][S_pad]        sum_r p[r, j]
 };
 
+// The parts of a row: launch_snap_t splits a row over at most one CTA per 128-key tile, and at most kSnMaxParts.
+static int snap_max_parts(const Dims& d) { return std::min(kSnMaxParts, (d.S + kSnTile - 1) / kSnTile); }
+
 // The scratch in ws.scorer; with a null base only its size (*bytes).
 static SnapScratch carve_snap(const Dims& d, int window, void* base, size_t* bytes = nullptr) {
     const size_t NQ = (size_t)(d.Hq / d.H) * window;
     const size_t S_pad = (size_t)((d.S + kTile - 1) / kTile) * kTile;
     Carve c(base);
     SnapScratch s;
-    s.partial = c.take<float2>((size_t)d.R * NQ * kSnMaxParts);
+    s.partial = c.take<float2>((size_t)d.R * NQ * snap_max_parts(d));
     s.colsum = c.take<float>((size_t)d.R * S_pad);
     if (bytes) *bytes = c.bytes;
     return s;
@@ -321,8 +325,7 @@ static cudaError_t launch_snap_t(const Dims& d, int dtype, const void* K, const 
     const int n_tiles128 = (d.S + kSnTile - 1) / kSnTile;
     int ctas_per_row = sm_count / d.R;
     if (ctas_per_row < 1) ctas_per_row = 1;
-    if (ctas_per_row > n_tiles128) ctas_per_row = n_tiles128;
-    if (ctas_per_row > kSnMaxParts) ctas_per_row = kSnMaxParts;
+    if (ctas_per_row > snap_max_parts(d)) ctas_per_row = snap_max_parts(d);  // the parts carve_snap sized
     int n_groups = sm_count / ctas_per_row;
     if (n_groups > d.R) n_groups = d.R;
     const int grid = n_groups * ctas_per_row;
@@ -363,7 +366,7 @@ static cudaError_t launch_snap_d(const Dims& d, int dtype, const void* K, const 
     const int NQ = G * window;
     // any group size / window with G * window <= 512 query rows per kv head: the resident Q block is padded to
     // 128 / 256 / 512 rows, padding rows are computed and ignored (Llama-3.2-3B: G = 3, Qwen2-7B: G = 7, ...)
-    if (NQ < 1 || NQ > 512) return cudaErrorNotSupported;
+    if (NQ < 1 || NQ > kSnapMaxRows) return cudaErrorNotSupported;
     const int NQP = NQ <= 128 ? 128 : (NQ <= 256 ? 256 : 512);
 #define KVP_SNAP(DD, NN) \
     if (d.D == DD && NQP == NN) return launch_snap_t<T, DD, NN>(d, dtype, K, q_window, window, kernel_size, ws, scores_out, st)

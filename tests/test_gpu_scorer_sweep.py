@@ -198,6 +198,46 @@ def test_snapkv_kernel_sizes_and_windows(dtype, G, window, S, kernel_size):
     run_snap(k, v, q, window, kernel_size, f"snapkv {_name(dtype)} G={G} w={window} S={S} k={kernel_size}")
 
 
+SNAP_MHA = [(dt, D, w) for dt in DTYPES for D in (64, 128) for w in (257, 384, 511)]
+
+
+@gpu
+@pytest.mark.parametrize("dtype,D,window", SNAP_MHA, ids=[f"{_name(a)}-d{b}-w{c}" for a, b, c in SNAP_MHA])
+def test_snapkv_one_query_head_per_kv_head_windows_above_256(dtype, D, window):
+    """Multi-head attention (G = 1) with windows of 257 to 511: the 512-row instantiation with up to half of its rows
+    padding, as a process's first call (the per-stream workspaces dropped, so none is larger than this call asks)."""
+    _native()._WS_CACHE.clear()
+    k, v, q = snap_inputs(3, 1, 1, 1500, D, window, dtype, 800 + window + D)
+    run_snap(k, v, q, window, 5, f"snapkv {snap_instantiation(dtype, D, 1, window)} G=1 w={window}")
+
+
+@gpu
+def test_snapkv_press_window_300_on_a_multi_head_llama():
+    """SnapKVPress(window_size=300) on a multi-head-attention model, as the first call of the process's workspaces."""
+    from transformers import DynamicCache
+
+    from kvpress_b200 import SnapKVPress
+    from kvpress_b200.presses.scorer_press import kept_count
+    from tests.tiny_models import tiny_llama
+
+    nat = _native()
+    model = tiny_llama(dtype=torch.bfloat16, device=DEV, head_dim=128, heads=4, kv_heads=4)
+    ids = torch.randint(2, 250, (1, 1000), device=DEV, generator=torch.Generator(device=DEV).manual_seed(5))
+    full = DynamicCache()
+    model.model(input_ids=ids, past_key_values=full)
+    nat._WS_CACHE.clear()
+    cache = DynamicCache()
+    with SnapKVPress(compression_ratio=0.5, window_size=300)(model):
+        model.model(input_ids=ids, past_key_values=cache)
+    n_kept = kept_count(1000, 0.5)
+    assert cache.get_seq_length() == n_kept
+    for lf, lc in zip(full.layers, cache.layers):
+        # the window is kept, and every kept row is a row of the full cache (values are gathered as they are)
+        assert torch.equal(lc.values[:, :, n_kept - 300:], lf.values[:, :, -300:])
+        hit = (lc.values[:, :, :, None, :] == lf.values[:, :, None, :, :]).all(-1).any(-1)
+        assert hit.all(), "a kept value row is not a row of the full cache"
+
+
 # ---------------------------------------------------------------------------------------------------
 # 3. persistent schedules: each shape asserts the regime it is meant to reach on this device
 # ---------------------------------------------------------------------------------------------------
