@@ -3,9 +3,9 @@
 // stream. Never allocates, never synchronises (except kvp_workspace_check), never throws.
 #include <math.h>
 #include <stdio.h>
-#include <stdlib.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstddef>
 #include <type_traits>
 
@@ -179,20 +179,22 @@ static int no_operands(const Dims&) { return KVP_OK; }
 
 enum class KnormPath { cluster, fused, two_kernels };
 
+// The first KnormPath knorm_path may take; only kvp_debug_knorm_first_path changes it, so that the tests can run one
+// input through every path.
+static std::atomic<int> g_knorm_first_path{0};
+
 // The kernels kvp_knorm_compress runs. `d` is null for a problem that failed validation: kvp_launches_per_compress
 // still counts one, by its size alone.
 static KnormPath knorm_path(const kvp_problem& p, const Dims* d) {
+    const int first = g_knorm_first_path.load(std::memory_order_relaxed);
     // DecodingPress-sized caches: one launch of the cluster kernel (knorm_cluster.cu), no memset, no scratch
-    if (d != nullptr && knorm_cluster_applicable(*d)) return KnormPath::cluster;
+    if (first <= 0 && d != nullptr && knorm_cluster_applicable(*d)) return KnormPath::cluster;
     // Small caches beyond the cluster path are launch-latency-bound: one persistent kernel does score + select +
     // compact. Large caches measured faster as two kernels (the fused kernel's mixed read/write item stream costs
     // more HBM efficiency than the saved launch; K re-reads miss L2 anyway).
-    static const size_t fused_max_bytes = [] {  // A/B knob: KVP_KNORM_FUSED_MAX_MB (default 32)
-        const char* v = getenv("KVP_KNORM_FUSED_MAX_MB");
-        return (size_t)((v && *v) ? atoll(v) : 32) << 20;
-    }();
+    constexpr size_t kFusedMaxBytes = (size_t)32 << 20;
     const size_t k_bytes = (size_t)p.B * p.Hkv * p.S * p.D * 2;
-    return k_bytes <= fused_max_bytes ? KnormPath::fused : KnormPath::two_kernels;
+    return first <= 1 && k_bytes <= kFusedMaxBytes ? KnormPath::fused : KnormPath::two_kernels;
 }
 
 }  // namespace kvp
@@ -311,6 +313,13 @@ int kvp_knorm_compress(const kvp_problem* p, const void* K, const void* V, void*
     }
     if ((rc = status(launch_knorm_score(c.d, p->dtype, K, c.ws, scores_out, true, c.st)))) return rc;
     return status(launch_select_compact(c.d, K, V, K_out, V_out, idx_out, c.ws, c.st));
+}
+
+// Test hook, not in the public header: the first path knorm_path may take (0 = cluster, the default; 1 = fused;
+// 2 = two kernels). Returns the previous value, or -1 (nothing changed) for any other `first`.
+int kvp_debug_knorm_first_path(int first) {
+    if (first < 0 || first > 2) return -1;
+    return g_knorm_first_path.exchange(first, std::memory_order_relaxed);
 }
 
 // ---- KeyDiff -------------------------------------------------------------------------------------

@@ -14,10 +14,6 @@
 #include "common.cuh"
 #include "knorm_chunk.cuh"
 
-#ifndef KVP_KD_BUTTERFLY
-#define KVP_KD_BUTTERFLY 0
-#endif
-
 namespace kvp {
 
 struct KeyDiffScratch {
@@ -202,28 +198,11 @@ keydiff_score_kernel(const T* __restrict__ K, Strides3 ks, int H, int S, int D, 
                 dot = fmaf(p.x, a[2 * j], dot);
                 dot = fmaf(p.y, a[2 * j + 1], dot);
             }
-#if KVP_KD_BUTTERFLY
-            // prepared experiment (default off, see DESIGN §5.3): one butterfly for both sums — after the first
-            // exchange the lower half of the sub-warp owns ss and the upper half owns dot; log2(LPR)+1 shuffles
-            // instead of 2*log2(LPR)
-            {
-                constexpr int HALF = LPR / 2;
-                const bool upper = (sub & HALF) != 0;
-                float keep = upper ? dot : ss;
-                keep += __shfl_xor_sync(0xFFFFFFFFu, upper ? ss : dot, HALF);
-#pragma unroll
-                for (int off = HALF / 2; off >= 1; off >>= 1) keep += __shfl_xor_sync(0xFFFFFFFFu, keep, off);
-                const float other = __shfl_xor_sync(0xFFFFFFFFu, keep, HALF);
-                ss = upper ? other : keep;
-                dot = upper ? keep : other;
-            }
-#else
 #pragma unroll
             for (int off = LPR / 2; off >= 1; off >>= 1) {
                 ss += __shfl_xor_sync(0xFFFFFFFFu, ss, off);
                 dot += __shfl_xor_sync(0xFFFFFFFFu, dot, off);
             }
-#endif
             if (sub == 0) {
                 const int sl = warp * TOK_PER_WARP + (it + u) * RPW + rsel;
                 const float cosv = dot / fmaxf(sqrtf(ss), 1e-8f) * inv_anorm;

@@ -6,8 +6,6 @@
 // (a sub-warp of LPR lanes per 2*D-byte row, U independent loads in flight per lane), stages
 // the 16-bit ordered keys in shared memory, writes them coalesced and adds the tile's
 // histogram of (key >> 8) to the row histogram the select stage starts from.
-#include <stdlib.h>
-
 #include "common.cuh"
 #include "knorm_chunk.cuh"
 
@@ -16,19 +14,14 @@ namespace kvp {
 template <typename T, int LPR>
 __global__ void __launch_bounds__(kTileThreads)
 knorm_score_kernel(const T* __restrict__ K, Strides3 ks, int H, int S, int D, Workspace ws,
-                   uint16_t* __restrict__ scores_out, int want_keys, int keep_from_row) {
+                   uint16_t* __restrict__ scores_out, int want_keys) {
     __shared__ uint16_t skeys[kScoreChunk];
     __shared__ uint16_t sscores[kScoreChunk];
     __shared__ uint32_t shist[256];
     const int chunk = blockIdx.x, row = blockIdx.y, tid = threadIdx.x;
     shist[tid] = 0;  // kTileThreads == 256
     pdl_launch_dependents();  // the select+compact kernel behind this one may start to take residency
-    // L2 plan of a compress call (keep_from_row >= 0): the compaction stage re-reads the kept K rows, last rows first.
-    // The rows it reaches while they can still be in L2 are loaded evict_last, the earlier ones evict_first, so that
-    // the stream of early rows does not push the late ones out.
-    if (keep_from_row < 0) knorm_score_chunk<T, LPR>(K, ks, row / H, row % H, chunk, S, D, skeys, sscores);
-    else if (row >= keep_from_row) knorm_score_chunk<T, LPR, 1>(K, ks, row / H, row % H, chunk, S, D, skeys, sscores);
-    else knorm_score_chunk<T, LPR, 2>(K, ks, row / H, row % H, chunk, S, D, skeys, sscores);
+    knorm_score_chunk<T, LPR>(K, ks, row / H, row % H, chunk, S, D, skeys, sscores);
     __syncthreads();
     flush_or_store_scores(skeys, sscores, shist, row, chunk * kScoreChunk, S, ws, scores_out, want_keys);
 }
@@ -39,21 +32,8 @@ static cudaError_t launch_knorm_t(const Dims& d, const void* K, const Workspace&
     dim3 grid((d.S + kScoreChunk - 1) / kScoreChunk, d.R);
     const T* Kp = static_cast<const T*>(K);
     uint16_t* so = static_cast<uint16_t*>(scores_out);
-    // rows whose K (row_bytes each) fits kKeepBytes of L2 at the end of the pass are kept for the compaction stage
-    static const long long keep_mb = [] {  // A/B knob: KVP_KNORM_L2_KEEP_MB (default 0 = no hints: measured no gain)
-        const char* v = getenv("KVP_KNORM_L2_KEEP_MB");
-        return (long long)((v && *v) ? atoll(v) : 0);
-    }();
-    int keep_from_row = -1;
-    const long long row_bytes = (long long)d.S * d.D * 2;
-    if (want_keys && keep_mb > 0 && (long long)d.R * row_bytes > (keep_mb << 20)) {
-        const long long n_keep = (keep_mb << 20) / row_bytes;
-        keep_from_row = d.R - (int)n_keep;  // n_keep == 0: everything evict_first except nothing kept
-        if (n_keep == 0) keep_from_row = -1;
-    }
     with_lanes_per_row(d.D, [&](auto lpr) {
-        knorm_score_kernel<T, lpr><<<grid, kTileThreads, 0, st>>>(Kp, d.ks, d.H, d.S, d.D, ws, so, want_keys ? 1 : 0,
-                                                                  keep_from_row);
+        knorm_score_kernel<T, lpr><<<grid, kTileThreads, 0, st>>>(Kp, d.ks, d.H, d.S, d.D, ws, so, want_keys ? 1 : 0);
     });
     return cudaPeekAtLastError();
 }

@@ -52,10 +52,9 @@ struct RowSums {
 // Writes -||k_s||_2 (rounded once to the storage dtype) and its ordered key for the 256 positions of
 // `chunk` into shared memory. 256 threads; a sub-warp of LPR lanes per 2*D-byte row, U independent
 // 128-bit loads in flight per lane. Caller synchronises before reading skeys / sscores.
-// kHint: L2 policy of the loads. 1 = evict_last (rows that the compaction stage re-reads soon: they should survive
-// in the 126 MB L2), 2 = evict_first (rows that will be long gone by then: they should not push the others out),
-// 0 = no hint.
-template <typename T, int LPR, int kHint = 0>
+// kEvictLast: the loads carry an L2 evict_last hint (rows that the compaction stage re-reads soon: they should survive
+// in the 126 MB L2); otherwise they carry no hint.
+template <typename T, int LPR, bool kEvictLast = false>
 __device__ __forceinline__ void knorm_score_chunk(const T* __restrict__ K, Strides3 ks, int b, int h,
                                                   int chunk, int S, int D, uint16_t* skeys,
                                                   uint16_t* sscores) {
@@ -72,7 +71,7 @@ __device__ __forceinline__ void knorm_score_chunk(const T* __restrict__ K, Strid
     const int nvec = D >> 3;      // 16-byte pieces per row
     const T* base = K + (int64_t)b * ks.b + (int64_t)h * ks.h + (int64_t)sub * 8;
     const int s_warp = chunk * kScoreChunk + warp * TOK_PER_WARP;
-    const uint64_t pol = kHint == 1 ? l2_policy_evict_last() : (kHint == 2 ? l2_policy_evict_first() : 0ull);
+    const uint64_t pol = kEvictLast ? l2_policy_evict_last() : 0ull;
 
 #pragma unroll 1
     for (int it = 0; it < ITERS; it += U) {
@@ -82,7 +81,7 @@ __device__ __forceinline__ void knorm_score_chunk(const T* __restrict__ K, Strid
             const int s = s_warp + (it + u) * RPW + rsel;
             v[u] = make_int4(0, 0, 0, 0);
             if (s < S && sub < nvec)
-                v[u] = kHint != 0 ? ldg_hint(base + (int64_t)s * ks.s, pol) : ldg_plain(base + (int64_t)s * ks.s);
+                v[u] = kEvictLast ? ldg_hint(base + (int64_t)s * ks.s, pol) : ldg_plain(base + (int64_t)s * ks.s);
         }
         float ssu[U];
 #pragma unroll

@@ -17,7 +17,6 @@
 //      registers from global memory when it was not staged — to their final places (ascending positions, ties to the lowest positions — same rule as select_compact.cu).
 // No global atomics, no flags, no workspace: the only inter-CTA communication is the key exchange.
 #include <cooperative_groups.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "umma.cuh"
@@ -25,22 +24,6 @@
 namespace cg = cooperative_groups;
 
 namespace kvp {
-
-#ifdef KVP_CL_PROFILE
-// phase timestamps (globaltimer, ns) of CTA (0, 0), thread 0
-__device__ unsigned long long g_cl_prof[16];
-__device__ __forceinline__ unsigned long long cl_now() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-#define CL_MARK(i) do { if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) g_cl_prof[i] = cl_now(); } while (0)
-extern "C" void kvp_debug_cluster_profile(unsigned long long* out) {
-    cudaMemcpyFromSymbol(out, g_cl_prof, 16 * sizeof(unsigned long long));
-}
-#else
-#define CL_MARK(i) do {} while (0)
-#endif
 
 constexpr int kClThreads = 256;
 constexpr int kClMaxKeysPerThread = 24;  // keys of the row a thread holds in registers: S <= 256 * 24 = 6144
@@ -115,7 +98,6 @@ knorm_cluster_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 
     // ---- 1. stage the slice [start, start + P): one bulk copy per row, all in flight at once --------------------------
     const int start = rank * P;
     const int n_rows = max(0, min(P, S - start));
-    CL_MARK(0);
     if (tid == 0) {
         umma::mbar_init(&load_bar, 1);
         umma::mbar_fence_init();
@@ -153,11 +135,8 @@ knorm_cluster_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 
     }
     // all CTAs of the cluster have started (their shared memory exists) before anyone writes into it; the barrier
     // overlaps the loads in flight
-    CL_MARK(1);
     cluster.sync();
-    CL_MARK(2);
     umma::mbar_wait(&load_bar, 0);
-    CL_MARK(3);
 
     // ---- score the slice from shared memory: one thread per row, fixed summation order ----------------------------------
     uint16_t* my_keys = all_keys + (size_t)rank * P;
@@ -188,7 +167,6 @@ knorm_cluster_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 
         my_keys[r] = key;
     }
     __syncthreads();
-    CL_MARK(4);
 
     // ---- 2. all-gather of the keys through distributed shared memory ---------------------------------------------
     {
@@ -200,9 +178,7 @@ knorm_cluster_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 
             for (int i = tid; i < n8; i += kClThreads) dst[i] = src[i];
         }
     }
-    CL_MARK(5);
     cluster.sync();  // release / acquire at cluster scope: every slice of all_keys is complete everywhere
-    CL_MARK(6);
 
     // ---- 3. exact threshold of the row, computed redundantly by every CTA -----------------------------------------
     // The whole row's keys sit in shared memory (position s at all_keys[s]: slices are contiguous); every thread takes
@@ -271,8 +247,6 @@ knorm_cluster_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 
     const uint32_t n_take = (uint32_t)n_kept - tot[0];  // ties (key == T) to take, lowest positions first
     const uint32_t gt_before = tot[1], eq_before = tot[2];
     __syncthreads();
-
-    CL_MARK(7);
     // ---- 4. rank the slice (position order) and copy the kept rows ------------------------------------------------
     uint32_t taken_eq = min(eq_before, n_take);  // ties already granted to lower positions
     const uint32_t out_base = gt_before + taken_eq;
@@ -307,7 +281,6 @@ knorm_cluster_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 
         taken_eq += took;
         __syncthreads();
     }
-    CL_MARK(8);
     if (count == 0) return;
     const int64_t out_row0 = (int64_t)row * n_kept + out_base;
     if (idx_out != nullptr)
@@ -350,7 +323,6 @@ knorm_cluster_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 
         }
     }
     bulk_store_wait();  // shared memory must stay valid until the bulk stores have read it
-    CL_MARK(9);
 }
 
 template <typename T, int KPT>
@@ -378,12 +350,8 @@ static cudaError_t launch_cluster_t(const Dims& d, const ClusterPlan& pl, const 
 }
 
 static bool choose_cluster(const Dims& d, ClusterPlan* pl) {
-    static const int knob_c = [] {  // A/B knob: cluster size (portable maximum 8); 0 disables the path
-        const char* v = getenv("KVP_KNORM_CLUSTER");
-        return (v && *v) ? atoi(v) : 8;
-    }();
-    if (knob_c <= 0 || d.R > 65535) return false;
-    int C = knob_c > 8 ? 8 : knob_c;
+    if (d.R > 65535) return false;
+    int C = 8;  // the portable maximum cluster size
     // few positions per row: a smaller cluster keeps every CTA busy
     while (C > 1 && (d.S + C - 1) / C < 64) C >>= 1;
     *pl = cluster_plan(d, C);

@@ -15,7 +15,6 @@
 //                    position order. Ties at T go to the lowest positions.
 // Tiles are visited in REVERSE order of the score stage so the K rows touched last (still in the
 // 126 MB L2) are re-read first.
-#include <stdlib.h>
 #include <type_traits>
 
 #include "common.cuh"
@@ -23,31 +22,9 @@
 
 namespace kvp {
 
-#ifdef KVP_SEL_PROFILE
-__device__ long long g_sel_prof[16];
-#define SEL_T0(name) const long long name = clock64()
-#define SEL_ACC(slot, name) do { if (blockIdx.x == 0 && threadIdx.x == 0) g_sel_prof[slot] += clock64() - name; } while (0)
-#define SEL_CNT(slot) do { if (blockIdx.x == 0 && threadIdx.x == 0) g_sel_prof[slot] += 1; } while (0)
-extern "C" void kvp_debug_sel_profile(long long* out, int reset) {
-    if (reset) {
-        long long z[16] = {0};
-        cudaMemcpyToSymbol(g_sel_prof, z, sizeof(z));
-    } else {
-        cudaMemcpyFromSymbol(out, g_sel_prof, 16 * sizeof(long long));
-    }
-}
-#else
-#define SEL_T0(name) do {} while (0)
-#define SEL_ACC(slot, name) do {} while (0)
-#define SEL_CNT(slot) do {} while (0)
-#endif
-
-// tuning knobs of the compact items
-#ifndef KVP_SEL_U
-#define KVP_SEL_U 3
-#define KVP_SEL_TWO true
-#define KVP_SEL_CTAS 3
-#endif
+constexpr int kSelU = 3;       // compact items: 16-byte vectors per thread and batch of copy_rows_kv
+constexpr int kSelCtas = 3;    // compact items: CTAs per SM of select_compact_kernel<void>
+constexpr int kRerotCtas = 4;  // re-rotating variant: 64 regs, 4 CTAs/SM (issue-bound on sincosf)
 
 constexpr int kTilesPerWarp = 2;                                  // refine: tiles per warp
 constexpr int kGroupTiles = (kTileThreads / 32) * kTilesPerWarp;  // tiles per refine item (16)
@@ -56,7 +33,7 @@ constexpr int kGroupTiles = (kTileThreads / 32) * kTilesPerWarp;  // tiles per r
 // K rows are plain loads (they may still sit in L2 from the score stage), V rows and all stores are
 // streamed (evict-first). The loads of two consecutive batches (2 x 2*U 16-byte loads per thread) are
 // issued before the first store, so a typical item (<= 128 kept rows of 256 B) is ONE memory round trip.
-template <int U, bool kTwoBatches>
+template <int U>
 __device__ __forceinline__ void copy_rows_kv(const char* __restrict__ srcK, int64_t k_row_bytes,
                                              const char* __restrict__ srcV, int64_t v_row_bytes,
                                              char* __restrict__ dstK, char* __restrict__ dstV,
@@ -90,21 +67,13 @@ __device__ __forceinline__ void copy_rows_kv(const char* __restrict__ srcK, int6
             }
         }
     };
-    if (kTwoBatches) {
-        for (int base = threadIdx.x; base < total; base += 2 * STEP) {
-            int4 ak[U], av[U], bk[U], bv[U];
-            load(ak, av, base);
-            const bool second = (base + STEP) < total;
-            if (second) load(bk, bv, base + STEP);
-            store(ak, av, base);
-            if (second) store(bk, bv, base + STEP);
-        }
-    } else {
-        for (int base = threadIdx.x; base < total; base += STEP) {
-            int4 ak[U], av[U];
-            load(ak, av, base);
-            store(ak, av, base);
-        }
+    for (int base = threadIdx.x; base < total; base += 2 * STEP) {
+        int4 ak[U], av[U], bk[U], bv[U];
+        load(ak, av, base);
+        const bool second = (base + STEP) < total;
+        if (second) load(bk, bv, base + STEP);
+        store(ak, av, base);
+        if (second) store(bk, bv, base + STEP);
     }
 }
 
@@ -367,7 +336,6 @@ __device__ __forceinline__ void compact_item(SelectSmem& sm, int row, int tile, 
     const int s = tile * kTile + tid;
     uint32_t key = 0;
     if (kKeysReady) key = __ldcg(&ws.keys[(size_t)row * ws.S_pad + s]);  // in flight during the wait below
-    SEL_T0(t_wait);
     // The row scan publishes tile_prefix[row][tile] = {kept_before + 1, tied_before + 1} last (the table is
     // zeroed by the per-call memset), so one polled load doubles as the readiness flag (bounded spin;
     // traps instead of hanging the GPU).
@@ -399,8 +367,6 @@ __device__ __forceinline__ void compact_item(SelectSmem& sm, int row, int tile, 
     }
     __syncthreads();
     if (sm.abort) return;
-    SEL_ACC(0, t_wait);
-    SEL_T0(t_rank);
     if (!kKeysReady) key = __ldcg(&ws.keys[(size_t)row * ws.S_pad + s]);
     const uint2 meta = make_uint2(sm.meta[0], sm.meta[1]);
     const uint2 before = make_uint2(sm.thr[0], sm.thr[1]);
@@ -433,8 +399,6 @@ __device__ __forceinline__ void compact_item(SelectSmem& sm, int row, int tile, 
     if (is_gt || (is_eq && eq_rank < tie_room)) sm.list[gt_rank + min(eq_rank, tie_room)] = s;
     const int count = (int)(tot_gt + min(tot_eq, tie_room));
     __syncthreads();
-    SEL_ACC(1, t_rank);
-    SEL_T0(t_copy);
     if (count > 0) {
         const int64_t out_row0 = (int64_t)row * n_kept + out_base;
         if (idx_out != nullptr && tid < count) idx_out[out_row0 + tid] = sm.list[tid];
@@ -444,16 +408,14 @@ __device__ __forceinline__ void compact_item(SelectSmem& sm, int row, int tile, 
         if (K_out == nullptr) {
             // selection only (kvp_scores_select): the kept positions in idx_out are the whole result
         } else if constexpr (std::is_void<TR>::value) {
-            copy_rows_kv<KVP_SEL_U, KVP_SEL_TWO>(k_src, ks.s * 2, v_src, vs.s * 2, K_out + out_row0 * row_bytes,
-                                                 V_out + out_row0 * row_bytes, row_bytes, sm.list, count, D >> 3);
+            copy_rows_kv<kSelU>(k_src, ks.s * 2, v_src, vs.s * 2, K_out + out_row0 * row_bytes,
+                                V_out + out_row0 * row_bytes, row_bytes, sm.list, count, D >> 3);
         } else {
             copy_rows_k_rerotated<TR>(k_src, ks.s * 2, K_out + out_row0 * row_bytes, row_bytes, sm.list, count, D,
                                       inv_freq, (int)out_base);
             copy_rows_single(v_src, vs.s * 2, V_out + out_row0 * row_bytes, row_bytes, sm.list, count, D >> 3);
         }
     }
-    SEL_ACC(2, t_copy);
-    SEL_CNT(3);
 }
 
 // Persistent select+compact kernel: CTAs pull items from one ticket counter. Items [0, nA) are the
@@ -461,11 +423,8 @@ __device__ __forceinline__ void compact_item(SelectSmem& sm, int row, int tile, 
 // flag), items [nA, nA + nB) the compact items (last rows / last tiles first, so K rows the score
 // stage touched last are re-read while still in L2). A compact item only waits for refine items,
 // which precede it in the queue and never wait themselves => no deadlock for any grid size.
-#ifndef KVP_REROT_CTAS
-#define KVP_REROT_CTAS 4  // re-rotating variant: 64 regs, 4 CTAs/SM (issue-bound on sincosf)
-#endif
 template <typename TR>
-__global__ void __launch_bounds__(kTileThreads, std::is_void<TR>::value ? KVP_SEL_CTAS : KVP_REROT_CTAS)
+__global__ void __launch_bounds__(kTileThreads, std::is_void<TR>::value ? kSelCtas : kRerotCtas)
 select_compact_kernel(const char* __restrict__ K, const char* __restrict__ V, Strides3 ks,
                       Strides3 vs, char* __restrict__ K_out, char* __restrict__ V_out,
                       int32_t* __restrict__ idx_out, int H, int S, int D, int n_kept,
@@ -475,26 +434,20 @@ select_compact_kernel(const char* __restrict__ K, const char* __restrict__ V, St
     const int n_groups = (ws.n_tiles + kGroupTiles - 1) / kGroupTiles;
     const int nA = R * n_groups, nB = R * ws.n_tiles;
     pdl_wait();  // keys + histograms of the score stage are complete and visible
-    SEL_T0(t_kernel);
     // The ticket of the NEXT item is drawn while the current one is processed (its round trip hides behind the item).
     // A CTA therefore holds one ticket it has not started; deadlock-free as before: a held refine ticket belongs to a
     // CTA that is processing an earlier refine item, and refine items never wait.
     uint32_t next_ticket = 0;
     if (threadIdx.x == 0) next_ticket = atomicAdd(&ws.counters[0], 1u);
     while (true) {
-        SEL_T0(t_ticket);
         __syncthreads();  // previous item's shared state is dead
         if (threadIdx.x == 0) sm.item = (int)next_ticket;
         __syncthreads();
-        SEL_ACC(4, t_ticket);
         const int item = sm.item;
         if (item >= nA + nB) break;
         if (threadIdx.x == 0) next_ticket = atomicAdd(&ws.counters[0], 1u);
         if (item < nA) {
-            SEL_T0(t_ref);
             refine_item(sm, item / n_groups, item % n_groups, n_groups, S, n_kept, ws);
-            SEL_ACC(5, t_ref);
-            SEL_CNT(6);
         } else {
             const int j = item - nA;
             const int row = R - 1 - j / ws.n_tiles;
@@ -502,7 +455,6 @@ select_compact_kernel(const char* __restrict__ K, const char* __restrict__ V, St
             compact_item<TR, true>(sm, row, tile, K, V, ks, vs, K_out, V_out, idx_out, H, S, D, n_kept, ws, inv_freq);
         }
     }
-    SEL_ACC(7, t_kernel);
 }
 
 template <typename Kern>
@@ -520,16 +472,9 @@ static cudaError_t launch_select_compact_t(const Dims& d, const void* K, const v
     auto kern = select_compact_kernel<TR>;
     static PerDeviceInt occupancy;  // one per <TR> instantiation of this launcher
     const int grid = persistent_grid(kern, kTileThreads, n_items, occupancy);
-#ifndef KVP_NO_PDL
     return launch_pdl(kern, dim3(grid), dim3(kTileThreads), 0, st, static_cast<const char*>(K),
                       static_cast<const char*>(V), d.ks, d.vs, static_cast<char*>(K_out), static_cast<char*>(V_out),
                       idx_out, d.H, d.S, d.D, d.n_kept, ws, inv_freq);
-#else
-    kern<<<grid, kTileThreads, 0, st>>>(static_cast<const char*>(K), static_cast<const char*>(V), d.ks, d.vs,
-                                        static_cast<char*>(K_out), static_cast<char*>(V_out), idx_out, d.H,
-                                        d.S, d.D, d.n_kept, ws, inv_freq);
-    return cudaPeekAtLastError();
-#endif
 }
 
 cudaError_t launch_select_compact(const Dims& d, const void* K, const void* V, void* K_out,
@@ -659,7 +604,7 @@ knorm_fused_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 ks
         if (it.kind == 0) {
             sm.hist[tid] = 0;
             if (k_evict_last)
-                knorm_score_chunk<T, LPR, 1>(K, ks, it.row / H, it.row % H, it.idx, S, D, skeys, sscores);
+                knorm_score_chunk<T, LPR, true>(K, ks, it.row / H, it.row % H, it.idx, S, D, skeys, sscores);
             else
                 knorm_score_chunk<T, LPR>(K, ks, it.row / H, it.row % H, it.idx, S, D, skeys, sscores);
             __syncthreads();
@@ -681,31 +626,20 @@ knorm_fused_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 ks
     }
 }
 
-// Debug / A-B knobs of the fused kernel's queue (read once): KVP_KNORM_FUSED_LAG = 1 | 2,
-// KVP_KNORM_FUSED_HEAD = percent of a row's score items in front of the mixed tail (lag 1),
-// KVP_KNORM_FUSED_KLAST = 1: score-stage K loads carry an L2 evict_last hint.
-static int env_int(const char* name, int dflt) {
-    const char* v = getenv(name);
-    return (v && *v) ? atoi(v) : dflt;
-}
-
 template <typename T>
 static cudaError_t launch_knorm_fused_t(const Dims& d, const void* K, const void* V, void* K_out,
                                         void* V_out, int32_t* idx_out, void* scores_out,
                                         const Workspace& ws, cudaStream_t st) {
-    static const int knob_lag = env_int("KVP_KNORM_FUSED_LAG", 0);
-    static const int knob_head = env_int("KVP_KNORM_FUSED_HEAD", 50);
-    static const int knob_klast = env_int("KVP_KNORM_FUSED_KLAST", -1);
     FusedQueue fq;
     fq.R = d.R;
     fq.nT = ws.n_tiles;
     fq.nA = (ws.n_tiles + kGroupTiles - 1) / kGroupTiles;
     // one kv-head row of K larger than ~8 MB: keep only two rows live in L2 (lag 1), else the latency-optimal lag 2
     const bool big_rows = (size_t)d.S * d.D * 2 >= ((size_t)8 << 20);
-    fq.lag = (knob_lag == 1 || knob_lag == 2) ? knob_lag : (big_rows ? 1 : 2);
+    fq.lag = big_rows ? 1 : 2;
     if (fq.lag > d.R) fq.lag = d.R;
-    fq.m_head = fq.lag == 1 ? (int)((long long)fq.nT * knob_head / 100) : 0;
-    const int k_last = knob_klast >= 0 ? knob_klast : (big_rows ? 1 : 0);
+    fq.m_head = fq.lag == 1 ? (int)((long long)fq.nT * 50 / 100) : 0;  // half a row's score items ahead of the tail
+    const int k_last = big_rows ? 1 : 0;  // big rows: score-stage K loads carry an L2 evict_last hint
     const long long total = fused_total_items(fq);
     if (total > 0x7FFFFFFFll) return cudaErrorNotSupported;
     with_lanes_per_row(d.D, [&](auto lpr) {
@@ -752,10 +686,10 @@ streaming_compact_kernel(const char* __restrict__ K, const char* __restrict__ V,
     if (idx_out != nullptr)
         for (int j = tid; j < count; j += kTileThreads) idx_out[out_row0 + j] = s_list[j];
     const int64_t row_bytes = (int64_t)D * 2;
-    copy_rows_kv<4, true>(K + ((int64_t)b * ks.b + (int64_t)h * ks.h) * 2, ks.s * 2,
-                 V + ((int64_t)b * vs.b + (int64_t)h * vs.h) * 2, vs.s * 2,
-                 K_out + out_row0 * row_bytes, V_out + out_row0 * row_bytes, row_bytes, s_list, count,
-                 D >> 3);
+    copy_rows_kv<4>(K + ((int64_t)b * ks.b + (int64_t)h * ks.h) * 2, ks.s * 2,
+                    V + ((int64_t)b * vs.b + (int64_t)h * vs.h) * 2, vs.s * 2,
+                    K_out + out_row0 * row_bytes, V_out + out_row0 * row_bytes, row_bytes, s_list, count,
+                    D >> 3);
 }
 
 cudaError_t launch_streaming_compress(const Dims& d, int n_sink, const void* K, const void* V,

@@ -35,32 +35,18 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 // Bounded wait: a barrier that never flips (a bug) traps instead of hanging the GPU.
 // try_wait carries a suspend-time hint: the waiting warp sleeps until the barrier's phase completes (or the hint
 // expires) instead of re-issuing the poll, so waiting roles do not take issue slots from the consumer warps.
-#ifndef KVP_MBAR_HINT_NS
-#define KVP_MBAR_HINT_NS 20000  // 0: plain polling (A/B)
-#endif
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     const uint32_t addr = smem_u32(bar);
     uint32_t done = 0;
     for (uint32_t spins = 0; !done; ++spins) {
-#if KVP_MBAR_HINT_NS > 0
         asm volatile(
             "{\n\t.reg .pred p;\n\t"
             "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
             "selp.u32 %0, 1, 0, p;\n\t}"
             : "=r"(done)
-            : "r"(addr), "r"(parity), "r"((uint32_t)KVP_MBAR_HINT_NS)  // sleep up to this long per poll, woken by the barrier
+            : "r"(addr), "r"(parity), "r"(20000u)  // sleep up to 20 us per poll, woken by the barrier
             : "memory");
         if (spins > (1u << 18)) __trap();  // > 5 s without progress
-#else
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(addr), "r"(parity)
-            : "memory");
-        if (spins > (1u << 26)) __trap();
-#endif
     }
 }
 

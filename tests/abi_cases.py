@@ -27,10 +27,11 @@ STRIDES = (256000, 128000, 128)
 PYTHON = [sys.executable, *(["-s"] if sys.flags.no_user_site else [])]
 
 
-def child_env(**knobs) -> dict:
-    """This process's environment with the library's KVP_* knobs at their defaults, then `knobs`."""
+def child_env(**extra) -> dict:
+    """This process's environment without the tests' KVP_* variables (KVP_RECORD_* re-records references), then
+    `extra`."""
     env = {k: v for k, v in os.environ.items() if not k.startswith("KVP_")}
-    env.update(knobs)
+    env.update(extra)
     return env
 
 

@@ -118,7 +118,7 @@ def matrix() -> dict:
 
 
 def test_every_status_workspace_size_and_launch_count_matches_the_recording():
-    got = in_child(f"{__name__}:matrix")  # the library's knobs at their defaults
+    got = in_child(f"{__name__}:matrix")
     names = {k: v.pop("names") for k, v in got.items() if "names" in v}
     if RECORD:
         STORE.write_text("{\n" + ",\n".join(f"{json.dumps(k)}: {json.dumps(v)}" for k, v in got.items()) + "\n}\n")

@@ -211,3 +211,18 @@ def test_ea_pair_kernel_partition_is_balanced_and_complete():
             assert touching == list(range(first, first + count)), (n_units, n_tp, n_pairs, u)
             assert 2 * count <= 160                                            # kEaMaxParts slots per (row, head)
     assert fn(4, 10, 41, 0, 0, out) == -1                                      # more pairs than items: the launcher clamps
+
+
+def test_sources_read_no_environment_and_switch_on_no_kvp_macro():
+    """What the library computes and which kernels it runs depend on its arguments alone: no source file calls getenv,
+    and no preprocessor conditional names a KVP_ macro (a switch nothing defines leaves one side of it uncompiled and
+    untested)."""
+    csrc = HEADER.parent.parent / "kvpress_b200" / "csrc"
+    files = sorted(f for f in csrc.rglob("*") if f.is_file())
+    assert any(f.suffix == ".cu" for f in files)
+    found = []
+    for f in files:
+        for n, line in enumerate(f.read_text().splitlines(), 1):
+            if "getenv" in line or re.match(r"\s*#\s*(if|ifdef|ifndef|elif)\b.*\bKVP_", line):
+                found.append(f"{f.name}:{n}: {line.strip()}")
+    assert not found, found

@@ -24,7 +24,7 @@ Bars (the helpers are those of tests/test_gpu_scorer_sweep.py):
      those scores, independent of the kernel's own;
   5. strided layouts are consumed in place and give outputs bitwise equal to contiguous copies;
   6. the same inputs give bitwise-equal outputs on the fused and two-kernel paths, and 1-ulp-close scores with a
-     canonical selection on the cluster path (child processes: the path knobs are read once per process);
+     canonical selection on the cluster path (`kvp_debug_knorm_first_path` sets the first path the dispatch may take);
   7. fused and two kernels: optional outputs do not change K' / V', two calls are bitwise equal, a captured call replays
      correctly on new inputs, and no bounded wait expires.
 Measured on an H100 80GB HBM3 (700 W power limit) over every case of this file: at most 1 ulp from the rounded fp64
@@ -52,12 +52,13 @@ DEV = "cuda:0"
 ROOT = Path(__file__).resolve().parent.parent
 CSRC = ROOT / "kvpress_b200" / "csrc"
 DTYPES = [torch.bfloat16, torch.float16]
-PATH_OF_LAUNCHES = {1: "cluster", 2: "fused", 3: "two_kernels"}
+PATHS = ("cluster", "fused", "two_kernels")  # in dispatch order: kvp_debug_knorm_first_path's 0, 1, 2
+PATH_OF_LAUNCHES = {1 + i: path for i, path in enumerate(PATHS)}
 
 
 # ---------------------------------------------------------------------------------------------------
 # the dispatch: knorm_path (api.cu), choose_cluster / cluster_plan / launch_knorm_cluster (knorm_cluster.cu),
-# launch_knorm_fused_t (select_compact.cu), launch_knorm_t (knorm.cu), all knobs at their defaults
+# launch_knorm_fused_t (select_compact.cu), launch_knorm_t (knorm.cu)
 # ---------------------------------------------------------------------------------------------------
 CL_THREADS, CL_MAX_KPT, CL_MAX_SMEM = 256, 24, 200 * 1024
 FUSED_MAX_BYTES = 32 << 20  # K bytes up to which the fused kernel runs
@@ -157,8 +158,6 @@ def layout_shape(where: str, kind: str):
 LAYOUT_CASES = [(where, kind, dt) for where in LAYOUT_SHAPES for kind in LAYOUTS for dt in DTYPES]
 
 CROSS_SHAPES = [(1, 8, 2560, 128), (2, 4, 5000, 64)]
-CROSS_RUNS = {"cluster": {}, "fused": {"KVP_KNORM_CLUSTER": "0"},
-              "two_kernels": {"KVP_KNORM_CLUSTER": "0", "KVP_KNORM_FUSED_MAX_MB": "0"}}
 CALL_SHAPES = {"fused": (2, 4, 6000, 128), "two_kernels": (3, 4, 12000, 128)}
 
 
@@ -178,19 +177,35 @@ import ctypes, importlib.util, json, sys
 spec = importlib.util.spec_from_file_location("kvp_native", sys.argv[1])
 nat = importlib.util.module_from_spec(spec)
 spec.loader.exec_module(nat)
-out = []
-for B, H, S, D in json.loads(sys.argv[2]):
-    p = nat.KvpProblem()
-    p.B, p.Hkv, p.Hq, p.S, p.D, p.n_kept, p.dtype = B, H, H, S, D, 1, 0
-    p.k_stride = p.v_stride = (ctypes.c_int64 * 3)(H * S * D, S * D, D)
-    out.append(nat.launches_per_compress(p, nat.SCORER_KNORM))
-print(json.dumps(out))
+lib = nat.load()
+
+
+def launches():
+    out = []
+    for B, H, S, D in json.loads(sys.argv[2]):
+        p = nat.KvpProblem()
+        p.B, p.Hkv, p.Hq, p.S, p.D, p.n_kept, p.dtype = B, H, H, S, D, 1, 0
+        p.k_stride = p.v_stride = (ctypes.c_int64 * 3)(H * S * D, S * D, D)
+        out.append(nat.launches_per_compress(p, nat.SCORER_KNORM))
+    return out
+
+
+res = {"default": launches(), "previous": []}
+for first in (1, 2, 0):
+    res["previous"].append(lib.kvp_debug_knorm_first_path(first))
+    res[str(first)] = launches()
+res["rejected"] = [lib.kvp_debug_knorm_first_path(first) for first in (-1, 3)]
+res["after_rejected"] = launches()
+print(json.dumps(res))
 """
 
 
 def test_knorm_dispatch_matches_launch_count():
     """kvp_launches_per_compress (1 = cluster, 2 = fused, 3 = two kernels) agrees with knorm_dispatch on every case
-    shape, and every case is listed under the path knorm_dispatch gives it. No device: a child process that sees none."""
+    shape, and every case is listed under the path knorm_dispatch gives it. kvp_debug_knorm_first_path(1 or 2) moves
+    every case to the path it forces, or to two kernels where K is too large for the fused kernel; the hook returns
+    the previous value, rejects values outside 0..2 and, set back to 0, restores the default dispatch. No device: a
+    child process that sees none."""
     cases = sorted(set(_all_cases()))
     for path, shape in cases:
         assert knorm_dispatch(*shape, torch.bfloat16).path == path, (path, shape)
@@ -199,8 +214,14 @@ def test_knorm_dispatch_matches_launch_count():
                        cwd=ROOT, env=child_env(CUDA_VISIBLE_DEVICES=""), capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, r.stderr[-4000:]
     got = json.loads(r.stdout.strip().splitlines()[-1])
-    wrong = [(shape, PATH_OF_LAUNCHES[n], path) for (path, shape), n in zip(cases, got) if PATH_OF_LAUNCHES[n] != path]
-    assert not wrong, f"(shape, library path, restated path): {wrong}"
+    assert got["previous"] == [0, 1, 2] and got["rejected"] == [-1, -1]
+    assert got["0"] == got["default"] and got["after_rejected"] == got["default"]
+    for first in ("default", "1", "2"):
+        forced = 0 if first == "default" else int(first)
+        want = [PATHS[max(PATHS.index(path), forced)] for path, _ in cases]
+        wrong = [(shape, PATH_OF_LAUNCHES[n], w) for (_, shape), n, w in zip(cases, got[first], want)
+                 if PATH_OF_LAUNCHES[n] != w]
+        assert not wrong, f"first path {first}: (shape, library path, restated path): {wrong}"
 
 
 def test_lanes_per_row_follows_common():
@@ -472,42 +493,35 @@ def test_knorm_strided_layouts(where, kind, dtype):
 
 
 # ---------------------------------------------------------------------------------------------------
-# 4. the three paths on the same inputs (child processes: KVP_KNORM_CLUSTER / KVP_KNORM_FUSED_MAX_MB are read once
-#    per process)
+# 4. the three paths on the same inputs (kvp_debug_knorm_first_path moves the cluster-sized cases off the cluster path)
 # ---------------------------------------------------------------------------------------------------
-_CROSS_CHILD = r"""
-import importlib.util, json, sys
-import torch
-spec = importlib.util.spec_from_file_location("kvp_native", sys.argv[1])
-nat = importlib.util.module_from_spec(spec)
-spec.loader.exec_module(nat)
-nat.load()
-launches, res = int(sys.argv[3]), {}
-for dt in (torch.bfloat16, torch.float16):
-    for B, H, S, D in json.loads(sys.argv[4]):
-        gen = torch.Generator(device="cuda:0").manual_seed(S * 31 + D)
-        scale = torch.exp2(torch.rand(B, H, S, 1, generator=gen, device="cuda:0") * 16 - 8)
-        k = (torch.randn(B, H, S, D, generator=gen, device="cuda:0") * scale).to(dt)
-        v = torch.randn(B, H, S, D, generator=gen, device="cuda:0").to(dt)
-        for n in (257, S // 2):
-            assert nat.launches_per_compress(nat.make_problem(k, v, n), nat.SCORER_KNORM) == launches
-            out = nat.knorm_compress(k, v, n, return_indices=True, return_scores=True)
-            res[f"{dt}-{B}x{H}x{S}x{D}-{n}"] = [t.cpu() for t in (k, v, *out)]
-torch.save(res, sys.argv[2])
-"""
+def _run_cross(nat, launches):
+    """{case: [k, v, k_out, v_out, idx, scores]} of every CROSS_SHAPES input on the path that takes `launches`."""
+    res = {}
+    for dt in DTYPES:
+        for B, H, S, D in CROSS_SHAPES:
+            gen = torch.Generator(device=DEV).manual_seed(S * 31 + D)
+            scale = torch.exp2(torch.rand(B, H, S, 1, generator=gen, device=DEV) * 16 - 8)
+            k = (torch.randn(B, H, S, D, generator=gen, device=DEV) * scale).to(dt)
+            v = torch.randn(B, H, S, D, generator=gen, device=DEV).to(dt)
+            for n in (257, S // 2):
+                assert nat.launches_per_compress(nat.make_problem(k, v, n), nat.SCORER_KNORM) == launches
+                out = nat.knorm_compress(k, v, n, return_indices=True, return_scores=True)
+                res[f"{dt}-{B}x{H}x{S}x{D}-{n}"] = [k, v, *out]
+    return res
 
 
 @gpu
-def test_knorm_paths_agree_on_one_input(tmp_path):
+def test_knorm_paths_agree_on_one_input_through_the_first_path_hook():
+    nat = _native()
+    lib = nat.load()
     got = {}
-    for path, knobs in CROSS_RUNS.items():
-        out = tmp_path / f"{path}.pt"
-        launches = {"cluster": 1, "fused": 2, "two_kernels": 3}[path]
-        r = subprocess.run([*PYTHON, "-c", _CROSS_CHILD, str(ROOT / "kvpress_b200" / "native.py"), str(out),
-                            str(launches), json.dumps(CROSS_SHAPES)],
-                           cwd=ROOT, env=child_env(**knobs), capture_output=True, text=True, timeout=300)
-        assert r.returncode == 0, f"{path}: {r.stderr[-4000:]}"
-        got[path] = torch.load(out)
+    for first, path in enumerate(PATHS):
+        previous = lib.kvp_debug_knorm_first_path(first)
+        try:
+            got[path] = _run_cross(nat, first + 1)
+        finally:
+            lib.kvp_debug_knorm_first_path(previous)
     assert len(got["cluster"]) == 2 * 2 * len(CROSS_SHAPES)
     for case, (k, v, k_out, v_out, idx, sc) in got["fused"].items():
         assert all(_same(a, b) for a, b in zip(got["cluster"][case][:2], (k, v))), f"{case}: inputs differ"

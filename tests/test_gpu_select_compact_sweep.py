@@ -57,15 +57,15 @@ TILE_THREADS = 256  # kTileThreads
 SFX_STRIDE = 264    # kSfxStride
 TILES_PER_WARP = 2  # kTilesPerWarp
 GROUP_TILES = TILE_THREADS // 32 * TILES_PER_WARP  # kGroupTiles: tiles per refine item
-SEL_U = 3           # KVP_SEL_U: 16-byte vectors per thread and batch in copy_rows_kv of the compact items
-SEL_CTAS = 3        # KVP_SEL_CTAS
-REROT_CTAS = 4      # KVP_REROT_CTAS
-STREAM_U = 4        # copy_rows_kv<4, true> of streaming_compact_kernel
+SEL_U = 3           # kSelU: 16-byte vectors per thread and batch in copy_rows_kv of the compact items
+SEL_CTAS = 3        # kSelCtas
+REROT_CTAS = 4      # kRerotCtas
+STREAM_U = 4        # copy_rows_kv<4> of streaming_compact_kernel
 MAX_ROWS = 65535    # B·Hkv: gridDim.y of the score kernels
 
 
 def copy_edges(u: int):
-    """copy_rows_kv<u, true> copies count·nvec vectors in steps of TILE_THREADS·u, two steps per loop iteration"""
+    """copy_rows_kv<u> copies count·nvec vectors in steps of TILE_THREADS·u, two steps per loop iteration"""
     step = TILE_THREADS * u
     return (step, 2 * step)
 
@@ -331,7 +331,7 @@ def _constant(text: str, name: str) -> int:
     return int(m.group(1), 0)
 
 
-def test_boundaries_follow_the_source_constants():
+def test_boundaries_follow_the_source_constexprs():
     """The constants the boundary lists are derived from are the sources'; the lists hold every edge they imply."""
     common = (CSRC / "common.cuh").read_text()
     sc = (CSRC / "select_compact.cu").read_text()
@@ -339,11 +339,13 @@ def test_boundaries_follow_the_source_constants():
     assert _constant(common, "kSfxStride") == SFX_STRIDE and SFX_STRIDE >= TILE + 2
     assert _constant(sc, "kTilesPerWarp") == TILES_PER_WARP
     assert "kGroupTiles = (kTileThreads / 32) * kTilesPerWarp" in sc
-    assert _constant(sc, "KVP_SEL_U") == SEL_U and _constant(sc, "KVP_SEL_CTAS") == SEL_CTAS
-    assert _constant(sc, "KVP_REROT_CTAS") == REROT_CTAS
-    assert "copy_rows_kv<KVP_SEL_U, KVP_SEL_TWO>(" in sc and "#define KVP_SEL_TWO true" in sc
+    assert _constant(sc, "kSelU") == SEL_U and _constant(sc, "kSelCtas") == SEL_CTAS
+    assert _constant(sc, "kRerotCtas") == REROT_CTAS
+    assert "copy_rows_kv<kSelU>(" in sc
+    copy = re.search(r"void copy_rows_kv\(.*?\n}", sc, re.S).group(0)
+    assert "base += 2 * STEP" in copy  # two steps per loop iteration, as copy_edges assumes
     streaming = re.search(r"streaming_compact_kernel\(.*?\n}", sc, re.S).group(0)
-    assert re.findall(r"copy_rows_kv<(\d+), true>", streaming) == [str(STREAM_U)]
+    assert re.findall(r"copy_rows_kv<(\d+)>", streaming) == [str(STREAM_U)]
     assert "p->B * p->Hkv > 65535" in (CSRC / "api.cu").read_text() and MAX_ROWS == 65535
     # S on both sides of 1, one group, one group + 1, two groups and two groups + 1 tiles
     for t in (1, GROUP_TILES, GROUP_TILES + 1, 2 * GROUP_TILES, 2 * GROUP_TILES + 1):
