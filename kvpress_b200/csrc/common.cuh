@@ -376,36 +376,31 @@ __device__ __forceinline__ void publish_max_valid(float m, const Workspace& ws) 
 // (DecodingPress compactions, per-layer prefill hooks).
 int device_sm_count();                         // SM count of the CURRENT device
 constexpr int kMaxDevices = 64;
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device). `done` is the CALLER's function-local
-// static (one per launcher instantiation): kernels that differ only in non-type template arguments share one function
-// POINTER TYPE, so a cache keyed on the template type of this helper would be shared between them.
-struct PerDeviceOnce {
-    unsigned long long mask = 0;  // bit per device; a lost race only repeats the idempotent call
-};
-template <typename Kern>
-static inline cudaError_t ensure_dynamic_smem(Kern kern, int bytes, PerDeviceOnce& done) {
+// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device). The kernel is the template argument, so
+// every kernel has its own cache.
+template <auto kKern>
+static inline cudaError_t ensure_dynamic_smem(int bytes) {
+    static unsigned long long done = 0;  // bit per device; a lost race only repeats the idempotent call
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < kMaxDevices && ((done.mask >> dev) & 1ull)) return cudaSuccess;
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e == cudaSuccess && dev >= 0 && dev < kMaxDevices) done.mask |= 1ull << dev;
+    if (dev >= 0 && dev < kMaxDevices && ((done >> dev) & 1ull)) return cudaSuccess;
+    e = cudaFuncSetAttribute(kKern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess && dev >= 0 && dev < kMaxDevices) done |= 1ull << dev;
     return e;
 }
-// resident CTAs per SM of a kernel (occupancy query) once per (kernel, device); `cache` as above
-struct PerDeviceInt {
-    int v[kMaxDevices] = {0};
-};
-template <typename Kern>
-static inline int cached_ctas_per_sm(Kern kern, int threads, PerDeviceInt& cache, int dyn_smem = 0) {
+// resident CTAs per SM of a kernel (occupancy query) once per (kernel, device)
+template <auto kKern>
+static inline int cached_ctas_per_sm(int threads, int dyn_smem = 0) {
+    static int per_dev[kMaxDevices] = {0};
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) dev = 0;
-    if (cache.v[dev] == 0) {
+    if (per_dev[dev] == 0) {
         int per_sm = 0;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, dyn_smem);
-        cache.v[dev] = per_sm > 0 ? per_sm : 1;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kKern, threads, dyn_smem);
+        per_dev[dev] = per_sm > 0 ? per_sm : 1;
     }
-    return cache.v[dev];
+    return per_dev[dev];
 }
 
 // ---- host: workspace layouts ------------------------------------------------------------------

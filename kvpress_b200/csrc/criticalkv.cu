@@ -19,7 +19,6 @@
 
 namespace kvp {
 
-constexpr int kCkvThreads = 384;  // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue
 constexpr int kCkvN = 128;        // Wo rows (output features) per chunk: the wgmma N
 constexpr int kCkvMt = 2;         // 64-row m-tiles per consumer warpgroup (DESIGN.md §3, CriticalKV)
 constexpr int kCkvRows = 2 * 64 * kCkvMt;  // positions per item
@@ -52,15 +51,13 @@ struct CkvSmem {
     static constexpr int kPanels = D / 64;                    // 64-element (128 B) panels along d
     static constexpr int kVBytes = kPanels * kCkvRows * 128;  // one V tile
     static constexpr int kWBytes = kPanels * kCkvN * 128;     // one Wo chunk
-    // Wo ring: as deep as shared memory allows next to the two V buffers, at most 4
-    static constexpr int kFit = (227 * 1024 - 1024 - 2 * kVBytes - 256) / kWBytes;
-    static constexpr int kStages = kFit >= 4 ? 4 : kFit;
+    static constexpr int kStages = umma::ring_stages(2 * kVBytes + 256, kWBytes);  // Wo ring next to two V buffers
     static_assert(kStages >= 2, "Wo ring needs two stages");
     static constexpr int kVOff = 0;
     static constexpr int kWOff = 2 * kVBytes;
     static constexpr int kBarOff = kWOff + kStages * kWBytes;
     static constexpr int kTotal = kBarOff + 256;
-    static_assert(kTotal + 1024 <= 227 * 1024, "shared memory budget");
+    static_assert(umma::smem_request(kTotal) <= umma::kSmemBudget, "shared memory budget");
 };
 
 // CTA p of n_workers owns the items [ckv_start(p), ckv_start(p + 1)): equal contiguous ranges.
@@ -75,7 +72,7 @@ __host__ __device__ inline long long ckv_start(int p, long long total, int n_wor
 // 8i + 2qd + 1), register by register, chunk after chunk; at the end of the item it adds its two sums and the four
 // threads of a row add theirs (xor 1, then xor 2). The order depends only on the shape.
 template <typename T, int D>
-__global__ void __launch_bounds__(kCkvThreads, 1)
+__global__ void __launch_bounds__(umma::kTmaCtaThreads, 1)
 criticalkv_kernel(const __grid_constant__ CUtensorMap mapV, const __grid_constant__ CUtensorMap mapW,
                   const uint16_t* __restrict__ base, int64_t sb, int64_t sh, uint16_t* __restrict__ scores_out, int H,
                   int G, int S, int R, int n_tiles, int n_chunks, int n_workers, float eps) {
@@ -84,25 +81,15 @@ criticalkv_kernel(const __grid_constant__ CUtensorMap mapV, const __grid_constan
     unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_v = smem + L::kVOff;
     unsigned char* s_w = smem + L::kWOff;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
-    constexpr int kStages = L::kStages;
-    uint64_t* w_full = bars;        // [kStages <= 4]
-    uint64_t* w_empty = bars + 4;   // [kStages]
-    uint64_t* v_full = bars + 8;    // [2]
-    uint64_t* v_empty = bars + 10;  // [2]
+    auto* w_ring = reinterpret_cast<umma::TmaRing<L::kStages>*>(smem + L::kBarOff);
+    auto* v_ring = reinterpret_cast<umma::TmaRing<2>*>(w_ring + 1);  // the two V buffers
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     if (tid == 0) {
         umma::prefetch_tmap(&mapV);
         umma::prefetch_tmap(&mapW);
-        for (int i = 0; i < kStages; ++i) {
-            umma::mbar_init(&w_full[i], 1);
-            umma::mbar_init(&w_empty[i], 8);  // lane 0 of each consumer warp, once its MMAs on the chunk completed
-        }
-        for (int i = 0; i < 2; ++i) {
-            umma::mbar_init(&v_full[i], 1);
-            umma::mbar_init(&v_empty[i], 8);
-        }
+        w_ring->init(umma::kTmaConsumerWarps);
+        v_ring->init(umma::kTmaConsumerWarps);
         umma::mbar_fence_init();
     }
     __syncthreads();
@@ -119,19 +106,15 @@ criticalkv_kernel(const __grid_constant__ CUtensorMap mapV, const __grid_constan
             for (long long it = i_begin; it < i_end; ++it, ++v_it) {
                 const int row = (int)(it / n_tiles), tile = (int)(it - (long long)row * n_tiles);
                 const int b = row / H, j = row % H;
-                const int vb = v_it & 1;
-                umma::mbar_wait(&v_empty[vb], ((v_it >> 1) & 1) ^ 1);
-                umma::mbar_arrive_expect_tx(&v_full[vb], L::kVBytes);
+                const int vb = v_ring->acquire(v_it, L::kVBytes);
                 for (int kp = 0; kp < L::kPanels; ++kp)
-                    umma::tma_load_4d(s_v + vb * L::kVBytes + kp * (kCkvRows * 128), &mapV, &v_full[vb], kp * 64,
+                    umma::tma_load_4d(s_v + vb * L::kVBytes + kp * (kCkvRows * 128), &mapV, v_ring->full(vb), kp * 64,
                                       tile * kCkvRows, j, b);
                 for (int gc = 0; gc < n_gc; ++gc, ++w_it) {
                     const int g = gc / n_chunks, c = gc - g * n_chunks;
-                    const int stage = w_it % kStages;
-                    umma::mbar_wait(&w_empty[stage], ((w_it / kStages) & 1) ^ 1);
-                    umma::mbar_arrive_expect_tx(&w_full[stage], L::kWBytes);
+                    const int stage = w_ring->acquire(w_it, L::kWBytes);
                     for (int kp = 0; kp < L::kPanels; ++kp)
-                        umma::tma_load_3d(s_w + stage * L::kWBytes + kp * (kCkvN * 128), &mapW, &w_full[stage],
+                        umma::tma_load_3d(s_w + stage * L::kWBytes + kp * (kCkvN * 128), &mapW, w_ring->full(stage),
                                           (j * G + g) * D + kp * 64, c * kCkvN, 0);
                 }
             }
@@ -143,15 +126,13 @@ criticalkv_kernel(const __grid_constant__ CUtensorMap mapV, const __grid_constan
         uint32_t w_it = 0, v_it = 0;
         for (long long it = i_begin; it < i_end; ++it, ++v_it) {
             const int row = (int)(it / n_tiles), tile = (int)(it - (long long)row * n_tiles);
-            const int vb = v_it & 1;
-            umma::mbar_wait(&v_full[vb], (v_it >> 1) & 1);
+            const int vb = v_ring->wait(v_it);
             const uint32_t v_base = umma::smem_u32(s_v + vb * L::kVBytes);
             float sum[kCkvMt][4];
 #pragma unroll
             for (int mt = 0; mt < kCkvMt; ++mt) sum[mt][0] = sum[mt][1] = sum[mt][2] = sum[mt][3] = 0.f;
             for (int gc = 0; gc < n_gc; ++gc, ++w_it) {
-                const int stage = w_it % kStages;
-                umma::mbar_wait(&w_full[stage], (w_it / kStages) & 1);
+                const int stage = w_ring->wait(w_it);
                 const uint32_t w_base = umma::smem_u32(s_w + stage * L::kWBytes);
 #pragma unroll
                 for (int mt = 0; mt < kCkvMt; ++mt) {
@@ -172,12 +153,9 @@ criticalkv_kernel(const __grid_constant__ CUtensorMap mapV, const __grid_constan
 #pragma unroll
                     for (int i = 0; i < kCkvN / 2; ++i) sum[mt][i & 3] += fabsf(acc[i]);
                 }
-                // the chunk's MMAs have completed: hand the stage back to the producer
-                __syncwarp();
-                if (lane == 0) umma::mbar_arrive(&w_empty[stage]);
+                w_ring->release(stage);  // the chunk's MMAs have completed
             }
-            __syncwarp();
-            if (lane == 0) umma::mbar_arrive(&v_empty[vb]);
+            v_ring->release(vb);
             const int b = row / H, j = row % H;
 #pragma unroll
             for (int mt = 0; mt < kCkvMt; ++mt) {
@@ -217,10 +195,9 @@ static cudaError_t launch_criticalkv_t(const Dims& d, const void* V, const void*
     int n_workers = device_sm_count();
     if ((long long)n_workers > total) n_workers = (int)total;  // every CTA owns at least one item
 
-    const int smem = L::kTotal + 1024;
-    auto kern = criticalkv_kernel<T, D>;
-    static PerDeviceOnce smem_set;  // one per <T, D> instantiation of this launcher
-    cudaError_t e = ensure_dynamic_smem(kern, smem, smem_set);
+    constexpr int smem = umma::smem_request(L::kTotal);
+    constexpr auto kern = criticalkv_kernel<T, D>;
+    cudaError_t e = ensure_dynamic_smem<kern>(smem);
     if (e != cudaSuccess) return e;
     CUtensorMap mapV, mapW;
     if ((e = make_tmap_cache(&mapV, V, d, d.vs, kCkvRows)) != cudaSuccess) return e;
@@ -228,9 +205,9 @@ static cudaError_t launch_criticalkv_t(const Dims& d, const void* V, const void*
     if ((e = make_tmap_rows(&mapW, wo, (uint64_t)d.Hq * D, hidden, wo_stride, 1, (uint64_t)wo_stride * hidden,
                             kCkvN)) != cudaSuccess)
         return e;
-    kern<<<n_workers, kCkvThreads, smem, st>>>(mapV, mapW, static_cast<const uint16_t*>(base), sb, sh,
-                                                static_cast<uint16_t*>(scores_out), d.H, d.Hq / d.H, d.S, d.R,
-                                                n_tiles, n_chunks, n_workers, eps);
+    kern<<<n_workers, umma::kTmaCtaThreads, smem, st>>>(mapV, mapW, static_cast<const uint16_t*>(base), sb, sh,
+                                                        static_cast<uint16_t*>(scores_out), d.H, d.Hq / d.H, d.S, d.R,
+                                                        n_tiles, n_chunks, n_workers, eps);
     return cudaPeekAtLastError();
 }
 

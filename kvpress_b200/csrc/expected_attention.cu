@@ -26,7 +26,6 @@
 namespace kvp {
 
 constexpr int kEaTile = 128;      // key rows per MMA tile (M)
-constexpr int kEaThreads = 384;   // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue
 constexpr int kEaMaxParts = 160;  // upper bound on CTAs per (b,h) row (>= SM count)
 constexpr int kEaVnormLoads = 8;  // 16-byte V loads in flight per lane of a value-norm warp
 
@@ -64,16 +63,14 @@ struct EaSmem {
     static constexpr int kCovBytes = GR * kPanels * kCovHeadPanel;
     static constexpr int kStageBytes = kPanels * kEaTile * 128;
     static constexpr int kBiasBytes = GR * D * 4;          // 2 sqrt(d) mu_g in fp32
-    // K-tile ring: as deep as shared memory allows, at most 4
-    static constexpr int kFit = (227 * 1024 - 1024 - kCovBytes - kBiasBytes - 512) / kStageBytes;
-    static constexpr int kStages = kFit >= 4 ? 4 : kFit;
+    static constexpr int kStages = umma::ring_stages(kCovBytes + kBiasBytes + 512, kStageBytes);
     static_assert(kStages >= 2, "K ring needs two stages");
     static constexpr int kCovOff = 0;
     static constexpr int kStageOff = kCovBytes;
     static constexpr int kBiasOff = kStageOff + kStages * kStageBytes;
     static constexpr int kBarOff = kBiasOff + kBiasBytes;
     static constexpr int kTotal = kBarOff + 512;
-    static_assert(kTotal + 1024 <= 227 * 1024, "shared memory budget");
+    static_assert(umma::smem_request(kTotal) <= umma::kSmemBudget, "shared memory budget");
 };
 
 // Work: unit = (row, group of GR query heads of its kv head); item = (unit, 128-position tile). The items are cut into
@@ -115,7 +112,7 @@ extern "C" int kvp_debug_ea_pair_partition(int n_units, int n_tp, int n_pairs, i
 // accumulator columns 8 j + 2 qd + {0, 1} for j = 2 kk, 2 kk + 1. A thread holds two rows and D/4 columns; the four
 // threads of a row add their partial dot products.
 template <typename T, int D, int GR>
-__global__ void __launch_bounds__(kEaThreads, 1)
+__global__ void __launch_bounds__(umma::kTmaCtaThreads, 1)
 ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapCov,
                  const T* __restrict__ mu, const T* __restrict__ V, Strides3 vs, int use_vnorm, int H, int Hq, int S,
                  int n_sink, int R, int n_tiles128, int n_workers, int n_parts, EaScratch sc, int S_pad, int g_total,
@@ -128,12 +125,9 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
     unsigned char* s_cov = smem + L::kCovOff;
     unsigned char* s_stage = smem + L::kStageOff;
     float* s_bias = reinterpret_cast<float*>(smem + L::kBiasOff);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
-    constexpr int kStages = L::kStages;
-    uint64_t* k_full = bars;          // [kStages <= 4]
-    uint64_t* k_empty = bars + 4;     // [kStages]
-    uint64_t* cov_full = bars + 8;    // [1]
-    float* s_red = reinterpret_cast<float*>(bars + 10);  // [8 warps][GR heads][2]
+    auto* k_ring = reinterpret_cast<umma::TmaRing<L::kStages>*>(smem + L::kBarOff);
+    uint64_t* cov_full = reinterpret_cast<uint64_t*>(k_ring + 1);
+    float* s_red = reinterpret_cast<float*>(cov_full + 1);  // [8 warps][GR heads][2]
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     const int P = blockIdx.x;
@@ -141,10 +135,7 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
     if (tid == 0) {
         umma::prefetch_tmap(&mapK);
         umma::prefetch_tmap(&mapCov);
-        for (int i = 0; i < kStages; ++i) {
-            umma::mbar_init(&k_full[i], 1);
-            umma::mbar_init(&k_empty[i], 8);  // lane 0 of each consumer warp, once its k rows are in registers
-        }
+        k_ring->init(umma::kTmaConsumerWarps);
         umma::mbar_init(cov_full, 1);
         umma::mbar_fence_init();
     }
@@ -170,7 +161,7 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
         const int part = P - first_cta;                 // this CTA's slot among the unit's softmax partials
 
         __syncthreads();  // every MMA of the previous unit has completed: s_cov, s_bias, s_red reusable
-        for (int n = tid; n < GR * D; n += kEaThreads)
+        for (int n = tid; n < GR * D; n += umma::kTmaCtaThreads)
             s_bias[n] = (n / D < n_real)
                             ? bias_scale * F16Traits<T>::to_float(reinterpret_cast<const uint16_t*>(mu)[(size_t)hq0 * D + n])
                             : 0.f;
@@ -185,12 +176,10 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                         umma::tma_load_3d(s_cov + (kp * GR + g) * L::kCovHeadPanel, &mapCov, cov_full, kp * 64, 0,
                                           hq0 + g);
                 for (int t = t_begin; t < t_end; ++t, ++k_it) {
-                    const int stage = k_it % kStages;
-                    umma::mbar_wait(&k_empty[stage], ((k_it / kStages) & 1) ^ 1);
-                    umma::mbar_arrive_expect_tx(&k_full[stage], L::kStageBytes);
+                    const int stage = k_ring->acquire(k_it, L::kStageBytes);
                     for (int kp = 0; kp < L::kPanels; ++kp)
                         umma::tma_load_4d(s_stage + stage * L::kStageBytes + kp * (kEaTile * 128), &mapK,
-                                          &k_full[stage], kp * 64, t * kEaTile, h, b);
+                                          k_ring->full(stage), kp * 64, t * kEaTile, h, b);
                 }
             } else if (warp > 0 && use_vnorm && g_off == 0) {
                 // ===== value norms of this CTA's positions of the row, next to the MMAs =====
@@ -210,17 +199,14 @@ ea_logits_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
             }
             umma::mbar_wait(cov_full, cov_it & 1);
             for (int t = t_begin; t < t_end; ++t, ++k_it) {
-                const int stage = k_it % kStages;
-                umma::mbar_wait(&k_full[stage], (k_it / kStages) & 1);
+                const int stage = k_ring->wait(k_it);
                 const uint32_t k_base = umma::smem_u32(s_stage + stage * L::kStageBytes);
                 uint32_t ka[D / 16][4];  // this warp's 16 rows of the tile: the A fragment of each k-step
 #pragma unroll
                 for (int kk = 0; kk < D / 16; ++kk)
                     umma::ldmatrix_x4(ka[kk], k_base + (kk >> 2) * (kEaTile * 128) +
                                                   umma::sw128_offset(r_ld, 2 * (kk & 3) + (lane >> 4)));
-                // the k rows are in registers: hand the stage back to the producer before the MMAs
-                __syncwarp();
-                if (lane == 0) umma::mbar_arrive(&k_empty[stage]);
+                k_ring->release(stage);  // the k rows are in registers: hand the stage back before the MMAs
                 // Head g's logits are finished (quad sum, scale, store, online max / sum-exp) while the tensor cores
                 // work on head g + 1: the MMAs are issued first, then the previous head's finish runs before the wait.
                 // Only the last head's finish is exposed. Both rows' shuffles come before the store branch, since a
@@ -548,13 +534,13 @@ static cudaError_t launch_ea_logits_t(const Dims& d, const void* K, const void* 
     cudaError_t e;
     if ((e = make_tmap_cache(&mapK, K, d, d.ks, kEaTile)) != cudaSuccess) return e;
     if ((e = make_tmap_rows(&mapCov, cov, D, D, D, (uint64_t)d.B * d.Hq, (uint64_t)D * D, D)) != cudaSuccess) return e;
-    const int smem = L::kTotal + 1024;
-    auto kern = ea_logits_kernel<T, D, GR>;
-    static PerDeviceOnce smem_set;  // one per <T, D, GR> instantiation of this launcher
-    if ((e = ensure_dynamic_smem(kern, smem, smem_set)) != cudaSuccess) return e;
-    kern<<<n_workers, kEaThreads, smem, st>>>(mapK, mapCov, static_cast<const T*>(mu), static_cast<const T*>(V), d.vs,
-                                              use_vnorm, d.H, d.Hq, d.S, n_sink, d.R, n_tiles128, n_workers, n_parts,
-                                              sc, ws.S_pad, g_total, n_split);
+    constexpr int smem = umma::smem_request(L::kTotal);
+    constexpr auto kern = ea_logits_kernel<T, D, GR>;
+    if ((e = ensure_dynamic_smem<kern>(smem)) != cudaSuccess) return e;
+    kern<<<n_workers, umma::kTmaCtaThreads, smem, st>>>(mapK, mapCov, static_cast<const T*>(mu),
+                                                        static_cast<const T*>(V), d.vs, use_vnorm, d.H, d.Hq, d.S,
+                                                        n_sink, d.R, n_tiles128, n_workers, n_parts, sc, ws.S_pad,
+                                                        g_total, n_split);
     return cudaPeekAtLastError();
 }
 

@@ -328,9 +328,8 @@ knorm_cluster_kernel(const T* __restrict__ K, const T* __restrict__ V, Strides3 
 template <typename T, int KPT>
 static cudaError_t launch_cluster_t(const Dims& d, const ClusterPlan& pl, const void* K, const void* V, void* K_out,
                                     void* V_out, int32_t* idx_out, void* scores_out, cudaStream_t st) {
-    auto kern = knorm_cluster_kernel<T, KPT>;
-    static PerDeviceOnce smem_set;  // one per <T, KPT> instantiation of this launcher
-    cudaError_t e = ensure_dynamic_smem(kern, kClMaxSmem, smem_set);
+    constexpr auto kern = knorm_cluster_kernel<T, KPT>;
+    cudaError_t e = ensure_dynamic_smem<kern>(kClMaxSmem);
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(pl.C, d.R, 1);

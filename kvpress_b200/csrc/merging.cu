@@ -157,7 +157,7 @@ __device__ __forceinline__ bool mg_better(float v, int c, float bv, int bc) {
 }
 
 template <typename T, int DP>
-__global__ void __launch_bounds__(kSnThreads, 1)
+__global__ void __launch_bounds__(umma::kTmaCtaThreads, 1)
 merging_argmax_kernel(const __grid_constant__ CUtensorMap mapE, const __grid_constant__ CUtensorMap mapT, int S_pad,
                       int n_kept, int n_evict, int R, MgScratch sc) {
     using L = SnSmem<DP, 128>;  // resident: 128 evicted rows; ring: 128 kept rows per stage
@@ -165,22 +165,15 @@ merging_argmax_kernel(const __grid_constant__ CUtensorMap mapE, const __grid_con
     unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_a = smem + L::kQOff;
     unsigned char* s_stage = smem + L::kStageOff;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
-    uint64_t* b_full = bars;       // [kStages <= 4]
-    uint64_t* b_empty = bars + 4;  // [kStages]
-    uint64_t* a_full = bars + 8;
-    uint64_t* a_empty = bars + 9;
+    auto* b_ring = reinterpret_cast<umma::TmaRing<L::kStages>*>(smem + L::kBarOff);
+    auto* a_ring = reinterpret_cast<umma::TmaRing<1>*>(b_ring + 1);  // the resident evicted block
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     if (tid == 0) {
         umma::prefetch_tmap(&mapE);
         umma::prefetch_tmap(&mapT);
-        for (int i = 0; i < L::kStages; ++i) {
-            umma::mbar_init(&b_full[i], 1);
-            umma::mbar_init(&b_empty[i], 8);  // lane 0 of each consumer warp
-        }
-        umma::mbar_init(a_full, 1);
-        umma::mbar_init(a_empty, 8);
+        b_ring->init(umma::kTmaConsumerWarps);
+        a_ring->init(umma::kTmaConsumerWarps);
         umma::mbar_fence_init();
     }
     __syncthreads();
@@ -195,17 +188,14 @@ merging_argmax_kernel(const __grid_constant__ CUtensorMap mapE, const __grid_con
             uint32_t b_it = 0, a_it = 0;
             for (int u = blockIdx.x; u < n_items; u += gridDim.x, ++a_it) {
                 const int row = u / n_blocks, blk = u % n_blocks;
-                umma::mbar_wait(a_empty, (a_it & 1) ^ 1);
-                umma::mbar_arrive_expect_tx(a_full, L::kQBytes);  // rows past n_evict read as zero
+                a_ring->acquire(a_it, L::kQBytes);  // rows past n_evict read as zero
                 for (int kp = 0; kp < L::kPanels; ++kp)
-                    umma::tma_load_3d(s_a + kp * L::kQPanel, &mapE, a_full, kp * 64, blk * 128, row);
+                    umma::tma_load_3d(s_a + kp * L::kQPanel, &mapE, a_ring->full(0), kp * 64, blk * 128, row);
                 for (int t = 0; t < n_tiles; ++t, ++b_it) {
-                    const int stage = b_it % L::kStages;
-                    umma::mbar_wait(&b_empty[stage], ((b_it / L::kStages) & 1) ^ 1);
-                    umma::mbar_arrive_expect_tx(&b_full[stage], L::kStageBytes);  // rows past n_kept read as zero
+                    const int stage = b_ring->acquire(b_it, L::kStageBytes);  // rows past n_kept read as zero
                     for (int kp = 0; kp < L::kPanels; ++kp)
-                        umma::tma_load_3d(s_stage + stage * L::kStageBytes + kp * kSnTile * 128, &mapT, &b_full[stage],
-                                          kp * 64, t * kSnTile, row);
+                        umma::tma_load_3d(s_stage + stage * L::kStageBytes + kp * kSnTile * 128, &mapT,
+                                          b_ring->full(stage), kp * 64, t * kSnTile, row);
                 }
             }
         }
@@ -218,17 +208,15 @@ merging_argmax_kernel(const __grid_constant__ CUtensorMap mapE, const __grid_con
             const float* inv_kept = sc.inv + (size_t)row * S_pad;
             float bv[2] = {-INFINITY, -INFINITY};
             int bc[2] = {INT_MAX, INT_MAX};
-            umma::mbar_wait(a_full, a_it & 1);
+            a_ring->wait(a_it);
             const uint32_t abase = umma::smem_u32(s_a) + cw * 64 * 128;
 #pragma unroll 1
             for (int t = 0; t < n_tiles; ++t, ++b_it) {
-                const int stage = b_it % L::kStages;
-                umma::mbar_wait(&b_full[stage], (b_it / L::kStages) & 1);
+                const int stage = b_ring->wait(b_it);
                 float acc[64];
                 snap_mma<T, DP>(acc, abase, L::kQPanel, umma::smem_u32(s_stage + stage * L::kStageBytes),
                                 kSnTile * 128);
-                __syncwarp();
-                if (lane == 0) umma::mbar_arrive(&b_empty[stage]);  // the product has completed: hand the stage back
+                b_ring->release(stage);  // the product has completed
                 // columns 8 jj + 2 qd + {0, 1} of the tile, ascending per thread
 #pragma unroll
                 for (int jj = 0; jj < 16; ++jj) {
@@ -247,8 +235,7 @@ merging_argmax_kernel(const __grid_constant__ CUtensorMap mapE, const __grid_con
                     }
                 }
             }
-            __syncwarp();
-            if (lane == 0) umma::mbar_arrive(a_empty);  // every product on the block has completed
+            a_ring->release(0);  // every product on the block has completed
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
                 float v = bv[hh];
@@ -602,11 +589,11 @@ static cudaError_t launch_mg_argmax(const Dims& d, const MgScratch& sc, int S_pa
         cudaSuccess)
         return e;
     if ((e = make_tmap_rows(&mapT, sc.keys, DP, d.n_kept, DP, d.R, head_stride, 128)) != cudaSuccess) return e;
-    const int smem = L::kTotal + 1024;
-    auto k = merging_argmax_kernel<T, DP>;
-    static PerDeviceOnce smem_set;  // one per <T, DP> instantiation of this launcher
-    if ((e = ensure_dynamic_smem(k, smem, smem_set)) != cudaSuccess) return e;
-    return launch_pdl(k, dim3(grid), dim3(kSnThreads), smem, st, mapE, mapT, S_pad, d.n_kept, n_evict, d.R, sc);
+    constexpr int smem = umma::smem_request(L::kTotal);
+    constexpr auto k = merging_argmax_kernel<T, DP>;
+    if ((e = ensure_dynamic_smem<k>(smem)) != cudaSuccess) return e;
+    return launch_pdl(k, dim3(grid), dim3(umma::kTmaCtaThreads), smem, st, mapE, mapT, S_pad, d.n_kept, n_evict, d.R,
+                      sc);
 }
 
 template <typename T>

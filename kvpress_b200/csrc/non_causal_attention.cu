@@ -74,22 +74,21 @@ struct NcaSmem {
     static constexpr int kPanel = CS * 128;  // bytes of one 64-column panel of a chunk
     static constexpr int kChunkBytes = kPanels * kPanel;
     static constexpr int kCbBytes = 2 * CS * 4;
-    static constexpr int kFit = (227 * 1024 - 1024 - kChunkBytes - kCbBytes - 256) / kChunkBytes;
-    static constexpr int kStages = kFit >= 4 ? 4 : kFit;
+    static constexpr int kStages = umma::ring_stages(kChunkBytes + kCbBytes + 256, kChunkBytes);
     static_assert(kStages >= 2, "Q ring needs two stages");
     static constexpr int kKOff = 0;
     static constexpr int kStageOff = kChunkBytes;
     static constexpr int kCbOff = kStageOff + kStages * kChunkBytes;
     static constexpr int kBarOff = kCbOff + kCbBytes;
     static constexpr int kTotal = kBarOff + 256;
-    static_assert(kTotal + 1024 <= 227 * 1024, "shared memory budget");
+    static_assert(umma::smem_request(kTotal) <= umma::kSmemBudget, "shared memory budget");
 };
 
 // ---- the column sums -------------------------------------------------------------------------------------------------
 // Consumer warpgroup cw owns the 64-row blocks cw, cw + 2, ... of the chunk: as query rows in pass A, as keys in pass B.
 // A thread holds rows (16 w + l/4, +8) of a block and 32 of the 128 columns of each product.
 template <typename T, int D, int CS>
-__global__ void __launch_bounds__(kSnThreads, 1)
+__global__ void __launch_bounds__(umma::kTmaCtaThreads, 1)
 nca_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapQ,
                   const T* __restrict__ V, Strides3 vs, int H, int G, int S, int R, int n_chunks, NcaScratch sc,
                   int S_pad) {
@@ -101,22 +100,15 @@ nca_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
     unsigned char* s_k = smem + L::kKOff;
     unsigned char* s_stage = smem + L::kStageOff;
     float* s_cb = reinterpret_cast<float*>(smem + L::kCbOff);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
-    uint64_t* q_full = bars;       // [kStages <= 4]
-    uint64_t* q_empty = bars + 4;  // [kStages]
-    uint64_t* k_full = bars + 8;
-    uint64_t* k_empty = bars + 9;
+    auto* q_ring = reinterpret_cast<umma::TmaRing<L::kStages>*>(smem + L::kBarOff);
+    auto* k_ring = reinterpret_cast<umma::TmaRing<1>*>(q_ring + 1);  // the resident K chunk
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     if (tid == 0) {
         umma::prefetch_tmap(&mapK);
         umma::prefetch_tmap(&mapQ);
-        for (int i = 0; i < L::kStages; ++i) {
-            umma::mbar_init(&q_full[i], 1);
-            umma::mbar_init(&q_empty[i], 8);  // lane 0 of each consumer warp, after pass B on the chunk
-        }
-        umma::mbar_init(k_full, 1);
-        umma::mbar_init(k_empty, 8);
+        q_ring->init(umma::kTmaConsumerWarps);
+        k_ring->init(umma::kTmaConsumerWarps);
         umma::mbar_fence_init();
     }
     __syncthreads();
@@ -130,20 +122,17 @@ nca_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                 const int c = u / R, row = u % R;
                 const int b = row / H, j = row % H;
                 const int n_qt = (min(CS, S - c * CS) + kSnTile - 1) / kSnTile;  // Q tiles holding valid rows
-                umma::mbar_wait(k_empty, (k_it & 1) ^ 1);
-                umma::mbar_arrive_expect_tx(k_full, L::kChunkBytes);  // key rows past S read as zero
+                k_ring->acquire(k_it, L::kChunkBytes);  // key rows past S read as zero
                 for (int t = 0; t < kTiles; ++t)
                     for (int kp = 0; kp < L::kPanels; ++kp)
-                        umma::tma_load_4d(s_k + kp * L::kPanel + t * kSnTile * 128, &mapK, k_full, kp * 64,
+                        umma::tma_load_4d(s_k + kp * L::kPanel + t * kSnTile * 128, &mapK, k_ring->full(0), kp * 64,
                                           c * CS + t * kSnTile, j, b);
                 for (int g = 0; g < G; ++g, ++q_it) {
-                    const int stage = q_it % L::kStages;
-                    umma::mbar_wait(&q_empty[stage], ((q_it / L::kStages) & 1) ^ 1);
-                    umma::mbar_arrive_expect_tx(&q_full[stage], (uint32_t)(n_qt * L::kPanels * kSnTile * 128));
+                    const int stage = q_ring->acquire(q_it, (uint32_t)(n_qt * L::kPanels * kSnTile * 128));
                     for (int t = 0; t < n_qt; ++t)
                         for (int kp = 0; kp < L::kPanels; ++kp)
                             umma::tma_load_3d(s_stage + stage * L::kChunkBytes + kp * L::kPanel + t * kSnTile * 128,
-                                              &mapQ, &q_full[stage], kp * 64, c * CS + t * kSnTile,
+                                              &mapQ, q_ring->full(stage), kp * 64, c * CS + t * kSnTile,
                                               (b * H + j) * G + g);
                 }
             }
@@ -165,15 +154,14 @@ nca_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
             const int n_valid = min(CS, S - c * CS);  // valid rows (queries and keys) of the chunk
             const int n_qt = (n_valid + kSnTile - 1) / kSnTile;
             const uint32_t kbase = umma::smem_u32(s_k);
-            umma::mbar_wait(k_full, k_it & 1);
+            k_ring->wait(k_it);
             float tot[kMyBlocks][2];
 #pragma unroll
             for (int i = 0; i < kMyBlocks; ++i) tot[i][0] = tot[i][1] = 0.f;
             for (int g = 0; g < G; ++g, ++q_it) {
-                const int stage = q_it % L::kStages;
                 float* cb = s_cb + (q_it & 1) * CS;
+                const int stage = q_ring->wait(q_it);
                 const uint32_t qbase = umma::smem_u32(s_stage + stage * L::kChunkBytes);
-                umma::mbar_wait(&q_full[stage], (q_it / L::kStages) & 1);
                 // ---- pass A: every valid query row's max and sum exp2 over all CS keys of the chunk ----
                 // Both passes keep their own epilogues rather than qk_tiles.cuh's (no key is masked here): built on
                 // those, this kernel measured about 1 % slower at cs = 256 (H100 80GB HBM3, 700 W).
@@ -253,12 +241,9 @@ nca_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                         tot[i][1] += a2 + a3;
                     }
                 }
-                __syncwarp();
-                if (lane == 0) umma::mbar_arrive(&q_empty[stage]);
+                q_ring->release(stage);
             }
-            // every MMA on the K chunk has completed: hand it back to the producer
-            __syncwarp();
-            if (lane == 0) umma::mbar_arrive(k_empty);
+            k_ring->release(0);  // every MMA on the K chunk has completed
             // the padded query rows of a last chunk: pad of them, each 1/CS on every key (exact: CS is a power of 2)
             const float pad_share = (float)max(0, (c + 1) * CS - S) / CS;
 #pragma unroll
@@ -372,13 +357,12 @@ static cudaError_t launch_nca_t(const Dims& d, const void* K, const void* V, con
     // q [B Hq, S, D] contiguous
     if ((e = make_tmap_rows(&mapQ, q, D, d.S, D, (uint64_t)d.B * d.Hq, (uint64_t)d.S * D, kSnTile)) != cudaSuccess)
         return e;
-    const int smem = L::kTotal + 1024;
-    auto k1 = nca_colsum_kernel<T, D, CS>;
-    static PerDeviceOnce smem_set;  // one per <T, D, CS> instantiation of this launcher
-    if ((e = ensure_dynamic_smem(k1, smem, smem_set)) != cudaSuccess) return e;
+    constexpr int smem = umma::smem_request(L::kTotal);
+    constexpr auto k1 = nca_colsum_kernel<T, D, CS>;
+    if ((e = ensure_dynamic_smem<k1>(smem)) != cudaSuccess) return e;
 
-    k1<<<grid, kSnThreads, smem, st>>>(mapK, mapQ, static_cast<const T*>(V), d.vs, d.H, G, d.S, d.R, n_chunks, sc,
-                                       ws.S_pad);
+    k1<<<grid, umma::kTmaCtaThreads, smem, st>>>(mapK, mapQ, static_cast<const T*>(V), d.vs, d.H, G, d.S, d.R, n_chunks,
+                                                 sc, ws.S_pad);
     if ((e = cudaPeekAtLastError()) != cudaSuccess) return e;
     nca_partials_kernel<<<dim3(ws.n_tiles, d.R), kTileThreads, 0, st>>>(d.S, ws.S_pad, sc);
     if ((e = cudaPeekAtLastError()) != cudaSuccess) return e;

@@ -70,13 +70,12 @@ struct ObsColSmem {
     static constexpr int kPanels = D / 64;
     static constexpr int kTileBytes = kPanels * kSnTile * 128;  // a K tile or a Q chunk
     static constexpr int kPanel = kSnTile * 128;                // bytes of one 64-column panel of either
-    static constexpr int kFit = (227 * 1024 - 1024 - kTileBytes - 256) / kTileBytes;
-    static constexpr int kStages = kFit >= 4 ? 4 : kFit;
+    static constexpr int kStages = umma::ring_stages(kTileBytes + 256, kTileBytes);
     static constexpr int kKOff = 0;
     static constexpr int kStageOff = kTileBytes;
     static constexpr int kBarOff = kStageOff + kStages * kTileBytes;
     static constexpr int kTotal = kBarOff + 256;
-    static_assert(kTotal + 1024 <= 227 * 1024, "shared memory budget");
+    static_assert(umma::smem_request(kTotal) <= umma::kSmemBudget, "shared memory budget");
 };
 
 // ---- pass 1: per-query-row softmax normalisers --------------------------------------------------------------------
@@ -85,7 +84,7 @@ struct ObsColSmem {
 // tile; a thread holds rows (16 w + l/4, +8) of a block and 32 of the 128 keys, keeps an online (max, sum exp2) per
 // row, and the four threads that share a row merge theirs at the end of the item.
 template <typename T, int D, int NQP>
-__global__ void __launch_bounds__(kSnThreads, 1)
+__global__ void __launch_bounds__(umma::kTmaCtaThreads, 1)
 obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapQ, int H, int G,
                  int S, int n_q, int qpos, int R, int n_blocks, float c, ObsScratch sc) {
     using L = SnSmem<D, NQP>;
@@ -93,10 +92,8 @@ obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
     unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_q = smem + L::kQOff;
     unsigned char* s_stage = smem + L::kStageOff;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
-    uint64_t* k_full = bars;       // [kStages <= 4]
-    uint64_t* k_empty = bars + 4;  // [kStages]
-    uint64_t* q_full = bars + 8;
+    auto* k_ring = reinterpret_cast<umma::TmaRing<L::kStages>*>(smem + L::kBarOff);
+    uint64_t* q_full = reinterpret_cast<uint64_t*>(k_ring + 1);
 
     constexpr int kMyBlocks = NQP / 128;  // 64-row blocks of Q per consumer warpgroup
     const int NQ = G * qpos;
@@ -106,10 +103,7 @@ obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
     if (tid == 0) {
         umma::prefetch_tmap(&mapK);
         umma::prefetch_tmap(&mapQ);
-        for (int i = 0; i < L::kStages; ++i) {
-            umma::mbar_init(&k_full[i], 1);
-            umma::mbar_init(&k_empty[i], 8);  // lane 0 of each consumer warp, after its MMAs completed
-        }
+        k_ring->init(umma::kTmaConsumerWarps);
         umma::mbar_init(q_full, 1);
         umma::mbar_fence_init();
     }
@@ -133,12 +127,10 @@ obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                         umma::tma_load_3d(s_q + kp * L::kQPanel + g * qpos * 128, &mapQ, q_full, kp * 64, p0,
                                           (b * H + j) * G + g);
                 for (int t = 0; t < n_tiles; ++t, ++k_it) {
-                    const int stage = k_it % L::kStages;
-                    umma::mbar_wait(&k_empty[stage], ((k_it / L::kStages) & 1) ^ 1);
-                    umma::mbar_arrive_expect_tx(&k_full[stage], L::kStageBytes);
+                    const int stage = k_ring->acquire(k_it, L::kStageBytes);
                     for (int kp = 0; kp < L::kPanels; ++kp)
                         umma::tma_load_4d(s_stage + stage * L::kStageBytes + kp * (kSnTile * 128), &mapK,
-                                          &k_full[stage], kp * 64, t * kSnTile, j, b);
+                                          k_ring->full(stage), kp * 64, t * kSnTile, j, b);
                 }
             }
         } else {
@@ -153,8 +145,7 @@ obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                 }
             umma::mbar_wait(q_full, q_it & 1);
             for (int t = 0; t < n_tiles; ++t, ++k_it) {
-                const int stage = k_it % L::kStages;
-                umma::mbar_wait(&k_full[stage], (k_it / L::kStages) & 1);
+                const int stage = k_ring->wait(k_it);
                 const uint32_t kb = umma::smem_u32(s_stage + stage * L::kStageBytes);
                 const int key0 = t * kSnTile + 2 * qd;
                 const bool interior = (t + 1) * kSnTile <= off + p0 + 1;  // every key visible to every row
@@ -171,8 +162,7 @@ obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
                         online_row_update(acc, hh, c, interior, key0, limit, S, run_m[i][hh], run_z[i][hh]);
                     }
                 }
-                __syncwarp();
-                if (lane == 0) umma::mbar_arrive(&k_empty[stage]);
+                k_ring->release(stage);
             }
             ++q_it;
 #pragma unroll
@@ -197,7 +187,7 @@ obs_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant
 // chunks of an item come in (head, chunk) order, each thread adds them in that order into one fp32 sum per key, and
 // the four threads that share a key add theirs at the end of the item (xor 1, then xor 2).
 template <typename T, int D>
-__global__ void __launch_bounds__(kSnThreads, 1)
+__global__ void __launch_bounds__(umma::kTmaCtaThreads, 1)
 obs_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapQ, int H, int G,
                   int S, int n_q, int R, int n_ktiles, float c, ObsScratch sc, int S_pad) {
     using L = ObsColSmem<D>;
@@ -205,23 +195,16 @@ obs_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
     unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_k = smem + L::kKOff;
     unsigned char* s_stage = smem + L::kStageOff;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
-    uint64_t* q_full = bars;       // [kStages <= 4]
-    uint64_t* q_empty = bars + 4;  // [kStages]
-    uint64_t* k_full = bars + 8;
-    uint64_t* k_empty = bars + 9;
+    auto* q_ring = reinterpret_cast<umma::TmaRing<L::kStages>*>(smem + L::kBarOff);
+    auto* k_ring = reinterpret_cast<umma::TmaRing<1>*>(q_ring + 1);  // the resident K tile
 
     const int off = S - n_q;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = tid >> 7;
     if (tid == 0) {
         umma::prefetch_tmap(&mapK);
         umma::prefetch_tmap(&mapQ);
-        for (int i = 0; i < L::kStages; ++i) {
-            umma::mbar_init(&q_full[i], 1);
-            umma::mbar_init(&q_empty[i], 8);  // lane 0 of each consumer warp, after its MMAs on the chunk completed
-        }
-        umma::mbar_init(k_full, 1);
-        umma::mbar_init(k_empty, 8);
+        q_ring->init(umma::kTmaConsumerWarps);
+        k_ring->init(umma::kTmaConsumerWarps);
         umma::mbar_fence_init();
     }
     __syncthreads();
@@ -235,18 +218,16 @@ obs_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                 const int kt = u / R, row = u % R;
                 const int b = row / H, j = row % H;
                 const int i_min = obs_colsum_imin(S, n_q, kt), n_chunks = obs_colsum_chunks(S, n_q, kt);
-                umma::mbar_wait(k_empty, (k_it & 1) ^ 1);
-                umma::mbar_arrive_expect_tx(k_full, L::kTileBytes);
+                k_ring->acquire(k_it, L::kTileBytes);
                 for (int kp = 0; kp < L::kPanels; ++kp)
-                    umma::tma_load_4d(s_k + kp * L::kPanel, &mapK, k_full, kp * 64, kt * kSnTile, j, b);
+                    umma::tma_load_4d(s_k + kp * L::kPanel, &mapK, k_ring->full(0), kp * 64, kt * kSnTile, j, b);
                 for (int g = 0; g < G; ++g)
                     for (int ch = 0; ch < n_chunks; ++ch, ++q_it) {
-                        const int stage = q_it % L::kStages;
-                        umma::mbar_wait(&q_empty[stage], ((q_it / L::kStages) & 1) ^ 1);
-                        umma::mbar_arrive_expect_tx(&q_full[stage], L::kTileBytes);
+                        const int stage = q_ring->acquire(q_it, L::kTileBytes);
                         for (int kp = 0; kp < L::kPanels; ++kp)
-                            umma::tma_load_3d(s_stage + stage * L::kTileBytes + kp * L::kPanel, &mapQ, &q_full[stage],
-                                              kp * 64, i_min + ch * kSnTile, (b * H + j) * G + g);
+                            umma::tma_load_3d(s_stage + stage * L::kTileBytes + kp * L::kPanel, &mapQ,
+                                              q_ring->full(stage), kp * 64, i_min + ch * kSnTile,
+                                              (b * H + j) * G + g);
                     }
             }
         }
@@ -260,14 +241,13 @@ obs_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
             const int i_min = obs_colsum_imin(S, n_q, kt), n_chunks = obs_colsum_chunks(S, n_q, kt);
             const int key = kt * kSnTile + cw * 64 + w4 * 16 + (lane >> 2);  // and key + 8
             const uint32_t ka = umma::smem_u32(s_k) + cw * 64 * 128;
-            umma::mbar_wait(k_full, k_it & 1);
+            k_ring->wait(k_it);
             float tot0 = 0.f, tot1 = 0.f;
             for (int g = 0; g < G; ++g) {
                 const float* cb_h = sc.cb + (size_t)((b * H + j) * G + g) * n_q;
                 for (int ch = 0; ch < n_chunks; ++ch, ++q_it) {
-                    const int stage = q_it % L::kStages;
                     const int i0 = i_min + ch * kSnTile;
-                    umma::mbar_wait(&q_full[stage], (q_it / L::kStages) & 1);
+                    const int stage = q_ring->wait(q_it);
                     float acc[64];
                     const uint32_t qa = umma::smem_u32(s_stage + stage * L::kTileBytes);
                     umma::wgmma_fence();
@@ -288,8 +268,7 @@ obs_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                         cby[jj] = i + 1 < n_q ? __ldg(cb_h + i + 1) : -INFINITY;
                     }
                     umma::wgmma_wait_all();
-                    __syncwarp();
-                    if (lane == 0) umma::mbar_arrive(&q_empty[stage]);
+                    q_ring->release(stage);
                     // key s is visible to row i iff s <= off + i, i.e. iff (s - off - i0) <= column; only the first
                     // chunk of a head reaches below the diagonal
                     const int dk0 = ch == 0 ? key - off - i0 : -(1 << 30), dk1 = dk0 + 8;
@@ -310,9 +289,7 @@ obs_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                     tot1 += a2 + a3;
                 }
             }
-            // every MMA on the K tile has completed: hand it back to the producer
-            __syncwarp();
-            if (lane == 0) umma::mbar_arrive(k_empty);
+            k_ring->release(0);  // every MMA on the K tile has completed
             quad_sum(tot0, tot1);
             if (qd == 0 && key < S) sc.colsum[(size_t)row * S_pad + key] = tot0;
             if (qd == 0 && key + 8 < S) sc.colsum[(size_t)row * S_pad + key + 8] = tot1;
@@ -360,16 +337,15 @@ static cudaError_t launch_obs_t(const Dims& d, const void* K, const void* q, int
     const uint64_t n_heads = (uint64_t)d.B * d.Hq, head_stride = (uint64_t)n_q * D;
     if ((e = make_tmap_rows(&mapQ1, q, D, n_q, D, n_heads, head_stride, qpos)) != cudaSuccess) return e;
     if ((e = make_tmap_rows(&mapQ2, q, D, n_q, D, n_heads, head_stride, kSnTile)) != cudaSuccess) return e;
-    const int smem1 = L1::kTotal + 1024, smem2 = L2::kTotal + 1024;
-    auto k1 = obs_stats_kernel<T, D, NQP>;
-    auto k2 = obs_colsum_kernel<T, D>;
-    static PerDeviceOnce smem_set1, smem_set2;  // one pair per <T, D, NQP> instantiation of this launcher
-    if ((e = ensure_dynamic_smem(k1, smem1, smem_set1)) != cudaSuccess) return e;
-    if ((e = ensure_dynamic_smem(k2, smem2, smem_set2)) != cudaSuccess) return e;
+    constexpr int smem1 = umma::smem_request(L1::kTotal), smem2 = umma::smem_request(L2::kTotal);
+    constexpr auto k1 = obs_stats_kernel<T, D, NQP>;
+    constexpr auto k2 = obs_colsum_kernel<T, D>;
+    if ((e = ensure_dynamic_smem<k1>(smem1)) != cudaSuccess) return e;
+    if ((e = ensure_dynamic_smem<k2>(smem2)) != cudaSuccess) return e;
 
-    k1<<<grid1, kSnThreads, smem1, st>>>(mapK, mapQ1, d.H, G, d.S, n_q, qpos, d.R, n_blocks, c, sc);
+    k1<<<grid1, umma::kTmaCtaThreads, smem1, st>>>(mapK, mapQ1, d.H, G, d.S, n_q, qpos, d.R, n_blocks, c, sc);
     if ((e = cudaPeekAtLastError()) != cudaSuccess) return e;
-    k2<<<grid2, kSnThreads, smem2, st>>>(mapK, mapQ2, d.H, G, d.S, n_q, d.R, n_ktiles, c, sc, ws.S_pad);
+    k2<<<grid2, umma::kTmaCtaThreads, smem2, st>>>(mapK, mapQ2, d.H, G, d.S, n_q, d.R, n_ktiles, c, sc, ws.S_pad);
     if ((e = cudaPeekAtLastError()) != cudaSuccess) return e;
     obs_finalize_kernel<T><<<dim3(ws.n_tiles, d.R), kTileThreads, 0, st>>>(d.S, G, sc, ws,
                                                                             static_cast<uint16_t*>(scores_out));

@@ -10,7 +10,6 @@
 namespace kvp {
 
 constexpr int kSnTile = 128;
-constexpr int kSnThreads = 384;  // warpgroup 0: TMA producer (one thread); warpgroups 1, 2: wgmma + epilogue
 constexpr float kLog2e = 1.4426950408889634f;
 
 __device__ __forceinline__ float fast_exp2(float x) {  // MUFU.EX2, 2 ulp; exp2(-inf) = 0
@@ -28,15 +27,14 @@ struct SnSmem {
     static constexpr int kQBytes = kPanels * kQPanel;
     static constexpr int kStageBytes = kPanels * kSnTile * 128;
     static constexpr int kCbBytes = NQP * 4;              // pass 2: per query row -(max + log2 sum) in log2 units
-    static constexpr int kFit = (227 * 1024 - 1024 - kQBytes - kCbBytes - 256) / kStageBytes;
-    static constexpr int kStages = kFit >= 4 ? 4 : kFit;
+    static constexpr int kStages = umma::ring_stages(kQBytes + kCbBytes + 256, kStageBytes);
     static_assert(kStages >= 2, "K ring needs two stages");
     static constexpr int kQOff = 0;
     static constexpr int kStageOff = kQBytes;
     static constexpr int kCbOff = kStageOff + kStages * kStageBytes;
     static constexpr int kBarOff = kCbOff + kCbBytes;
     static constexpr int kTotal = kBarOff + 256;
-    static_assert(kTotal + 1024 <= 227 * 1024, "shared memory budget");
+    static_assert(umma::smem_request(kTotal) <= umma::kSmemBudget, "shared memory budget");
 };
 
 // acc[64] (+)= A[64 rows x D] * B[128 rows x D]^T, both K-major SW128 panels (`a_panel` / `b_panel` bytes apart)

@@ -457,9 +457,9 @@ select_compact_kernel(const char* __restrict__ K, const char* __restrict__ V, St
     }
 }
 
-template <typename Kern>
-static int persistent_grid(Kern kernel, int threads, int n_items, PerDeviceInt& occupancy) {
-    const int grid = device_sm_count() * cached_ctas_per_sm(kernel, threads, occupancy);
+template <auto kKern>
+static int persistent_grid(int threads, int n_items) {
+    const int grid = device_sm_count() * cached_ctas_per_sm<kKern>(threads);
     return n_items < grid ? n_items : grid;
 }
 
@@ -469,9 +469,8 @@ static cudaError_t launch_select_compact_t(const Dims& d, const void* K, const v
                                            const float* inv_freq, cudaStream_t st) {
     const int n_groups = (ws.n_tiles + kGroupTiles - 1) / kGroupTiles;
     const int n_items = d.R * n_groups + d.R * ws.n_tiles;
-    auto kern = select_compact_kernel<TR>;
-    static PerDeviceInt occupancy;  // one per <TR> instantiation of this launcher
-    const int grid = persistent_grid(kern, kTileThreads, n_items, occupancy);
+    constexpr auto kern = select_compact_kernel<TR>;
+    const int grid = persistent_grid<kern>(kTileThreads, n_items);
     return launch_pdl(kern, dim3(grid), dim3(kTileThreads), 0, st, static_cast<const char*>(K),
                       static_cast<const char*>(V), d.ks, d.vs, static_cast<char*>(K_out), static_cast<char*>(V_out),
                       idx_out, d.H, d.S, d.D, d.n_kept, ws, inv_freq);
@@ -643,9 +642,8 @@ static cudaError_t launch_knorm_fused_t(const Dims& d, const void* K, const void
     const long long total = fused_total_items(fq);
     if (total > 0x7FFFFFFFll) return cudaErrorNotSupported;
     with_lanes_per_row(d.D, [&](auto lpr) {
-        auto kern = knorm_fused_kernel<T, lpr>;
-        static PerDeviceInt occupancy;  // one per <T, LPR> instantiation of this lambda
-        const int grid = persistent_grid(kern, kTileThreads, (int)total, occupancy);
+        constexpr auto kern = knorm_fused_kernel<T, lpr>;
+        const int grid = persistent_grid<kern>(kTileThreads, (int)total);
         kern<<<grid, kTileThreads, 0, st>>>(static_cast<const T*>(K), static_cast<const T*>(V), d.ks, d.vs,
                                             static_cast<char*>(K_out), static_cast<char*>(V_out), idx_out,
                                             static_cast<uint16_t*>(scores_out), d.H, d.S, d.D, d.n_kept, ws, fq,

@@ -58,7 +58,7 @@ size_t snapkv_scratch_bytes(const Dims& d, int window) {
 // Producer of both passes (one thread): the resident Q block of this row, then the K tiles [t_begin, t_end).
 template <int D, int NQP>
 __device__ __forceinline__ void snap_produce(const CUtensorMap* mapK, const CUtensorMap* mapQ, unsigned char* s_q,
-                                             unsigned char* s_stage, uint64_t* k_full, uint64_t* k_empty,
+                                             unsigned char* s_stage, umma::TmaRing<SnSmem<D, NQP>::kStages>* k_ring,
                                              uint64_t* q_full, int q_row0, int b, int h, int t_begin, int t_end,
                                              uint32_t& k_it) {
     using L = SnSmem<D, NQP>;
@@ -69,12 +69,10 @@ __device__ __forceinline__ void snap_produce(const CUtensorMap* mapK, const CUte
         for (int r0 = 0; r0 < NQP; r0 += 256)
             umma::tma_load_3d(s_q + kp * L::kQPanel + r0 * 128, mapQ, q_full, kp * 64, q_row0 + r0, 0);
     for (int t = t_begin; t < t_end; ++t, ++k_it) {
-        const int stage = k_it % L::kStages;
-        umma::mbar_wait(&k_empty[stage], ((k_it / L::kStages) & 1) ^ 1);
-        umma::mbar_arrive_expect_tx(&k_full[stage], L::kStageBytes);
+        const int stage = k_ring->acquire(k_it, L::kStageBytes);
         for (int kp = 0; kp < L::kPanels; ++kp)
-            umma::tma_load_4d(s_stage + stage * L::kStageBytes + kp * (kSnTile * 128), mapK, &k_full[stage], kp * 64,
-                              t * kSnTile, h, b);
+            umma::tma_load_4d(s_stage + stage * L::kStageBytes + kp * (kSnTile * 128), mapK, k_ring->full(stage),
+                              kp * 64, t * kSnTile, h, b);
     }
 }
 
@@ -83,7 +81,7 @@ __device__ __forceinline__ void snap_produce(const CUtensorMap* mapK, const CUte
 // a thread holds rows (16 w + l/4, +8) of a block and 32 of the 128 keys, keeps an online (max, sum exp2) per row,
 // and the four threads that share a row merge theirs at the end of the row.
 template <typename T, int D, int NQP>
-__global__ void __launch_bounds__(kSnThreads, 1)
+__global__ void __launch_bounds__(umma::kTmaCtaThreads, 1)
 snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapQ, int H,
                   int G, int S, int window, int R, int n_tiles128, int ctas_per_row, int n_parts,
                   SnapScratch sc) {
@@ -92,10 +90,8 @@ snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
     unsigned char* smem = umma::smem_align_1024(smem_raw);
     unsigned char* s_q = smem + L::kQOff;
     unsigned char* s_stage = smem + L::kStageOff;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
-    uint64_t* k_full = bars;       // [kStages <= 4]
-    uint64_t* k_empty = bars + 4;  // [kStages]
-    uint64_t* q_full = bars + 8;
+    auto* k_ring = reinterpret_cast<umma::TmaRing<L::kStages>*>(smem + L::kBarOff);
+    uint64_t* q_full = reinterpret_cast<uint64_t*>(k_ring + 1);
 
     constexpr int kMyBlocks = NQP / 128;  // 64-row blocks of Q per consumer warpgroup
     const int NQ = G * window;
@@ -107,10 +103,7 @@ snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
     if (tid == 0) {
         umma::prefetch_tmap(&mapK);
         umma::prefetch_tmap(&mapQ);
-        for (int i = 0; i < L::kStages; ++i) {
-            umma::mbar_init(&k_full[i], 1);
-            umma::mbar_init(&k_empty[i], 8);  // lane 0 of each consumer warp, after its MMAs completed
-        }
+        k_ring->init(umma::kTmaConsumerWarps);
         umma::mbar_init(q_full, 1);
         umma::mbar_fence_init();
     }
@@ -129,8 +122,7 @@ snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
 
         if (wg == 0) {
             if (tid == 0)
-                snap_produce<D, NQP>(&mapK, &mapQ, s_q, s_stage, k_full, k_empty, q_full, q_row0, b, h, t_begin, t_end,
-                                     k_it);
+                snap_produce<D, NQP>(&mapK, &mapQ, s_q, s_stage, k_ring, q_full, q_row0, b, h, t_begin, t_end, k_it);
         } else {
             const int cw = wg - 1, w4 = warp & 3, qd = lane & 3;
             float run_m[kMyBlocks][2], run_z[kMyBlocks][2];
@@ -143,8 +135,7 @@ snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                 }
             umma::mbar_wait(q_full, q_it & 1);
             for (int t = t_begin; t < t_end; ++t, ++k_it) {
-                const int stage = k_it % L::kStages;
-                umma::mbar_wait(&k_full[stage], (k_it / L::kStages) & 1);
+                const int stage = k_ring->wait(k_it);
                 const uint32_t kb = umma::smem_u32(s_stage + stage * L::kStageBytes);
                 const int key0 = t * kSnTile + 2 * qd;
                 const bool interior = (t + 1) * kSnTile <= S - window;  // no masking, all keys valid
@@ -161,8 +152,7 @@ snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
                         online_row_update(acc, hh, c, interior, key0, limit, S, run_m[i][hh], run_z[i][hh]);
                     }
                 }
-                __syncwarp();
-                if (lane == 0) umma::mbar_arrive(&k_empty[stage]);
+                k_ring->release(stage);
             }
             ++q_it;
 #pragma unroll
@@ -185,7 +175,7 @@ snap_stats_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constan
 // Q; a thread holds keys (16 w + l/4, +8) and sums exp2(c y - m_r - log2 Z_r) = p[r, key] over its columns. The four
 // threads that share a key add their sums; every key of a tile belongs to exactly one thread.
 template <typename T, int D, int NQP>
-__global__ void __launch_bounds__(kSnThreads, 1)
+__global__ void __launch_bounds__(umma::kTmaCtaThreads, 1)
 snap_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_constant__ CUtensorMap mapQ, int H,
                    int G, int S, int window, int R, int n_tiles128, int ctas_per_row, int n_parts,
                    SnapScratch sc, int S_pad) {
@@ -195,10 +185,8 @@ snap_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_consta
     unsigned char* s_q = smem + L::kQOff;
     unsigned char* s_stage = smem + L::kStageOff;
     float* s_cb = reinterpret_cast<float*>(smem + L::kCbOff);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::kBarOff);
-    uint64_t* k_full = bars;
-    uint64_t* k_empty = bars + 4;
-    uint64_t* q_full = bars + 8;
+    auto* k_ring = reinterpret_cast<umma::TmaRing<L::kStages>*>(smem + L::kBarOff);
+    uint64_t* q_full = reinterpret_cast<uint64_t*>(k_ring + 1);
 
     constexpr int kNChunks = NQP / 128;  // 128-column MMAs per tile
     const int NQ = G * window;
@@ -210,10 +198,7 @@ snap_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_consta
     if (tid == 0) {
         umma::prefetch_tmap(&mapK);
         umma::prefetch_tmap(&mapQ);
-        for (int i = 0; i < L::kStages; ++i) {
-            umma::mbar_init(&k_full[i], 1);
-            umma::mbar_init(&k_empty[i], 8);
-        }
+        k_ring->init(umma::kTmaConsumerWarps);
         umma::mbar_init(q_full, 1);
         umma::mbar_fence_init();
     }
@@ -231,7 +216,7 @@ snap_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_consta
         const int b = row / H, h = row % H;
         const int q_row0 = (b * (H * G) + h * G) * window;
         __syncthreads();
-        for (int n = tid; n < NQP; n += kSnThreads) {
+        for (int n = tid; n < NQP; n += umma::kTmaCtaThreads) {
             // exact normaliser of query row n from the per-CTA partials of pass 1:
             // p[n, j] = exp2(c*y - m) / Z = exp2(c*y + cb),  cb = -m - log2 Z; padding rows (n >= NQ) add exactly 0
             float cb = -INFINITY;
@@ -252,14 +237,12 @@ snap_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_consta
 
         if (wg == 0) {
             if (tid == 0)
-                snap_produce<D, NQP>(&mapK, &mapQ, s_q, s_stage, k_full, k_empty, q_full, q_row0, b, h, t_begin, t_end,
-                                     k_it);
+                snap_produce<D, NQP>(&mapK, &mapQ, s_q, s_stage, k_ring, q_full, q_row0, b, h, t_begin, t_end, k_it);
         } else {
             const int cw = wg - 1, w4 = warp & 3, qd = lane & 3;
             umma::mbar_wait(q_full, q_it & 1);
             for (int t = t_begin; t < t_end; ++t, ++k_it) {
-                const int stage = k_it % L::kStages;
-                umma::mbar_wait(&k_full[stage], (k_it / L::kStages) & 1);
+                const int stage = k_ring->wait(k_it);
                 const uint32_t kb = umma::smem_u32(s_stage + stage * L::kStageBytes) + cw * 64 * 128;
                 float tot0 = 0.f, tot1 = 0.f;
 #pragma unroll 1
@@ -269,8 +252,7 @@ snap_colsum_kernel(const __grid_constant__ CUtensorMap mapK, const __grid_consta
                     snap_mma<T, D>(acc, kb, kSnTile * 128, umma::smem_u32(s_q + nc * 128 * 128), L::kQPanel);
                     colsum_tile(acc, s_cb + nc * 128, qd, c, tot0, tot1);
                 }
-                __syncwarp();
-                if (lane == 0) umma::mbar_arrive(&k_empty[stage]);
+                k_ring->release(stage);
                 quad_sum(tot0, tot1);
                 const int pos = t * kSnTile + cw * 64 + w4 * 16 + (lane >> 2);
                 if (qd == 0 && pos < S - window) sc.colsum[(size_t)row * S_pad + pos] = tot0;
@@ -336,19 +318,17 @@ static cudaError_t launch_snap_t(const Dims& d, int dtype, const void* K, const 
     if ((e = make_tmap_cache(&mapK, K, d, d.ks, kSnTile)) != cudaSuccess) return e;
     const uint64_t rows = (uint64_t)d.B * d.Hq * window;
     if ((e = make_tmap_rows(&mapQ, q_window, D, rows, D, 1, rows * D, NQP < 256 ? NQP : 256)) != cudaSuccess) return e;
-    const int smem = L::kTotal + 1024;
-    auto k1 = snap_stats_kernel<T, D, NQP>;
-    auto k2 = snap_colsum_kernel<T, D, NQP>;
-    static PerDeviceOnce smem_set1, smem_set2;  // one pair per <T, D, NQP> instantiation of this launcher
-    if ((e = ensure_dynamic_smem(k1, smem, smem_set1)) != cudaSuccess) return e;
-    e = ensure_dynamic_smem(k2, smem, smem_set2);
-    if (e != cudaSuccess) return e;
+    constexpr int smem = umma::smem_request(L::kTotal);
+    constexpr auto k1 = snap_stats_kernel<T, D, NQP>;
+    constexpr auto k2 = snap_colsum_kernel<T, D, NQP>;
+    if ((e = ensure_dynamic_smem<k1>(smem)) != cudaSuccess) return e;
+    if ((e = ensure_dynamic_smem<k2>(smem)) != cudaSuccess) return e;
 
-    k1<<<grid, kSnThreads, smem, st>>>(mapK, mapQ, d.H, G, d.S, window, d.R, n_tiles128, ctas_per_row,
-                                       n_parts, sc);
+    k1<<<grid, umma::kTmaCtaThreads, smem, st>>>(mapK, mapQ, d.H, G, d.S, window, d.R, n_tiles128, ctas_per_row,
+                                                 n_parts, sc);
     if ((e = cudaPeekAtLastError()) != cudaSuccess) return e;
-    k2<<<grid, kSnThreads, smem, st>>>(mapK, mapQ, d.H, G, d.S, window, d.R, n_tiles128, ctas_per_row, n_parts,
-                                       sc, ws.S_pad);
+    k2<<<grid, umma::kTmaCtaThreads, smem, st>>>(mapK, mapQ, d.H, G, d.S, window, d.R, n_tiles128, ctas_per_row,
+                                                 n_parts, sc, ws.S_pad);
     if ((e = cudaPeekAtLastError()) != cudaSuccess) return e;
     dim3 grid3((ws.n_tiles + kFinalizeTiles - 1) / kFinalizeTiles, d.R);
     snap_finalize_kernel<T><<<grid3, kTileThreads, 0, st>>>(d.S, window, kernel_size, 1.0f / (float)NQ, sc, ws,

@@ -14,9 +14,19 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return (uint32_t)__cvta_generic_to_shared(p);
 }
 // Dynamic shared memory is only guaranteed 16-B aligned: round up to the 1024 B a SWIZZLE_128B panel needs (the
-// launchers request 1024 B more than the layout uses).
+// launchers request smem_request(layout) bytes, kSmemAlignSlack more than the layout uses).
 __device__ __forceinline__ unsigned char* smem_align_1024(unsigned char* smem_raw) {
     return reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+}
+constexpr int kSmemBudget = 227 * 1024;  // dynamic shared memory one CTA may request on sm_90
+constexpr int kSmemAlignSlack = 1024;    // what the round-up to 1024 B may skip
+// The dynamic shared memory a kernel with a shared-memory layout of `layout_bytes` requests.
+constexpr int smem_request(int layout_bytes) { return layout_bytes + kSmemAlignSlack; }
+// Depth of a TMA ring of `stage_bytes` stages next to `fixed_bytes` of everything else: as deep as the budget allows,
+// at most 4.
+constexpr int ring_stages(int fixed_bytes, int stage_bytes) {
+    const int fit = (kSmemBudget - kSmemAlignSlack - fixed_bytes) / stage_bytes;
+    return fit < 4 ? fit : 4;
 }
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -49,6 +59,50 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         if (spins > (1u << 18)) __trap();  // > 5 s without progress
     }
 }
+
+// ---- the producer / consumer pipeline of the TMA-fed kernels ------------------------------------------------------
+// Their CTA: warpgroup 0 produces (one thread issues the TMA loads; its other warps may do side work), warpgroups 1
+// and 2 consume (wgmma + epilogue). A stage is handed back by lane 0 of each consumer warp.
+constexpr int kTmaCtaThreads = 384;
+constexpr int kTmaConsumerWarps = (kTmaCtaThreads - 128) / 32;
+
+// A ring of N stages in shared memory, each with a `full` barrier (one producer arrival plus the TMA bytes) and an
+// `empty` barrier (the consumers' arrivals). Iteration `it` of a role uses stage it % N in phase (it / N) & 1; the
+// producer and every consumer thread count their own iterations. A resident operand that the consumers hand back is
+// a TmaRing<1>.
+template <int N>
+struct TmaRing {
+    uint64_t full_bar[N];
+    uint64_t empty_bar[N];
+
+    // thread 0, before mbar_fence_init
+    __device__ __forceinline__ void init(uint32_t consumer_arrivals) {
+        for (int i = 0; i < N; ++i) {
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], consumer_arrivals);
+        }
+    }
+    // producer: waits until stage it % N is free, arms its full barrier for `bytes` and returns the stage
+    __device__ __forceinline__ int acquire(uint32_t it, uint32_t bytes) {
+        const int stage = it % N;
+        mbar_wait(&empty_bar[stage], ((it / N) & 1) ^ 1);
+        mbar_arrive_expect_tx(&full_bar[stage], bytes);
+        return stage;
+    }
+    // the barrier the stage's TMA loads complete on
+    __device__ __forceinline__ uint64_t* full(int stage) { return &full_bar[stage]; }
+    // consumer: waits until stage it % N is loaded and returns it
+    __device__ __forceinline__ int wait(uint32_t it) {
+        const int stage = it % N;
+        mbar_wait(&full_bar[stage], (it / N) & 1);
+        return stage;
+    }
+    // consumer warp, once none of its threads reads the stage any more
+    __device__ __forceinline__ void release(int stage) {
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(&empty_bar[stage]);
+    }
+};
 
 // ---- TMA tensor-map loads (tile mode, 128B swizzle) ---------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
