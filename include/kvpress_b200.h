@@ -19,6 +19,7 @@
  *     kvp_lagkv_*              <- kvpress/presses/lagkv_press.py (lag-relative K / V statistics, from K and V only)
  *     kvp_cur_*                <- kvpress/presses/cur_press.py (approximate K / V leverage scores, from K and V only)
  *     kvp_merging_*            <- kvpress/presses/merging_press.py (evicted values folded into their nearest kept row)
+ *     kvp_think_prune          <- kvpress/presses/think_press.py (key channels zeroed in place; no positions removed)
  *     kvp_scores_compress      <- scorer_press.py:93-100 for an arbitrary score tensor
  *                                 (what wrapper presses / user ScorerPress subclasses need)
  *
@@ -83,7 +84,8 @@ typedef enum kvp_scorer {
     /* 10 and 12 are not assigned: kvp_launches_per_compress answers KVP_ERR_BAD_ARGUMENT for them, as for any unknown
      * id */
     KVP_SCORER_CUR = 11,
-    KVP_SCORER_MERGING = 13 /* kvp_merging_*: the selection of the caller's scores, then the merge */
+    KVP_SCORER_MERGING = 13, /* kvp_merging_*: the selection of the caller's scores, then the merge */
+    KVP_SCORER_THINK = 14    /* kvp_think_prune: key channels, not positions */
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -360,6 +362,44 @@ int kvp_merging_compress(const kvp_problem* p, const void* scores, const int64_t
 int kvp_merging_merge(const kvp_problem* p, const void* K, const void* V, const int32_t* kept_idx,
                       float similarity_threshold, double merge_fraction, void* V_out, int32_t* target_out,
                       float* sim_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+
+/* ---- ThinKPress (kvpress/presses/think_press.py, https://arxiv.org/abs/2407.21018) -----------------------------------
+ * Zeroes the key CHANNELS that matter least to the last window queries, in place; no position is removed. Per row
+ * (b, kv head j), with G = Hq / Hkv, w = window and S positions:
+ *   qn(c)    = 1/(G w) sum_{g<G} sum_{i<w} q_window[b, jG+g, i, c]^2    (the query heads jG ... jG+G-1 of kv head j)
+ *   kn(c)    = 1/S sum_{s<S} K[b, j, s, c]^2
+ *   score(c) = qn(c) kn(c), an fp32 value
+ * The D - n_pruned largest scores are kept: at equal scores the lower channel is kept, and NaN ranks above every number
+ * (torch.topk), NaNs among themselves by channel. Every element of a pruned channel, at every position of the view, is
+ * set to +0.0 (bit pattern 0); every other element of K is left bit for bit. V is neither read nor written.
+ * Evaluation order: the squares of the 16-bit inputs are exact. kn: per block of 256 positions (fixed by S alone) fp32
+ * sums, each element passing through at most 68 fp32 additions; the blocks summed in ascending order in fp64, then / S.
+ * qn: fp64 sums in a fixed order, / (G w). score = (qn kn) evaluated in fp64, rounded once to fp32. Against the same
+ * definition in float64 (fp32 rounding of the exact product included), for S < 2^31 and G w < 2^31:
+ *   |score - score64| <= 2^-16 |score64|  (+ 2^-149 per position for bf16 keys below 2^-63 in magnitude)
+ * NaN / inf: a NaN key or query element makes its channel's score NaN; an inf key (or query) makes it inf, or NaN when
+ * the other factor is 0 (inf * 0). Only bf16 keys can leave the fp32 range: an element of magnitude 2^64 or more, or a
+ * channel's 256-position block sum beyond 3.4e38, makes kn inf where the float64 definition is finite; a product qn kn
+ * beyond the fp32 range is inf in the definition too. The scores, the pruned set and the zeroed K of a row are bitwise
+ * independent of the SM count, of the batch the row sits in and of the strides.
+ * Arguments:
+ *   K          [B, Hkv, S, D] in place, through p->k_stride; any strided view the problem validates. Nothing outside
+ *              the view is written. p->v_stride is ignored (K's strides are validated in its place); p->n_kept is
+ *              unused (callers pass S) but validated as usual.
+ *   q_window   RoPE'd queries [B, Hq, window, D], contiguous, in K's dtype, 16-byte aligned.
+ *   pruned_out nullable, int32 [B, Hkv, n_pruned], the pruned channels ascending.
+ *   channel_scores_out nullable, float32 [B, Hkv, D], the scores.
+ * Every head_dim the problem validates, every G and window >= 1.
+ * Check order (the first failure is returned): p null -> validate the problem -> window >= 1 and 0 <= n_pruned <= D, else
+ * KVP_ERR_BAD_ARGUMENT -> n_pruned == 0 returns KVP_OK and enqueues nothing (the outputs are not written) -> K, q_window
+ * null -> K, q_window 16-byte and pruned_out, channel_scores_out 4-byte alignment -> workspace null -> its 16-byte
+ * alignment -> its size. kvp_workspace_bytes(KVP_SCORER_THINK) is 4 R + 32 R + 4 R ceil(S / 256) D bytes, each region
+ * rounded up to 256 (R = B Hkv): row tickets, the pruned-channel bitmask and the per-block partial sums. A call takes 3
+ * launches (memset of the tickets, reduce + select, zero). Memory beyond the workspace: none.
+ * The return type is kvp_status, an int-sized enum with the values of every other entry point's int. */
+kvp_status kvp_think_prune(const kvp_problem* p, void* K, const void* q_window, int32_t window, int32_t n_pruned,
+                           int32_t* pruned_out, float* channel_scores_out, void* workspace, size_t workspace_bytes,
+                           kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

@@ -30,6 +30,7 @@ from kvpress_b200.presses.random_press import RandomPress
 from kvpress_b200.presses.scorer_press import ScorerPress
 from kvpress_b200.presses.snapkv_press import SnapKVPress
 from kvpress_b200.presses.streaming_llm_press import StreamingLLMPress
+from kvpress_b200.presses.think_press import ThinKPress
 from kvpress_b200.presses.tova_press import TOVAPress
 
 # Like the reference (kvpress/__init__.py:8,52): every attention function of transformers is wrapped at import,
@@ -56,6 +57,7 @@ __all__ = [
     "LagKVPress",
     "CURPress",
     "MergingPress",
+    "ThinKPress",
     "BlockPress",
     "ChunkPress",
     "ChunkKVPress",

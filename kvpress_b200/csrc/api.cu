@@ -76,6 +76,14 @@ static int largest_window(const Dims& d, int scorer) {
 static size_t layout(const Dims& d, int scorer, int window, void* base, Workspace* ws, size_t* zeroed) {
     Carve c(base);
     ws->R = d.R;
+    if (scorer == KVP_SCORER_THINK) {  // no selection of positions: the channel statistics alone (think.cu)
+        *ws = Workspace{};
+        ws->R = d.R;
+        ws->scorer_bytes = think_scratch_bytes(d);
+        ws->scorer = c.take<char>(ws->scorer_bytes);
+        *zeroed = 0;
+        return c.bytes;
+    }
     ws->n_tiles = (d.S + kTile - 1) / kTile;
     ws->S_pad = ws->n_tiles * kTile;
     ws->hist_hi = c.take<uint32_t>((size_t)d.R * 256);
@@ -240,6 +248,7 @@ int kvp_workspace_check(const kvp_problem* p, int scorer, const void* workspace,
     int rc = validate(p, &c.d, false);
     if (rc || (rc = c.carve(scorer, largest_window(c.d, scorer), const_cast<void*>(workspace), workspace_bytes)))
         return rc;
+    if (scorer == KVP_SCORER_THINK) return KVP_OK;  // its kernels have no bounded waits
     uint32_t flag = 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     cudaError_t e = cudaMemcpyAsync(&flag, c.ws.counters + kCounterErrSlot(c.d.R), sizeof(flag),
@@ -279,6 +288,7 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
             *launches_out = validate(p, &d, false) == KVP_OK && p->n_kept == p->S ? 6 : 7;
             break;
         }
+        case KVP_SCORER_THINK: *launches_out = 3; break;  // memset, reduce + select, zero
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -718,6 +728,27 @@ int kvp_merging_merge(const kvp_problem* p, const void* K, const void* V, const 
     };
     // no selection: nothing to clear
     return run(Kind::score, p, KVP_SCORER_MERGING, 0, {}, operands, merge, workspace, workspace_bytes, stream, false);
+}
+
+// ---- ThinK ---------------------------------------------------------------------------------------------------------
+kvp_status kvp_think_prune(const kvp_problem* p, void* K, const void* q_window, int32_t window, int32_t n_pruned,
+                           int32_t* pruned_out, float* channel_scores_out, void* workspace, size_t workspace_bytes,
+                           kvp_stream_t stream) {
+    if (p == nullptr) return KVP_ERR_NULL_POINTER;
+    kvp_problem pk = *p;  // V is not read: the problem is validated with K's strides in place of p->v_stride
+    for (int i = 0; i < 3; ++i) pk.v_stride[i] = pk.k_stride[i];
+    Call c;
+    int rc = validate(&pk, &c.d);
+    if (rc) return static_cast<kvp_status>(rc);
+    if (window < 1 || n_pruned < 0 || n_pruned > c.d.D) return KVP_ERR_BAD_ARGUMENT;
+    if (n_pruned == 0) return KVP_OK;
+    if (!K || !q_window) return KVP_ERR_NULL_POINTER;
+    if (!aligned16(K) || !aligned16(q_window) || !aligned4(pruned_out) || !aligned4(channel_scores_out))
+        return KVP_ERR_BAD_STRIDE;
+    c.st = static_cast<cudaStream_t>(stream);
+    if ((rc = c.carve(KVP_SCORER_THINK, 0, workspace, workspace_bytes))) return static_cast<kvp_status>(rc);
+    return static_cast<kvp_status>(status(launch_think_prune(c.d, p->dtype, K, q_window, window, n_pruned, pruned_out,
+                                                             channel_scores_out, c.ws.scorer, c.st)));
 }
 
 }  // extern "C"

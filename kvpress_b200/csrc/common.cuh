@@ -51,7 +51,7 @@ struct Workspace {
                          // zero = row not scanned yet
     int R;
     void* scorer;        // scorer-specific scratch (SnapKV / ExpectedAttention / KeyDiff / CriticalKV /
-                         // ObservedAttention / NonCausalAttention / CUR / Merging; LagKV needs none)
+                         // ObservedAttention / NonCausalAttention / CUR / Merging / ThinK; LagKV needs none)
     size_t scorer_bytes;
     int S_pad;
     int n_tiles;
@@ -479,5 +479,9 @@ int32_t* merging_scratch_kept(const Dims& d, const Workspace& ws);
 cudaError_t launch_merging(const Dims& d, int dtype, const void* K, const void* V, const int32_t* kept, float threshold,
                            double merge_fraction, void* V_out, int32_t* target_out, float* sim_out, const Workspace& ws,
                            cudaStream_t st);
+size_t think_scratch_bytes(const Dims& d);
+// a memset of the row tickets, the reduce + select kernel and the zero kernel on `scratch` (think_scratch_bytes)
+cudaError_t launch_think_prune(const Dims& d, int dtype, void* K, const void* q, int window, int n_pruned,
+                               int32_t* pruned_out, float* scores_out, void* scratch, cudaStream_t st);
 
 }  // namespace kvp

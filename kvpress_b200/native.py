@@ -22,6 +22,7 @@ _LIB_PATH = Path(__file__).resolve().parent / _LIB_NAME
  SCORER_CRITICALKV, SCORER_OBSERVED_ATTENTION, SCORER_NON_CAUSAL_ATTENTION, SCORER_LAGKV) = range(10)
 SCORER_CUR = 11  # KVP_SCORER_CUR; id 10 is not assigned
 SCORER_MERGING = 13  # KVP_SCORER_MERGING; id 12 is not assigned
+SCORER_THINK = 14  # KVP_SCORER_THINK: kvp_think_prune
 LAG_MAX = 1024  # the largest lag_size the LagKV kernel scores (kLagMax in csrc/common.cuh)
 CUR_WINDOW_MAX = 1024  # the largest local_window_size the CUR kernel scores (kCurWindowMax in csrc/common.cuh)
 CUR_RANK_MAX = 32  # the most projection columns the CUR kernel scores (kCurRankMax)
@@ -96,6 +97,7 @@ SIGNATURES = {
     "kvp_merging_compress": (
         ctypes.c_int, [_PP, _P, _PI64, _P, _P, ctypes.c_float, ctypes.c_double, _P, _P, _P, _P, _P, _P, _SZ, _P]),
     "kvp_merging_merge": (ctypes.c_int, [_PP, _P, _P, _P, ctypes.c_float, ctypes.c_double, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_think_prune": (ctypes.c_int, [_PP, _P, _P, _I, _I, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -761,3 +763,36 @@ def merging_merge(keys, values, kept_idx: torch.Tensor, similarity_threshold: fl
     _enqueue("kvp_merging_merge", keys.device, make_problem(keys, values, n_kept), keys, values, kept_idx, thr, frac,
              v_out, target, sim, scorer=SCORER_MERGING)
     return v_out, target, sim
+
+
+# --------------------------------------------------------------------------------------------------
+# ThinK (key channels zeroed in place)
+# --------------------------------------------------------------------------------------------------
+def think_prune(keys: torch.Tensor, q_window: torch.Tensor, n_pruned: int, return_pruned: bool = False,
+                return_scores: bool = False):
+    """ThinKPress.compress (include/kvpress_b200.h, kvp_think_prune): the n_pruned key channels of every [B, Hkv] row
+    with the smallest qn * kn are set to +0 IN PLACE, qn the mean square of the channel over the window queries
+    q_window [B, Hq, w, D] of the kv head's query heads, kn its mean square over the cached positions (ties: the higher
+    channel is pruned; NaN is pruned last). Returns (keys, pruned, scores): the same keys tensor, and with return_pruned
+    the pruned channels ascending (int32 [B, Hkv, n_pruned]), with return_scores the fp32 channel scores [B, Hkv, D].
+    With n_pruned == 0 nothing is enqueued and both optional outputs are None."""
+    _require_cuda_kv(keys, keys)
+    if not _rows_ok(keys):
+        raise RuntimeError("think_prune writes the keys in place: they need 16-byte aligned, unit-stride rows with "
+                           "outer strides that are multiples of 8 elements")
+    B, H, S, D = keys.shape
+    if not 0 <= n_pruned <= D:
+        raise ValueError(f"n_pruned must be in [0, {D}], got {n_pruned}")
+    if q_window.dim() != 4 or q_window.shape[0] != B or q_window.shape[3] != D or q_window.shape[2] < 1 or \
+            q_window.shape[1] % H:
+        raise RuntimeError(f"q_window must be [B, Hq, w >= 1, {D}] with Hq a multiple of {H}, got {tuple(q_window.shape)}")
+    if q_window.dtype != keys.dtype or q_window.device != keys.device:
+        raise RuntimeError("q_window must share dtype and device with the keys")
+    if n_pruned == 0:
+        return keys, None, None
+    q_window = q_window.contiguous()
+    pruned = torch.empty((B, H, n_pruned), dtype=torch.int32, device=keys.device) if return_pruned else None
+    scores = torch.empty((B, H, D), dtype=torch.float32, device=keys.device) if return_scores else None
+    _enqueue("kvp_think_prune", keys.device, make_problem(keys, keys, S, q_window.shape[1]), keys, q_window,
+             q_window.shape[2], int(n_pruned), pruned, scores, scorer=SCORER_THINK)
+    return keys, pruned, scores
