@@ -81,11 +81,12 @@ typedef enum kvp_scorer {
     KVP_SCORER_OBSERVED_ATTENTION = 7,
     KVP_SCORER_NON_CAUSAL_ATTENTION = 8,
     KVP_SCORER_LAGKV = 9,
-    /* 10 and 12 are not assigned: kvp_launches_per_compress answers KVP_ERR_BAD_ARGUMENT for them, as for any unknown
-     * id */
+    /* 10, 12 and 15 are not assigned: kvp_launches_per_compress answers KVP_ERR_BAD_ARGUMENT for them, as for any
+     * unknown id */
     KVP_SCORER_CUR = 11,
     KVP_SCORER_MERGING = 13, /* kvp_merging_*: the selection of the caller's scores, then the merge */
-    KVP_SCORER_THINK = 14    /* kvp_think_prune: key channels, not positions */
+    KVP_SCORER_THINK = 14,   /* kvp_think_prune: key channels, not positions */
+    KVP_SCORER_FINCH = 16    /* kvp_finch_*, kvp_scores_compress_chunked */
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -400,6 +401,65 @@ int kvp_merging_merge(const kvp_problem* p, const void* K, const void* V, const 
 kvp_status kvp_think_prune(const kvp_problem* p, void* K, const void* q_window, int32_t window, int32_t n_pruned,
                            int32_t* pruned_out, float* channel_scores_out, void* workspace, size_t workspace_bytes,
                            kvp_stream_t stream);
+
+/* ---- FinchPress (kvpress/presses/finch_press.py, https://direct.mit.edu/tacl/article/doi/10.1162/tacl_a_00716) ------
+ * SnapKV with the window set by the prompt: the w queries after the user's delimiter (the question) score the context
+ * and are always kept. Per row (b, kv head j), with G = Hq / Hkv and the window queries at positions S - w + i:
+ *   P[h, i, s]  = softmax over all S keys of q_window[b, h, i] . K[b, j, s] / sqrt(D), causal inside the window
+ *   c_i         = S - w + i if normalize != 0, else 1
+ *   score(s)    = 1/(G w) sum_{g<G} sum_{i<w} c_i P[b, jG+g, i, s]     for the context positions s < S - w
+ * evaluated in fp32 and rounded once to the cache dtype (a score beyond the fp16 range is +inf, as in the reference).
+ * The scale is 1/sqrt(D), as in the reference's compute_window_attention. Deviation: c_i is the exact integer; the
+ * reference multiplies its cache-dtype weights by an int64 arange, which rounds c_i to the cache dtype (8 significant
+ * bits in bf16; inf from 65520 on in fp16, which makes its scores inf or NaN). scores_out (nullable) holds the scores
+ * and, at the w window positions, the reference's sentinel: the largest context score of the whole call + 1, rounded
+ * to the cache dtype. The selection forces the window instead (as SnapKV's), so it is kept even where max + 1 rounds
+ * back to max.
+ * Selection of kvp_finch_compress:
+ *   - chunk_length == 0: the n_kept best positions of the row (chunk_kept and tail_kept are ignored).
+ *   - chunk_length > 0: chunk c covers [c L, min(S, (c+1) L)), L = chunk_length. Each of the n_full = S / L full chunks
+ *     keeps its chunk_kept best positions, the short last chunk (S mod L positions, if any) its tail_kept best; a window
+ *     position in the short last chunk competes for that chunk's budget. The host computes the counts (the reference's
+ *     max(1, int(len (1 - r)))); n_kept must be n_full chunk_kept + tail_kept.
+ *   Ties go to the lowest positions; the kept rows come out in ascending position order.
+ *   - inv_freq (nullable, fp32 [D/2]): the key kept at position s that lands in output row j is re-rotated by
+ *     (j - s) inv_freq with kvp_scores_compress_rerotate's rounding points; values are copied exactly. With a null
+ *     inv_freq K_out and V_out are exact gathers.
+ * q_window: RoPE'd window queries [B, Hq, w, D], contiguous, in K's dtype, 16-byte aligned; 1 <= w < S.
+ * Instantiated for bf16 / fp16, D in {64, 128} and 1 <= G <= 8; other shapes give KVP_ERR_UNSUPPORTED_SHAPE (FinchPress
+ * scores them with blocked cuBLAS GEMMs and selects through kvp_scores_compress_chunked). Indexing is 64-bit. Every sum
+ * has a fixed order that depends on (S, w, G, D) only: two calls give bitwise-equal results, and a row's scores do not
+ * depend on the batch or the strides.
+ * Check order (the first failure is returned): validate the problem -> (compress) n_kept == 0 returns KVP_OK ->
+ * (compress) K / V / K_out / V_out null and 16-byte alignment -> K (score), q_window, scores_out (score) null ->
+ * K (score), q_window 16-byte alignment -> w < 1 or w >= S gives KVP_ERR_BAD_ARGUMENT -> (compress) chunk_length < 0,
+ * or with chunk_length > 0: chunk_kept outside [1, L] while n_full > 0, tail_kept outside [1, S mod L] (0 when L
+ * divides S) or n_kept != n_full chunk_kept + tail_kept gives KVP_ERR_BAD_ARGUMENT -> D not 64 / 128 or G > 8 gives
+ * KVP_ERR_UNSUPPORTED_SHAPE -> workspace null -> its 16-byte alignment -> its size.
+ * kvp_workspace_bytes(KVP_SCORER_FINCH) sizes the largest window, w = S - 1: the selection regions every scorer has,
+ * plus 4 R S (chunked selection: kept positions) + 8 B Hq (64 qpos + w) (softmax partials; qpos = 128 for G = 1, else
+ * 64) + 4 B Hq w (normalisers) + 4 R S_pad (column sums), each region rounded up to 256 bytes (R = B Hkv, S_pad = S
+ * rounded up to 256). A compress takes 6 launches unchunked (memset, stats, merge, column sums, finalize,
+ * select+compact) and 7 chunked (the selection is a chunk select and a gather); scores_out adds the sentinel fill.
+ * Memory beyond the workspace: none; no [Hq, w, S] tensor is formed.
+ * The return type is kvp_status, an int-sized enum with the values of every other entry point's int. */
+kvp_status kvp_finch_score(const kvp_problem* p, const void* K, const void* q_window, int32_t window, int32_t normalize,
+                           void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+kvp_status kvp_finch_compress(const kvp_problem* p, const void* K, const void* V, const void* q_window, int32_t window,
+                              int32_t normalize, int32_t chunk_length, int32_t chunk_kept, int32_t tail_kept,
+                              const float* inv_freq, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
+                              void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+/* The chunked selection of kvp_finch_compress on caller scores [B, Hkv, S] (K's dtype, element strides score_stride for
+ * (b, h), s contiguous), with inv_freq nullable as there (D a multiple of 16 when given). Check order: validate the
+ * problem -> n_kept == 0 returns KVP_OK -> K / V / K_out / V_out null and alignment -> scores, score_stride null ->
+ * chunk_length < 1 or the chunk counts as above give KVP_ERR_BAD_ARGUMENT -> inv_freq with D not a multiple of 16
+ * gives KVP_ERR_UNSUPPORTED_SHAPE -> workspace (kvp_workspace_bytes(KVP_SCORER_FINCH) is enough). 4 launches (memset,
+ * keys, chunk select, gather). */
+kvp_status kvp_scores_compress_chunked(const kvp_problem* p, const void* scores, const int64_t* score_stride,
+                                       int32_t chunk_length, int32_t chunk_kept, int32_t tail_kept, const void* K,
+                                       const void* V, const float* inv_freq, void* K_out, void* V_out,
+                                       int32_t* idx_out, void* workspace, size_t workspace_bytes,
+                                       kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

@@ -30,6 +30,7 @@ from kvpress_b200.presses.random_press import RandomPress
 from kvpress_b200.presses.scorer_press import ScorerPress
 from kvpress_b200.presses.snapkv_press import SnapKVPress
 from kvpress_b200.presses.streaming_llm_press import StreamingLLMPress
+from kvpress_b200.presses.finch_press import FinchPress
 from kvpress_b200.presses.think_press import ThinKPress
 from kvpress_b200.presses.tova_press import TOVAPress
 
@@ -58,6 +59,7 @@ __all__ = [
     "CURPress",
     "MergingPress",
     "ThinKPress",
+    "FinchPress",
     "BlockPress",
     "ChunkPress",
     "ChunkKVPress",

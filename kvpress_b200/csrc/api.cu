@@ -16,13 +16,14 @@ namespace kvp {
 static thread_local char g_last_cuda_error[256] = "";
 
 // kvp_status of a CUDA call. The KeyDiff, SnapKV, ExpectedAttention, CriticalKV, ObservedAttention, NonCausalAttention,
-// LagKV and CUR score launchers report a shape they have no kernel for as cudaErrorNotSupported.
+// LagKV, CUR and Finch score launchers report a shape they have no kernel for as cudaErrorNotSupported.
 static int status(cudaError_t e, int scorer = KVP_SCORER_GENERIC) {
     if (e == cudaSuccess) return KVP_OK;
     if (e == cudaErrorNotSupported &&
         (scorer == KVP_SCORER_KEYDIFF || scorer == KVP_SCORER_SNAPKV || scorer == KVP_SCORER_EXPECTED_ATTENTION ||
          scorer == KVP_SCORER_CRITICALKV || scorer == KVP_SCORER_OBSERVED_ATTENTION ||
-         scorer == KVP_SCORER_NON_CAUSAL_ATTENTION || scorer == KVP_SCORER_LAGKV || scorer == KVP_SCORER_CUR))
+         scorer == KVP_SCORER_NON_CAUSAL_ATTENTION || scorer == KVP_SCORER_LAGKV || scorer == KVP_SCORER_CUR ||
+         scorer == KVP_SCORER_FINCH))
         return KVP_ERR_UNSUPPORTED_SHAPE;
     snprintf(g_last_cuda_error, sizeof(g_last_cuda_error), "%s: %s", cudaGetErrorName(e), cudaGetErrorString(e));
     // launch-configuration errors are not sticky: clear them, or the cudaPeekAtLastError() of every later call
@@ -62,15 +63,17 @@ static int validate(const kvp_problem* p, Dims* d, bool need_kv_strides = true) 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // The window kvp_workspace_bytes / kvp_workspace_check size a scorer's scratch for: the largest a call may pass.
-// ObservedAttention: n_q = S. SnapKV: the most query rows G * window <= kSnapMaxRows with window < S (at least 1, so
-// that a group too wide for any window still reaches the launcher's unsupported-shape status).
+// ObservedAttention: n_q = S. Finch: w = S - 1 (at least 1). SnapKV: the most query rows G * window <= kSnapMaxRows
+// with window < S (at least 1, so that a group too wide for any window still reaches the launcher's unsupported-shape
+// status).
 static int largest_window(const Dims& d, int scorer) {
     if (scorer == KVP_SCORER_OBSERVED_ATTENTION) return d.S;
+    if (scorer == KVP_SCORER_FINCH) return std::max(1, d.S - 1);
     return std::max(1, std::min(kSnapMaxRows / (d.Hq / d.H), d.S - 1));
 }
 
-// The workspace of a call: sized when `base` is null, carved otherwise. `window` is SnapKV's window, or the query rows
-// n_q of ObservedAttention. Returns the total bytes and, in *zeroed, the
+// The workspace of a call: sized when `base` is null, carved otherwise. `window` is SnapKV's or Finch's window, or the
+// query rows n_q of ObservedAttention. Returns the total bytes and, in *zeroed, the
 // leading bytes every call clears with one memset: the histograms, the counters and the tile prefixes. The
 // histograms are whole KiB per row, so hist_lo and the counters follow hist_hi without padding.
 static size_t layout(const Dims& d, int scorer, int window, void* base, Workspace* ws, size_t* zeroed) {
@@ -102,6 +105,7 @@ static size_t layout(const Dims& d, int scorer, int window, void* base, Workspac
                        : scorer == KVP_SCORER_NON_CAUSAL_ATTENTION ? non_causal_attention_scratch_bytes(d)
                        : scorer == KVP_SCORER_CUR                  ? cur_scratch_bytes(d)
                        : scorer == KVP_SCORER_MERGING              ? merging_scratch_bytes(d)
+                       : scorer == KVP_SCORER_FINCH                ? finch_scratch_bytes(d, window)
                                                                    : 0;
     ws->scorer = c.take<char>(ws->scorer_bytes);
     return c.bytes;
@@ -138,6 +142,8 @@ struct Io {
     const float* inv_freq;  // kvp_scores_compress_rerotate: the kept keys are re-rotated
     // where the selection writes the kept positions when idx_out is null and a later stage reads them (MergingPress)
     int32_t* (*kept_scratch)(const Dims&, const Workspace&) = nullptr;
+    // chunk_length > 0: the chunked selection of FinchPress (kvp_finch_compress, kvp_scores_compress_chunked)
+    int32_t chunk_length = 0, chunk_kept = 0, tail_kept = 0;
 };
 
 enum class Kind {
@@ -173,6 +179,10 @@ static int run(Kind kind, const kvp_problem* p, int scorer, int window, const Io
     if (zero && (rc = c.zero())) return rc;
     if ((rc = status(score(c), scorer))) return rc;
     if (kind == Kind::score) return KVP_OK;
+    if (io.chunk_length > 0)
+        return status(launch_select_compact_chunked(c.d, p->dtype, io.K, io.V, io.K_out, io.V_out, io.idx_out, c.ws,
+                                                    io.chunk_length, io.chunk_kept, io.tail_kept,
+                                                    finch_scratch_kept(c.d, c.ws), io.inv_freq, c.st));
     if (io.inv_freq)
         return status(launch_select_compact_rerotate(c.d, p->dtype, io.K, io.V, io.K_out, io.V_out, io.idx_out, c.ws,
                                                      io.inv_freq, c.st));
@@ -203,6 +213,24 @@ static KnormPath knorm_path(const kvp_problem& p, const Dims* d) {
     constexpr size_t kFusedMaxBytes = (size_t)32 << 20;
     const size_t k_bytes = (size_t)p.B * p.Hkv * p.S * p.D * 2;
     return first <= 1 && k_bytes <= kFusedMaxBytes ? KnormPath::fused : KnormPath::two_kernels;
+}
+
+// The chunk counts of a chunked selection (chunk_length > 0), see kvp_finch_compress in the header.
+static int chunk_counts_ok(const Dims& d, int32_t chunk_length, int32_t chunk_kept, int32_t tail_kept) {
+    const int n_full = d.S / chunk_length, tail = d.S % chunk_length;
+    if (n_full > 0 && (chunk_kept < 1 || chunk_kept > chunk_length)) return KVP_ERR_BAD_ARGUMENT;
+    if (tail > 0 ? (tail_kept < 1 || tail_kept > tail) : tail_kept != 0) return KVP_ERR_BAD_ARGUMENT;
+    const int64_t total = (int64_t)n_full * (n_full > 0 ? chunk_kept : 0) + tail_kept;
+    return total == d.n_kept ? KVP_OK : KVP_ERR_BAD_ARGUMENT;
+}
+
+// Finch's window and instantiation checks, after its null / alignment checks and (compress) its chunk checks.
+static int finch_window_ok(const Dims& d, int32_t window) {
+    return window >= 1 && window < d.S ? KVP_OK : KVP_ERR_BAD_ARGUMENT;
+}
+static int finch_shape_ok(const Dims& d) {
+    const int G = d.Hq / d.H;
+    return (d.D == 64 || d.D == 128) && G <= 8 ? KVP_OK : KVP_ERR_UNSUPPORTED_SHAPE;
 }
 
 }  // namespace kvp
@@ -289,6 +317,8 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
             break;
         }
         case KVP_SCORER_THINK: *launches_out = 3; break;  // memset, reduce + select, zero
+        // unchunked: memset, stats, merge, column sums, finalize, select+compact (chunked: one more, see the header)
+        case KVP_SCORER_FINCH: *launches_out = 6; break;
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -749,6 +779,70 @@ kvp_status kvp_think_prune(const kvp_problem* p, void* K, const void* q_window, 
     if ((rc = c.carve(KVP_SCORER_THINK, 0, workspace, workspace_bytes))) return static_cast<kvp_status>(rc);
     return static_cast<kvp_status>(status(launch_think_prune(c.d, p->dtype, K, q_window, window, n_pruned, pruned_out,
                                                              channel_scores_out, c.ws.scorer, c.st)));
+}
+
+// ---- Finch ---------------------------------------------------------------------------------------------------------
+static auto finch_stage(const kvp_problem* p, const void* K, const void* q_window, int32_t window, int32_t normalize,
+                        void* scores_out) {
+    return [=](const Call& c) {
+        return launch_finch_score(c.d, p->dtype, K, q_window, window, normalize, c.ws, scores_out, c.st);
+    };
+}
+
+kvp_status kvp_finch_score(const kvp_problem* p, const void* K, const void* q_window, int32_t window, int32_t normalize,
+                           void* scores_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!K || !q_window || !scores_out) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(K) || !aligned16(q_window)) return KVP_ERR_BAD_STRIDE;
+        int rc = finch_window_ok(d, window);
+        return rc ? rc : finch_shape_ok(d);
+    };
+    return static_cast<kvp_status>(run(Kind::score, p, KVP_SCORER_FINCH, window, {}, operands,
+                                       finch_stage(p, K, q_window, window, normalize, scores_out), workspace,
+                                       workspace_bytes, stream));
+}
+
+kvp_status kvp_finch_compress(const kvp_problem* p, const void* K, const void* V, const void* q_window, int32_t window,
+                              int32_t normalize, int32_t chunk_length, int32_t chunk_kept, int32_t tail_kept,
+                              const float* inv_freq, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
+                              void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!q_window) return KVP_ERR_NULL_POINTER;
+        if (!aligned16(q_window)) return KVP_ERR_BAD_STRIDE;
+        int rc = finch_window_ok(d, window);
+        if (rc) return rc;
+        if (chunk_length < 0) return KVP_ERR_BAD_ARGUMENT;
+        if (chunk_length > 0 && (rc = chunk_counts_ok(d, chunk_length, chunk_kept, tail_kept))) return rc;
+        return finch_shape_ok(d);
+    };
+    Io io = {K, V, K_out, V_out, idx_out, inv_freq};
+    io.chunk_length = chunk_length;
+    io.chunk_kept = chunk_kept;
+    io.tail_kept = tail_kept;
+    return static_cast<kvp_status>(run(Kind::compress, p, KVP_SCORER_FINCH, window, io, operands,
+                                       finch_stage(p, K, q_window, window, normalize, scores_out), workspace,
+                                       workspace_bytes, stream));
+}
+
+kvp_status kvp_scores_compress_chunked(const kvp_problem* p, const void* scores, const int64_t* score_stride,
+                                       int32_t chunk_length, int32_t chunk_kept, int32_t tail_kept, const void* K,
+                                       const void* V, const float* inv_freq, void* K_out, void* V_out,
+                                       int32_t* idx_out, void* workspace, size_t workspace_bytes,
+                                       kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!scores || !score_stride) return KVP_ERR_NULL_POINTER;
+        if (chunk_length < 1) return KVP_ERR_BAD_ARGUMENT;
+        int rc = chunk_counts_ok(d, chunk_length, chunk_kept, tail_kept);
+        if (rc) return rc;
+        return inv_freq && d.D % 16 != 0 ? KVP_ERR_UNSUPPORTED_SHAPE : KVP_OK;
+    };
+    Io io = {K, V, K_out, V_out, idx_out, inv_freq};
+    io.chunk_length = chunk_length;
+    io.chunk_kept = chunk_kept;
+    io.tail_kept = tail_kept;
+    // the Finch layout at the smallest window: the selection regions and the kept positions
+    return static_cast<kvp_status>(run(Kind::compress, p, KVP_SCORER_FINCH, 1, io, operands,
+                                       keys_from(p, scores, score_stride), workspace, workspace_bytes, stream));
 }
 
 }  // extern "C"

@@ -479,6 +479,21 @@ int32_t* merging_scratch_kept(const Dims& d, const Workspace& ws);
 cudaError_t launch_merging(const Dims& d, int dtype, const void* K, const void* V, const int32_t* kept, float threshold,
                            double merge_fraction, void* V_out, int32_t* target_out, float* sim_out, const Workspace& ws,
                            cudaStream_t st);
+// ObservedAttention's column-sum pass (observed_attention.cu) over the key tiles [0, n_ktiles) of every row: colsum[s] =
+// sum over the n_q query rows r of the kv head's G query heads of exp2(c q_r.k_s + cb[r]), causal for the query
+// positions S - n_q + r. cb is [B Hq][n_q] in log2 units. D = 64 / 128 only (cudaErrorNotSupported otherwise).
+cudaError_t launch_attention_colsum(const Dims& d, int dtype, const void* K, const void* q, int n_q, int n_ktiles,
+                                    float c, const float* cb, float* colsum, int S_pad, cudaStream_t st);
+size_t finch_scratch_bytes(const Dims& d, int window);
+int32_t* finch_scratch_kept(const Dims& d, const Workspace& ws);
+cudaError_t launch_finch_score(const Dims& d, int dtype, const void* K, const void* q_window, int window,
+                               int normalize, const Workspace& ws, void* scores_out, cudaStream_t st);
+// the chunk select and the gather of FinchPress's chunked selection (select_compact.cu) on the keys in ws; `kept` is
+// [R][n_kept] scratch; inv_freq null: exact gathers
+cudaError_t launch_select_compact_chunked(const Dims& d, int dtype, const void* K, const void* V, void* K_out,
+                                          void* V_out, int32_t* idx_out, const Workspace& ws, int chunk_length,
+                                          int chunk_kept, int tail_kept, int32_t* kept, const float* inv_freq,
+                                          cudaStream_t st);
 size_t think_scratch_bytes(const Dims& d);
 // a memset of the row tickets, the reduce + select kernel and the zero kernel on `scratch` (think_scratch_bytes)
 cudaError_t launch_think_prune(const Dims& d, int dtype, void* K, const void* q, int window, int n_pruned,

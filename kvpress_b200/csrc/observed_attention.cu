@@ -50,13 +50,9 @@ size_t observed_attention_scratch_bytes(const Dims& d, int n_q) {
 }
 
 // ---- schedule (host and device) ----------------------------------------------------------------------------------
-// Pass 1: query positions per item (G heads x qpos rows resident), items = R * ceil(n_q / qpos). Item u is the block
-// qb = n_blocks - 1 - u / R of row u % R: later blocks see more keys, so the work (K tiles) never increases with u.
-__host__ __device__ inline int obs_qpos(int G) { return G == 1 ? 128 : 64; }
-__host__ __device__ inline int obs_stats_tiles(int S, int n_q, int p0, int qpos) {  // K tiles of the block at p0
-    const int end = min(S, S - n_q + p0 + qpos);
-    return (end + kSnTile - 1) / kSnTile;
-}
+// Pass 1: query positions per item (G heads x obs_qpos(G) rows resident, qk_tiles.cuh), items = R * ceil(n_q / qpos).
+// Item u is the block qb = n_blocks - 1 - u / R of row u % R: later blocks see more keys, so the work (K tiles,
+// obs_stats_tiles) never increases with u.
 // Pass 2: items = R * ceil(S / 128). Item u is the key tile kt = u / R of row u % R; its query rows start at
 // i_min = max(0, 128 kt - (S - n_q)), so its work (G x Q chunks) never increases with u.
 __host__ __device__ inline int obs_colsum_imin(int S, int n_q, int kt) { return max(0, kt * kSnTile - (S - n_q)); }
@@ -315,38 +311,63 @@ obs_finalize_kernel(int S, int G, ObsScratch sc, Workspace ws, uint16_t* __restr
     });
 }
 
-// ---- host launcher ------------------------------------------------------------------------------------------------
+// ---- host launchers -----------------------------------------------------------------------------------------------
+// Pass 2 over the key tiles [0, n_ktiles) of every row (see qk_tiles.cuh, launch_attention_colsum).
+template <typename T, int D>
+static cudaError_t launch_obs_colsum_t(const Dims& d, const void* K, const void* q, int n_q, int n_ktiles, float c,
+                                       const float* cb, float* colsum, int S_pad, cudaStream_t st) {
+    using L2 = ObsColSmem<D>;
+    const int grid2 = (int)std::min<long long>(device_sm_count(), (long long)d.R * n_ktiles);
+    if (grid2 == 0) return cudaSuccess;
+    CUtensorMap mapK, mapQ2;
+    cudaError_t e;
+    if ((e = make_tmap_cache(&mapK, K, d, d.ks, kSnTile)) != cudaSuccess) return e;
+    const uint64_t n_heads = (uint64_t)d.B * d.Hq, head_stride = (uint64_t)n_q * D;
+    if ((e = make_tmap_rows(&mapQ2, q, D, n_q, D, n_heads, head_stride, kSnTile)) != cudaSuccess) return e;
+    constexpr int smem2 = umma::smem_request(L2::kTotal);
+    constexpr auto k2 = obs_colsum_kernel<T, D>;
+    if ((e = ensure_dynamic_smem<k2>(smem2)) != cudaSuccess) return e;
+    const ObsScratch sc = {const_cast<float*>(cb), colsum};
+    k2<<<grid2, umma::kTmaCtaThreads, smem2, st>>>(mapK, mapQ2, d.H, d.Hq / d.H, d.S, n_q, d.R, n_ktiles, c, sc, S_pad);
+    return cudaPeekAtLastError();
+}
+
+cudaError_t launch_attention_colsum(const Dims& d, int dtype, const void* K, const void* q, int n_q, int n_ktiles,
+                                    float c, const float* cb, float* colsum, int S_pad, cudaStream_t st) {
+    return with_dtype(dtype, [&](auto t) -> cudaError_t {
+        using T = decltype(t);
+        if (d.D == 128) return launch_obs_colsum_t<T, 128>(d, K, q, n_q, n_ktiles, c, cb, colsum, S_pad, st);
+        if (d.D == 64) return launch_obs_colsum_t<T, 64>(d, K, q, n_q, n_ktiles, c, cb, colsum, S_pad, st);
+        return cudaErrorNotSupported;
+    });
+}
+
 template <typename T, int D, int NQP>
 static cudaError_t launch_obs_t(const Dims& d, const void* K, const void* q, int n_q, float scaling,
                                 const Workspace& ws, void* scores_out, cudaStream_t st) {
     using L1 = SnSmem<D, NQP>;
-    using L2 = ObsColSmem<D>;
     const int sm_count = device_sm_count();
     const int G = d.Hq / d.H, qpos = obs_qpos(G);
     const ObsScratch sc = carve_obs(d, n_q, ws.scorer);
     const int n_blocks = (n_q + qpos - 1) / qpos;
     const int n_ktiles = (d.S + kSnTile - 1) / kSnTile;
     const int grid1 = (int)std::min<long long>(sm_count, (long long)d.R * n_blocks);
-    const int grid2 = (int)std::min<long long>(sm_count, (long long)d.R * n_ktiles);
     const float c = kLog2e * scaling;  // logits -> log2 domain
 
-    CUtensorMap mapK, mapQ1, mapQ2;
+    CUtensorMap mapK, mapQ1;
     cudaError_t e;
     if ((e = make_tmap_cache(&mapK, K, d, d.ks, kSnTile)) != cudaSuccess) return e;
     // q [B Hq, n_q, D] contiguous: rows past n_q of a head read as zero
     const uint64_t n_heads = (uint64_t)d.B * d.Hq, head_stride = (uint64_t)n_q * D;
     if ((e = make_tmap_rows(&mapQ1, q, D, n_q, D, n_heads, head_stride, qpos)) != cudaSuccess) return e;
-    if ((e = make_tmap_rows(&mapQ2, q, D, n_q, D, n_heads, head_stride, kSnTile)) != cudaSuccess) return e;
-    constexpr int smem1 = umma::smem_request(L1::kTotal), smem2 = umma::smem_request(L2::kTotal);
+    constexpr int smem1 = umma::smem_request(L1::kTotal);
     constexpr auto k1 = obs_stats_kernel<T, D, NQP>;
-    constexpr auto k2 = obs_colsum_kernel<T, D>;
     if ((e = ensure_dynamic_smem<k1>(smem1)) != cudaSuccess) return e;
-    if ((e = ensure_dynamic_smem<k2>(smem2)) != cudaSuccess) return e;
 
     k1<<<grid1, umma::kTmaCtaThreads, smem1, st>>>(mapK, mapQ1, d.H, G, d.S, n_q, qpos, d.R, n_blocks, c, sc);
     if ((e = cudaPeekAtLastError()) != cudaSuccess) return e;
-    k2<<<grid2, umma::kTmaCtaThreads, smem2, st>>>(mapK, mapQ2, d.H, G, d.S, n_q, d.R, n_ktiles, c, sc, ws.S_pad);
-    if ((e = cudaPeekAtLastError()) != cudaSuccess) return e;
+    if ((e = launch_obs_colsum_t<T, D>(d, K, q, n_q, n_ktiles, c, sc.cb, sc.colsum, ws.S_pad, st)) != cudaSuccess)
+        return e;
     obs_finalize_kernel<T><<<dim3(ws.n_tiles, d.R), kTileThreads, 0, st>>>(d.S, G, sc, ws,
                                                                             static_cast<uint16_t*>(scores_out));
     return cudaPeekAtLastError();

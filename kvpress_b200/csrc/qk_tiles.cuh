@@ -37,6 +37,15 @@ struct SnSmem {
     static_assert(umma::smem_request(kTotal) <= umma::kSmemBudget, "shared memory budget");
 };
 
+// Query blocks of the scorers whose query rows have positions S - n_q + i (ObservedAttention, Finch): a block holds
+// qpos consecutive positions of each of the G query heads of a kv head, resident as G qpos rows.
+__host__ __device__ inline int obs_qpos(int G) { return G == 1 ? 128 : 64; }
+// The K tiles the block starting at query row p0 sees (causal): keys [0, S - n_q + p0 + qpos), clipped to S.
+__host__ __device__ inline int obs_stats_tiles(int S, int n_q, int p0, int qpos) {
+    const int end = min(S, S - n_q + p0 + qpos);
+    return (end + kSnTile - 1) / kSnTile;
+}
+
 // acc[64] (+)= A[64 rows x D] * B[128 rows x D]^T, both K-major SW128 panels (`a_panel` / `b_panel` bytes apart)
 template <typename T, int D>
 __device__ __forceinline__ void snap_mma(float (&acc)[64], uint32_t a, int a_panel, uint32_t b, int b_panel) {

@@ -491,6 +491,148 @@ cudaError_t launch_select_compact_rerotate(const Dims& d, int dtype, const void*
     });
 }
 
+// ---- chunked selection (FinchPress with chunk_length) --------------------------------------------------------------
+// Chunk c of a row holds positions [c L, min(S, (c + 1) L)). The n_full = S / L full chunks keep their best chunk_kept,
+// the short last chunk (S % L positions, if any) its best tail_kept; chunk c's k-th kept position, in ascending order,
+// goes to output row c chunk_kept + k. Ties at a chunk's threshold go to its lowest positions.
+// Item of chunk_select_kernel = (chunk, row): the exact 16-bit threshold of the chunk from two 256-bin histograms of
+// its keys, then the kept positions in position order into `kept` [R][n_kept]. It reads 2 bytes per position three
+// times; the K / V rows are moved by chunk_gather_kernel, whose items are (256 output rows, row), so the copy spreads
+// over the GPU however long the chunks are.
+__global__ void __launch_bounds__(kTileThreads)
+chunk_select_kernel(int S, int L, int chunk_kept, int tail_kept, int n_kept, Workspace ws, int32_t* __restrict__ kept) {
+    __shared__ uint32_t hist[256];
+    __shared__ uint32_t wsum[2][8];
+    __shared__ uint32_t thr[2];
+    const int c = blockIdx.x, row = blockIdx.y, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int lo = c * L, hi = (int)std::min<long long>(S, (long long)lo + L);
+    const uint32_t k = c < S / L ? (uint32_t)chunk_kept : (uint32_t)tail_kept;
+    const uint16_t* keys = ws.keys + (size_t)row * ws.S_pad;
+    int32_t* out = kept + (size_t)row * n_kept + (size_t)c * chunk_kept;
+
+    // threshold bin of the high bytes, then the low byte inside it: T and the ties at T to take
+    hist[tid] = 0;
+    __syncthreads();
+    for (int base = lo; base < hi; base += kTileThreads) {
+        const int s = base + tid;
+        warp_hist_add(hist, s < hi ? (unsigned)(__ldcg(keys + s) >> 8) : 256u);
+    }
+    __syncthreads();
+    if (warp == 0) {
+        int b1;
+        uint32_t above;
+        warp_suffix_find(hist, k, lane, b1, above);
+        if (lane == 0) {
+            thr[0] = (uint32_t)b1;
+            thr[1] = k - above;  // >= 1
+        }
+    }
+    __syncthreads();
+    const uint32_t b1 = thr[0], need = thr[1];
+    hist[tid] = 0;
+    __syncthreads();
+    for (int base = lo; base < hi; base += kTileThreads) {
+        const int s = base + tid;
+        const uint32_t key = s < hi ? __ldcg(keys + s) : 0u;
+        warp_hist_add(hist, s < hi && (key >> 8) == b1 ? (key & 255u) : 256u);
+    }
+    __syncthreads();
+    if (warp == 0) {
+        int lo1;
+        uint32_t above;
+        warp_suffix_find(hist, need, lane, lo1, above);
+        if (lane == 0) {
+            thr[0] = (b1 << 8) | (uint32_t)lo1;
+            thr[1] = need - above;  // >= 1
+        }
+    }
+    __syncthreads();
+    const uint32_t T = thr[0], n_take = thr[1];
+
+    // kept positions in position order: the keys above T, and the first n_take keys equal to T
+    uint32_t kept_before = 0, eq_before = 0;
+    for (int base = lo; base < hi; base += kTileThreads) {
+        const int s = base + tid;
+        const uint32_t key = s < hi ? __ldcg(keys + s) : 0u;
+        const bool is_gt = s < hi && key > T, is_eq = s < hi && key == T;
+        const unsigned m_gt = __ballot_sync(0xFFFFFFFFu, is_gt), m_eq = __ballot_sync(0xFFFFFFFFu, is_eq);
+        if (lane == 0) {
+            wsum[0][warp] = __popc(m_gt);
+            wsum[1][warp] = __popc(m_eq);
+        }
+        __syncthreads();
+        uint32_t gt_rank = __popc(m_gt & ((1u << lane) - 1u)), eq_rank = __popc(m_eq & ((1u << lane) - 1u));
+        uint32_t tot_gt = 0, tot_eq = 0;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) {
+            gt_rank += (w < warp) ? wsum[0][w] : 0u;
+            eq_rank += (w < warp) ? wsum[1][w] : 0u;
+            tot_gt += wsum[0][w];
+            tot_eq += wsum[1][w];
+        }
+        __syncthreads();  // wsum is rewritten by the next tile
+        const uint32_t tie_room = n_take > eq_before ? n_take - eq_before : 0u;
+        if (is_gt || (is_eq && eq_rank < tie_room)) out[kept_before + gt_rank + min(eq_rank, tie_room)] = s;
+        kept_before += tot_gt + min(tot_eq, tie_room);
+        eq_before += tot_eq;
+    }
+}
+
+// Output rows [256 x, 256 x + 256) of row y: dst row j <- the kept position kept[y][j]; TR = cache dtype re-rotates the
+// keys by delta = j - s (copy_rows_k_rerotated), TR = void copies K and V exactly.
+template <typename TR>
+__global__ void __launch_bounds__(kTileThreads)
+chunk_gather_kernel(const char* __restrict__ K, const char* __restrict__ V, Strides3 ks, Strides3 vs,
+                    char* __restrict__ K_out, char* __restrict__ V_out, int32_t* __restrict__ idx_out, int H, int D,
+                    int n_kept, const int32_t* __restrict__ kept, const float* __restrict__ inv_freq) {
+    __shared__ int list[kTile];
+    const int row = blockIdx.y, tid = threadIdx.x, b = row / H, h = row % H;
+    const int j0 = blockIdx.x * kTile, count = min(kTile, n_kept - j0);
+    const int64_t out_row0 = (int64_t)row * n_kept + j0;
+    if (tid < count) {
+        list[tid] = kept[out_row0 + tid];
+        if (idx_out != nullptr) idx_out[out_row0 + tid] = list[tid];
+    }
+    __syncthreads();
+    const int64_t row_bytes = (int64_t)D * 2;
+    const char* k_src = K + ((int64_t)b * ks.b + (int64_t)h * ks.h) * 2;
+    const char* v_src = V + ((int64_t)b * vs.b + (int64_t)h * vs.h) * 2;
+    if constexpr (std::is_void<TR>::value) {
+        copy_rows_kv<kSelU>(k_src, ks.s * 2, v_src, vs.s * 2, K_out + out_row0 * row_bytes,
+                            V_out + out_row0 * row_bytes, row_bytes, list, count, D >> 3);
+    } else {
+        copy_rows_k_rerotated<TR>(k_src, ks.s * 2, K_out + out_row0 * row_bytes, row_bytes, list, count, D, inv_freq,
+                                  j0);
+        copy_rows_single(v_src, vs.s * 2, V_out + out_row0 * row_bytes, row_bytes, list, count, D >> 3);
+    }
+}
+
+cudaError_t launch_select_compact_chunked(const Dims& d, int dtype, const void* K, const void* V, void* K_out,
+                                          void* V_out, int32_t* idx_out, const Workspace& ws, int chunk_length,
+                                          int chunk_kept, int tail_kept, int32_t* kept, const float* inv_freq,
+                                          cudaStream_t st) {
+    const int n_chunks = (int)(((long long)d.S + chunk_length - 1) / chunk_length);
+    chunk_select_kernel<<<dim3(n_chunks, d.R), kTileThreads, 0, st>>>(d.S, chunk_length, chunk_kept, tail_kept,
+                                                                      d.n_kept, ws, kept);
+    cudaError_t e = cudaPeekAtLastError();
+    if (e != cudaSuccess) return e;
+    const dim3 grid((d.n_kept + kTile - 1) / kTile, d.R);
+    const char* k = static_cast<const char*>(K);
+    const char* v = static_cast<const char*>(V);
+    char* ko = static_cast<char*>(K_out);
+    char* vo = static_cast<char*>(V_out);
+    if (inv_freq == nullptr) {
+        chunk_gather_kernel<void><<<grid, kTileThreads, 0, st>>>(k, v, d.ks, d.vs, ko, vo, idx_out, d.H, d.D,
+                                                                 d.n_kept, kept, nullptr);
+    } else {
+        with_dtype(dtype, [&](auto t) {
+            chunk_gather_kernel<decltype(t)><<<grid, kTileThreads, 0, st>>>(k, v, d.ks, d.vs, ko, vo, idx_out, d.H,
+                                                                            d.D, d.n_kept, kept, inv_freq);
+        });
+    }
+    return cudaPeekAtLastError();
+}
+
 // ---- KnormPress: score + select + compact in ONE persistent kernel ---------------------------------
 // Work items of three kinds share one ticket queue: S(row, chunk) scores 256 positions and adds to the
 // row histogram; A(row, group) is the refine item (waits until all S items of its row are done);

@@ -23,6 +23,7 @@ _LIB_PATH = Path(__file__).resolve().parent / _LIB_NAME
 SCORER_CUR = 11  # KVP_SCORER_CUR; id 10 is not assigned
 SCORER_MERGING = 13  # KVP_SCORER_MERGING; id 12 is not assigned
 SCORER_THINK = 14  # KVP_SCORER_THINK: kvp_think_prune
+SCORER_FINCH = 16  # KVP_SCORER_FINCH: kvp_finch_*, kvp_scores_compress_chunked; id 15 is not assigned
 LAG_MAX = 1024  # the largest lag_size the LagKV kernel scores (kLagMax in csrc/common.cuh)
 CUR_WINDOW_MAX = 1024  # the largest local_window_size the CUR kernel scores (kCurWindowMax in csrc/common.cuh)
 CUR_RANK_MAX = 32  # the most projection columns the CUR kernel scores (kCurRankMax)
@@ -98,6 +99,9 @@ SIGNATURES = {
         ctypes.c_int, [_PP, _P, _PI64, _P, _P, ctypes.c_float, ctypes.c_double, _P, _P, _P, _P, _P, _P, _SZ, _P]),
     "kvp_merging_merge": (ctypes.c_int, [_PP, _P, _P, _P, ctypes.c_float, ctypes.c_double, _P, _P, _P, _P, _SZ, _P]),
     "kvp_think_prune": (ctypes.c_int, [_PP, _P, _P, _I, _I, _P, _P, _P, _SZ, _P]),
+    "kvp_finch_score": (ctypes.c_int, [_PP, _P, _P, _I, _I, _P, _P, _SZ, _P]),
+    "kvp_finch_compress": (ctypes.c_int, [_PP, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_scores_compress_chunked": (ctypes.c_int, [_PP, _P, _PI64, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -796,3 +800,68 @@ def think_prune(keys: torch.Tensor, q_window: torch.Tensor, n_pruned: int, retur
     _enqueue("kvp_think_prune", keys.device, make_problem(keys, keys, S, q_window.shape[1]), keys, q_window,
              q_window.shape[2], int(n_pruned), pruned, scores, scorer=SCORER_THINK)
     return keys, pruned, scores
+
+
+# --------------------------------------------------------------------------------------------------
+# Finch
+# --------------------------------------------------------------------------------------------------
+def chunk_counts(S: int, chunk_length: Optional[int], compression_ratio: float):
+    """(chunk_length, chunk_kept, tail_kept, n_kept) of FinchPress's selection: chunk_length 0 (None) keeps
+    int(S (1 - r)) of the row; otherwise each full chunk keeps max(1, int(L (1 - r))) and the short last chunk
+    max(1, int(len (1 - r))), as the reference's loop over chunks does."""
+    if not chunk_length:
+        return 0, 0, 0, int(S * (1 - compression_ratio))
+    L = int(chunk_length)
+    n_full, tail = divmod(S, L)
+    chunk_kept = max(1, int(L * (1 - compression_ratio))) if n_full else 0
+    tail_kept = max(1, int(tail * (1 - compression_ratio))) if tail else 0
+    return L, chunk_kept, tail_kept, n_full * chunk_kept + tail_kept
+
+
+def _inv_freq(inv_freq: Optional[torch.Tensor], keys: torch.Tensor) -> Optional[torch.Tensor]:
+    if inv_freq is None:
+        return None
+    if inv_freq.numel() * 2 != keys.shape[3]:
+        raise RuntimeError(f"inv_freq must have head_dim/2 = {keys.shape[3] // 2} entries, got {inv_freq.numel()}")
+    return inv_freq.to(device=keys.device, dtype=torch.float32).contiguous()
+
+
+def finch_score(keys, q_window, window: int, normalize: bool = True) -> torch.Tensor:
+    """FinchPress.score (include/kvpress_b200.h, kvp_finch_score): [B, Hkv, S] in the cache dtype, the window
+    positions holding the reference's max + 1 sentinel."""
+    _require_cuda_kv(keys, keys)
+    keys = _normalise(keys)
+    q_window = _check_q(q_window, keys, window)
+    p = make_problem(keys, keys, 0, q_window.shape[1])
+    return _score("kvp_finch_score", SCORER_FINCH, keys, p, keys, q_window, window, int(bool(normalize)))
+
+
+def finch_compress(keys, values, q_window, window: int, compression_ratio: float, chunk_length: Optional[int] = None,
+                   normalize: bool = True, inv_freq: Optional[torch.Tensor] = None, return_indices: bool = False,
+                   return_scores: bool = False):
+    """FinchPress.compress (kvp_finch_compress): the scores, the per-chunk selection (chunk_length None: the whole
+    row) and the compaction, the kept keys re-rotated to their new positions when inv_freq is given.
+    Returns (k_out, v_out, idx, scores)."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    q_window = _check_q(q_window, keys, window)
+    L, chunk_kept, tail_kept, n_kept = chunk_counts(keys.shape[2], chunk_length, compression_ratio)
+    return _compress("kvp_finch_compress", SCORER_FINCH, keys, values, n_kept,
+                     (keys, values, q_window, window, int(bool(normalize)), L, chunk_kept, tail_kept,
+                      _inv_freq(inv_freq, keys)), return_indices, return_scores, q_window.shape[1])
+
+
+def scores_compress_chunked(scores: torch.Tensor, keys, values, compression_ratio: float, chunk_length: int,
+                            inv_freq: Optional[torch.Tensor] = None, return_indices: bool = False):
+    """FinchPress's chunked selection on caller scores [B, Hkv, S] (kvp_scores_compress_chunked): each chunk of
+    chunk_length positions keeps its best max(1, int(len (1 - r))), the kept keys optionally re-rotated to their
+    new positions. Returns (k_out, v_out, idx)."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    scores, sstride = _caller_scores(scores, keys)
+    L, chunk_kept, tail_kept, n_kept = chunk_counts(keys.shape[2], chunk_length, compression_ratio)
+    if L < 1:
+        raise RuntimeError("scores_compress_chunked needs chunk_length >= 1")
+    return _compress("kvp_scores_compress_chunked", SCORER_FINCH, keys, values, n_kept,
+                     (scores, sstride, L, chunk_kept, tail_kept, keys, values, _inv_freq(inv_freq, keys)),
+                     return_indices)

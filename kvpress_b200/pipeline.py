@@ -19,6 +19,7 @@ from transformers.pipelines import PIPELINE_REGISTRY
 
 from kvpress_b200.presses.base_press import BasePress
 from kvpress_b200.presses.decoding_press import DecodingPress
+from kvpress_b200.presses.finch_press import FinchPress
 from kvpress_b200.presses.key_rerotation_press import KeyRerotationPress
 from kvpress_b200.presses.prefill_decoding_press import PrefillDecodingPress
 
@@ -106,8 +107,8 @@ class KVPressTextGenerationPipeline(Pipeline):
         answers = []
         with decode_ctx:
             for question_ids in input_tensors["questions_ids"]:
-                if isinstance(press, KeyRerotationPress):
-                    # pipeline.py:231-232 of the reference: the kept keys were re-rotated to positions
+                if isinstance(press, KeyRerotationPress) or (isinstance(press, FinchPress) and press.rerotate_keys):
+                    # pipeline.py:231-237 of the reference: the kept keys were re-rotated to positions
                     # 0..n_kept-1, so question and answer continue from the COMPRESSED length
                     context_length = cache.get_seq_length()
                 lengths_before = [cache.get_seq_length(i) for i in range(len(cache))]
