@@ -489,6 +489,239 @@ def rope_inv_freq(kind: str, D: int, seed: int = 0) -> torch.Tensor:
     return inv
 
 
+def scores64(k, q, w, normalize=True, rows=64):
+    """FinchPress: float64 [B, H, S - w] context scores, window rows in blocks."""
+    B, H, S, D = k.shape
+    G = q.shape[1] // H
+    kk = k.double()
+    qq = q.double().reshape(B, H, G, w, D)
+    col = torch.zeros(B, H, S - w, dtype=torch.float64, device=k.device)
+    pos = torch.arange(S, device=k.device)
+    for i0 in range(0, w, rows):
+        i1 = min(w, i0 + rows)
+        y = torch.einsum("bhgid,bhsd->bhgis", qq[:, :, :, i0:i1], kk) / math.sqrt(D)
+        rpos = torch.arange(S - w + i0, S - w + i1, device=k.device)
+        y.masked_fill_(pos[None, :] > rpos[:, None], float("-inf"))
+        p = torch.softmax(y, dim=-1)[..., : S - w]
+        if normalize:
+            p = p * rpos.double()[:, None]
+        col += p.sum(dim=(2, 3))
+    return col / (G * w)
+
+
+def assert_scores(got, k, q, w, normalize, what):
+    """FinchPress's bar (tests/test_gpu_finch.py): every context score within 1 ulp of the float64 value, the window
+    holding round(max + 1)."""
+    S = k.shape[2]
+    ref = scores64(k, q, w, normalize)
+    ctx = got[..., : S - w].double()
+    err = (ctx - ref).abs()
+    bound = ulp_at(ref, got.dtype)
+    bad = err > bound
+    assert not bad.any(), f"{what}: {int(bad.sum())} scores beyond 1 ulp, worst {float((err / bound).max())} ulp"
+    sentinel = (got[..., : S - w].float().max() + 1).to(got.dtype)
+    assert (got[..., S - w:] == sentinel).all(), f"{what}: window sentinel"
+
+
+# ---------------------------------------------------------------------------------------------------
+# the exact selection contract (tests/test_gpu_select_compact_sweep.py, tests/test_gpu_chunked_select_sweep.py)
+# ---------------------------------------------------------------------------------------------------
+INF_BITS = {torch.bfloat16: 0x7F80, torch.float16: 0x7C00}
+# kTile / kTileThreads of common.cuh (the select sweep's CPU test checks them against the source)
+TILE = 256
+TILE_THREADS = 256
+
+
+def copy_edges(u: int):
+    """copy_rows_kv<u> copies count·nvec vectors in steps of TILE_THREADS·u, two steps per loop iteration"""
+    step = TILE_THREADS * u
+    return (step, 2 * step)
+
+
+def edge_counts(nvec: int, u: int):
+    """kept counts of one tile whose count·nvec is the last multiple of nvec below, the first at or above, and the
+    first above each copy edge, where a tile can hold them; and 1 and a full tile"""
+    out = {1, TILE}
+    for e in copy_edges(u):
+        out |= {(e - 1) // nvec, -(-e // nvec), e // nvec + 1}
+    return sorted(c for c in out if 1 <= c <= TILE)
+
+
+def key16(bits: torch.Tensor, dtype) -> torch.Tensor:
+    """`ordered_key16` restated on int64, only to place n_kept at the kernels' bin edges (never to judge a result)"""
+    b = bits.long() & 0xFFFF
+    nan = (b & 0x7FFF) > INF_BITS[dtype]
+    b = torch.where(b == 0x8000, 0, b)
+    key = torch.where(b >= 0x8000, (~b) & 0xFFFF, b | 0x8000)
+    return torch.where(nan, 0xFFFF, key)
+
+
+def oracle_key(scores: torch.Tensor) -> torch.Tensor:
+    """The ranking key of `O.select_lowest_index_ties`: float value, -0 == +0, every NaN above +inf"""
+    s = scores.float()
+    s = torch.where(s == 0, torch.zeros_like(s), s)
+    bits = s.contiguous().view(torch.int32).to(torch.int64)
+    key = torch.where(bits < 0, -(bits & 0x7FFFFFFF), bits)
+    return torch.where(torch.isnan(s), torch.full_like(key, 2 ** 40), key)
+
+
+def canonical_order(scores: torch.Tensor) -> torch.Tensor:
+    """positions of every row by descending score, equal scores in ascending position order"""
+    return torch.sort(oracle_key(scores), dim=-1, descending=True, stable=True).indices
+
+
+def canonical(order: torch.Tensor, n: int) -> torch.Tensor:
+    return torch.sort(order[..., :n], dim=-1).values
+
+
+def chunk_orders(scores: torch.Tensor, L: int):
+    """The canonical order of each full chunk of L positions ([..., n_full, L], None without one) and of the short last
+    chunk ([..., S % L], None without one), positions relative to the chunk's start."""
+    S = scores.shape[-1]
+    n_full = S // L
+    full = canonical_order(scores[..., : n_full * L].unflatten(-1, (n_full, L))) if n_full else None
+    tail = canonical_order(scores[..., n_full * L:]) if S % L else None
+    return full, tail
+
+
+def chunked_from_orders(orders, L: int, chunk_kept: int, tail_kept: int) -> torch.Tensor:
+    """The chunked selection: chunk c holds positions [c L, min(S, (c + 1) L)); each full chunk keeps the canonical
+    top chunk_kept of its own scores, the short last chunk its top tail_kept, each ascending and offset by the chunk's
+    start, the chunks in order. int64 [..., n_full chunk_kept + tail_kept]."""
+    full, tail = orders
+    parts = []
+    if full is not None:
+        n_full = full.shape[-2]
+        kept = canonical(full, chunk_kept) + torch.arange(0, n_full * L, L, device=full.device)[:, None]
+        parts.append(kept.flatten(-2))
+    if tail is not None:
+        n_full = 0 if full is None else full.shape[-2]
+        parts.append(canonical(tail, tail_kept) + n_full * L)
+    return torch.cat(parts, dim=-1)
+
+
+def chunked_canonical(scores: torch.Tensor, L: int, chunk_kept: int, tail_kept: int) -> torch.Tensor:
+    return chunked_from_orders(chunk_orders(scores, L), L, chunk_kept, tail_kept)
+
+
+def chunked_oracle(scores: torch.Tensor, L: int, chunk_kept: int, tail_kept: int) -> torch.Tensor:
+    """`O.select_lowest_index_ties` applied chunk by chunk on the CPU (slow: one call per chunk)"""
+    S = scores.shape[-1]
+    s = scores.cpu()
+    parts = []
+    for lo in range(0, S, L):
+        hi = min(S, lo + L)
+        parts.append(O.select_lowest_index_ties(s[..., lo:hi], chunk_kept if hi - lo == L else tail_kept) + lo)
+    return torch.cat(parts, dim=-1)
+
+
+def all_patterns(dtype) -> torch.Tensor:
+    return torch.arange(-32768, 32768, dtype=torch.int32).to(torch.int16).view(dtype)
+
+
+def key_space_n_kept(keys: torch.Tensor, dtype):
+    """n_kept at every high-byte boundary c_b = #{key >> 8 >= b} and c_b +- 1, at every low-byte boundary of the bins
+    of NaN, +inf, -inf, +-0 and the subnormals, and 1, S - 1, S"""
+    S = keys.numel()
+    hi = keys >> 8
+    ns = {1, S - 1, S}
+    for b in range(256):
+        c = int((hi >= b).sum())
+        ns |= {c - 1, c, c + 1}
+    inf = INF_BITS[dtype]
+    special = torch.tensor([0xFFFF, 0x8000 | inf, (~(0x8000 | inf)) & 0xFFFF], dtype=torch.int64)  # NaN, +inf, -inf
+    sub = torch.arange(1, 1 << (10 if dtype == torch.float16 else 7))
+    bins = set((special >> 8).tolist()) | set((key16(torch.cat([sub, sub | 0x8000, torch.tensor([0])]), dtype) >> 8).tolist())
+    for b in bins:
+        for lo in range(256):
+            ns.add(int((keys >= (b << 8 | lo)).sum()))
+    return sorted(n for n in ns if 1 <= n <= S)
+
+
+def _pattern_keys(dtype):
+    pats = all_patterns(dtype).view(torch.int16)
+    return pats, key16(pats, dtype)
+
+
+def threshold_patterns(kind: str, dtype) -> torch.Tensor:
+    """the bit patterns of one threshold key (several for NaN and zero)"""
+    pats, keys = _pattern_keys(dtype)
+    inf = INF_BITS[dtype]
+    if kind == "neg_inf":
+        t = keys[pats.long() == (inf | 0x8000) - 65536]
+    elif kind == "most_negative":
+        t = keys[pats.long() == ((inf - 1) | 0x8000) - 65536]
+    elif kind == "nan":
+        t = torch.tensor([0xFFFF])
+    elif kind == "zero_mixed_sign":
+        t = torch.tensor([0x8000])
+    elif kind == "key_lo00":  # a negative value whose key ends in 0x00
+        t = torch.tensor([0x4000])
+    else:  # key_loff: a positive value whose key ends in 0xFF
+        t = torch.tensor([0xBFFF])
+    return pats[keys == int(t[0])]
+
+
+def rand_bits(shape, gen, dtype) -> torch.Tensor:
+    return torch.randint(-32768, 32768, tuple(shape), generator=gen, device=DEV, dtype=torch.int16).view(dtype)
+
+
+def mixed_scores(shape, dtype, gen) -> torch.Tensor:
+    """random bit patterns, half of them replaced by a few tied values: +-0, -inf, two NaN payloads, 1, -1"""
+    x = rand_bits(shape, gen, dtype)
+    pool = torch.tensor([0, -0.0, float("-inf"), 1.0, -1.0], dtype=dtype, device=DEV).view(torch.int16)
+    pool = torch.cat([pool, torch.tensor([INF_BITS[dtype] + 1, -1], dtype=torch.int16, device=DEV)]).view(dtype)
+    pick = torch.randint(0, pool.numel(), tuple(shape), generator=gen, device=DEV)
+    tied = torch.rand(tuple(shape), generator=gen, device=DEV) < 0.5
+    return torch.where(tied, pool[pick], x)
+
+
+def kv_for(B, H, S, D, dtype, gen):
+    """K, V of random bit patterns (NaN payloads included), and finite keys for the re-rotating call"""
+    return (rand_bits((B, H, S, D), gen, dtype), rand_bits((B, H, S, D), gen, dtype),
+            torch.randn(B, H, S, D, generator=gen, device=DEV).to(dtype))
+
+
+def _poison(*nbytes) -> set:
+    """Allocates blocks of these sizes in this order, fills them with 0xFF and frees them: the caching allocator hands
+    the same blocks to allocations of the same sizes in the same order. Returns their addresses."""
+    blocks = [torch.empty(n, dtype=torch.uint8, device=DEV) for n in nbytes if n > 0]
+    for b in blocks:
+        b.fill_(0xFF)
+    return {b.data_ptr() for b in blocks}
+
+
+def _landed(ptrs: set, *outs):
+    for o in outs:
+        if o is not None and o.numel() > 0:
+            assert o.data_ptr() in ptrs, "an output did not land on a poisoned block"
+
+
+def _score_copy_bytes(scores, dtype) -> int:
+    """bytes of the copy the binding makes of scores it cannot pass as they are (other dtype, or S not unit-stride)"""
+    if scores.dtype != dtype:
+        return scores.numel() * 2 + (scores.numel() * 2 if scores.stride(2) != 1 else 0)
+    return scores.numel() * 2 if scores.stride(2) != 1 else 0
+
+
+def _kv_out_bytes(k, n):
+    B, H, _, D = k.shape
+    return [B * H * n * D * 2] * 2 + [B * H * n * 4]
+
+
+def assert_idx(idx, want, what):
+    assert idx.dtype == torch.int32, f"{what}: idx is {idx.dtype}"
+    if not torch.equal(idx.long(), want):
+        bad = (idx.long() != want).nonzero()
+        i = bad[0].tolist()
+        raise AssertionError(f"{what}: {bad.shape[0]} of {want.numel()} kept positions differ from the canonical "
+                             f"selection, first at {i}: got {int(idx[tuple(i)])}, want {int(want[tuple(i)])}")
+
+
+def assert_gather(out, x, want, what):
+    assert torch.equal(_bits(out), _bits(_gather(x, want))), f"{what}: not a bitwise gather"
+
+
 def rerotation_admissible(k: torch.Tensor, idx: torch.Tensor, inv_freq: torch.Tensor) -> torch.Tensor:
     """[4, B, H, n, D]: k[idx] rotated by (j - idx_j) * inv_freq with every admissible (cos16, sin16) pair."""
     dtype, D = k.dtype, k.shape[-1]

@@ -16,7 +16,7 @@ import pytest
 import torch
 
 from kvpress_b200 import FinchPress, KVPressTextGenerationPipeline, finch_wide_head, native
-from tests.gpu_support import _gather, _same, rerotation_admissible, rope_inv_freq, tiny_gpu_llama
+from tests.gpu_support import _gather, _same, assert_scores, rerotation_admissible, rope_inv_freq, tiny_gpu_llama
 from tests.tiny_models import word_tokenizer, words
 
 pytestmark = pytest.mark.gpu
@@ -30,44 +30,6 @@ def inputs(B, H, G, S, D, w, dtype, seed=0):
     q = (torch.randn(B, H * G, w, D, generator=g, device=DEV) * 1.5).to(dtype)
     v = torch.randn(B, H, S, D, generator=g, device=DEV).to(dtype)
     return k, v, q
-
-
-def scores64(k, q, w, normalize=True, rows=64):
-    """float64 [B, H, S - w] context scores, window rows in blocks."""
-    B, H, S, D = k.shape
-    G = q.shape[1] // H
-    kk = k.double()
-    qq = q.double().reshape(B, H, G, w, D)
-    col = torch.zeros(B, H, S - w, dtype=torch.float64, device=k.device)
-    pos = torch.arange(S, device=k.device)
-    for i0 in range(0, w, rows):
-        i1 = min(w, i0 + rows)
-        y = torch.einsum("bhgid,bhsd->bhgis", qq[:, :, :, i0:i1], kk) / math.sqrt(D)
-        rpos = torch.arange(S - w + i0, S - w + i1, device=k.device)
-        y.masked_fill_(pos[None, :] > rpos[:, None], float("-inf"))
-        p = torch.softmax(y, dim=-1)[..., : S - w]
-        if normalize:
-            p = p * rpos.double()[:, None]
-        col += p.sum(dim=(2, 3))
-    return col / (G * w)
-
-
-def ulp(x, dtype):
-    m = torch.finfo(dtype).tiny
-    e = torch.floor(torch.log2(x.abs().clamp_min(m)))
-    return torch.exp2(e - (7 if dtype == BF16 else 10))
-
-
-def assert_scores(got, k, q, w, normalize, what):
-    S = k.shape[2]
-    ref = scores64(k, q, w, normalize)
-    ctx = got[..., : S - w].double()
-    err = (ctx - ref).abs()
-    bound = ulp(ref, got.dtype)
-    bad = err > bound
-    assert not bad.any(), f"{what}: {int(bad.sum())} scores beyond 1 ulp, worst {float((err / bound).max())} ulp"
-    sentinel = (got[..., : S - w].float().max() + 1).to(got.dtype)
-    assert (got[..., S - w:] == sentinel).all(), f"{what}: window sentinel"
 
 
 def chunked_topk(scores, w, L, ratio):

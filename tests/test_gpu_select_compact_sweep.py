@@ -43,17 +43,18 @@ import pytest
 import torch
 
 from oracle import press_oracle as O
-from tests.gpu_support import _name, _native, rerotation_admissible, rope_inv_freq, _sm_count
+from tests.gpu_support import (INF_BITS, TILE, TILE_THREADS, _bits, _kv_out_bytes, _landed, _name, _native, _poison,
+                               _score_copy_bytes, _sm_count, all_patterns, assert_gather, assert_idx,
+                               canonical, canonical_order, copy_edges, edge_counts, key16, kv_for, mixed_scores,
+                               key_space_n_kept, oracle_key, rand_bits, rerotation_admissible, rope_inv_freq,
+                               threshold_patterns, _pattern_keys)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
 CSRC = Path(__file__).resolve().parent.parent / "kvpress_b200" / "csrc"
 DTYPES = [torch.bfloat16, torch.float16]
-INF_BITS = {torch.bfloat16: 0x7F80, torch.float16: 0x7C00}
 
 # the constants of common.cuh / select_compact.cu the boundary lists are derived from (checked by a CPU test)
-TILE = 256          # kTile: positions per select / compact tile
-TILE_THREADS = 256  # kTileThreads
 SFX_STRIDE = 264    # kSfxStride
 TILES_PER_WARP = 2  # kTilesPerWarp
 GROUP_TILES = TILE_THREADS // 32 * TILES_PER_WARP  # kGroupTiles: tiles per refine item
@@ -64,21 +65,6 @@ STREAM_U = 4        # copy_rows_kv<4> of streaming_compact_kernel
 MAX_ROWS = 65535    # B·Hkv: gridDim.y of the score kernels
 
 
-def copy_edges(u: int):
-    """copy_rows_kv<u> copies count·nvec vectors in steps of TILE_THREADS·u, two steps per loop iteration"""
-    step = TILE_THREADS * u
-    return (step, 2 * step)
-
-
-def edge_counts(nvec: int, u: int):
-    """kept counts of one tile whose count·nvec is the last multiple of nvec below, the first at or above, and the
-    first above each copy edge, where a tile can hold them; and 1 and a full tile"""
-    out = {1, TILE}
-    for e in copy_edges(u):
-        out |= {(e - 1) // nvec, -(-e // nvec), e // nvec + 1}
-    return sorted(c for c in out if 1 <= c <= TILE)
-
-
 SHAPE_TILES = (1, GROUP_TILES, GROUP_TILES + 1, 2 * GROUP_TILES, 2 * GROUP_TILES + 1)
 SHAPE_S = [1, 2] + [t * TILE + d for t in SHAPE_TILES for d in (-1, 0, 1)]
 HEAD_DIMS = list(range(8, 257, 8))
@@ -86,79 +72,8 @@ LAYOUTS = ["contiguous", "k_contiguous_v_bshd", "v_row_slice", "k_broadcast_head
 
 
 # ---------------------------------------------------------------------------------------------------
-# keys and the reference
+# calls: poisoned outputs (tests/gpu_support.py _poison), workspace check
 # ---------------------------------------------------------------------------------------------------
-def key16(bits: torch.Tensor, dtype) -> torch.Tensor:
-    """`ordered_key16` restated on int64, only to place n_kept at the kernels' bin edges (never to judge a result)"""
-    b = bits.long() & 0xFFFF
-    nan = (b & 0x7FFF) > INF_BITS[dtype]
-    b = torch.where(b == 0x8000, 0, b)
-    key = torch.where(b >= 0x8000, (~b) & 0xFFFF, b | 0x8000)
-    return torch.where(nan, 0xFFFF, key)
-
-
-def oracle_key(scores: torch.Tensor) -> torch.Tensor:
-    """The ranking key of `O.select_lowest_index_ties`: float value, -0 == +0, every NaN above +inf"""
-    s = scores.float()
-    s = torch.where(s == 0, torch.zeros_like(s), s)
-    bits = s.contiguous().view(torch.int32).to(torch.int64)
-    key = torch.where(bits < 0, -(bits & 0x7FFFFFFF), bits)
-    return torch.where(torch.isnan(s), torch.full_like(key, 2 ** 40), key)
-
-
-def canonical_order(scores: torch.Tensor) -> torch.Tensor:
-    """positions of every row by descending score, equal scores in ascending position order"""
-    return torch.sort(oracle_key(scores), dim=-1, descending=True, stable=True).indices
-
-
-def canonical(order: torch.Tensor, n: int) -> torch.Tensor:
-    return torch.sort(order[..., :n], dim=-1).values
-
-
-def all_patterns(dtype) -> torch.Tensor:
-    return torch.arange(-32768, 32768, dtype=torch.int32).to(torch.int16).view(dtype)
-
-
-def _bits(x: torch.Tensor) -> torch.Tensor:
-    return x.contiguous().view(torch.int16)
-
-
-def _gather(x, idx):
-    return x.gather(2, idx.long().unsqueeze(-1).expand(-1, -1, -1, x.shape[-1]))
-
-
-def rand_bits(shape, gen, dtype) -> torch.Tensor:
-    return torch.randint(-32768, 32768, tuple(shape), generator=gen, device=DEV, dtype=torch.int16).view(dtype)
-
-
-def mixed_scores(shape, dtype, gen) -> torch.Tensor:
-    """random bit patterns, half of them replaced by a few tied values: +-0, -inf, two NaN payloads, 1, -1"""
-    x = rand_bits(shape, gen, dtype)
-    pool = torch.tensor([0, -0.0, float("-inf"), 1.0, -1.0], dtype=dtype, device=DEV).view(torch.int16)
-    pool = torch.cat([pool, torch.tensor([INF_BITS[dtype] + 1, -1], dtype=torch.int16, device=DEV)]).view(dtype)
-    pick = torch.randint(0, pool.numel(), tuple(shape), generator=gen, device=DEV)
-    tied = torch.rand(tuple(shape), generator=gen, device=DEV) < 0.5
-    return torch.where(tied, pool[pick], x)
-
-
-# ---------------------------------------------------------------------------------------------------
-# calls: poisoned outputs, workspace check
-# ---------------------------------------------------------------------------------------------------
-def _poison(*nbytes) -> set:
-    """Allocates blocks of these sizes in this order, fills them with 0xFF and frees them: the caching allocator hands
-    the same blocks to allocations of the same sizes in the same order. Returns their addresses."""
-    blocks = [torch.empty(n, dtype=torch.uint8, device=DEV) for n in nbytes if n > 0]
-    for b in blocks:
-        b.fill_(0xFF)
-    return {b.data_ptr() for b in blocks}
-
-
-def _landed(ptrs: set, *outs):
-    for o in outs:
-        if o is not None and o.numel() > 0:
-            assert o.data_ptr() in ptrs, "an output did not land on a poisoned block"
-
-
 def _select_problem(nat, scores, n):
     B, H, S = scores.shape
     p = nat.KvpProblem()
@@ -171,13 +86,6 @@ def _check_ws(nat, p, scorer=None):
     nat.workspace_check(p, scorer, nat._workspace(p, scorer, torch.device(DEV)))
 
 
-def _score_copy_bytes(scores, dtype) -> int:
-    """bytes of the copy the binding makes of scores it cannot pass as they are (other dtype, or S not unit-stride)"""
-    if scores.dtype != dtype:
-        return scores.numel() * 2 + (scores.numel() * 2 if scores.stride(2) != 1 else 0)
-    return scores.numel() * 2 if scores.stride(2) != 1 else 0
-
-
 def call_select(nat, scores, n, check=True):
     """`check`: workspace_check after the call (it synchronises the stream)"""
     B, H, _ = scores.shape
@@ -187,11 +95,6 @@ def call_select(nat, scores, n, check=True):
     if n and check:
         _check_ws(nat, _select_problem(nat, scores, n))
     return idx
-
-
-def _kv_out_bytes(k, n):
-    B, H, _, D = k.shape
-    return [B * H * n * D * 2] * 2 + [B * H * n * 4]
 
 
 def call_compress(nat, scores, k, v, n, inv=None, check=True):
@@ -211,19 +114,6 @@ def call_streaming(nat, k, v, n, n_sink):
     out = nat.streaming_compress(k, v, n, n_sink, return_indices=True)
     _landed(ptrs, *out)
     return out
-
-
-def assert_idx(idx, want, what):
-    assert idx.dtype == torch.int32, f"{what}: idx is {idx.dtype}"
-    if not torch.equal(idx.long(), want):
-        bad = (idx.long() != want).nonzero()
-        i = bad[0].tolist()
-        raise AssertionError(f"{what}: {bad.shape[0]} of {want.numel()} kept positions differ from the canonical "
-                             f"selection, first at {i}: got {int(idx[tuple(i)])}, want {int(want[tuple(i)])}")
-
-
-def assert_gather(out, x, want, what):
-    assert torch.equal(_bits(out), _bits(_gather(x, want))), f"{what}: not a bitwise gather"
 
 
 def assert_rerotated(k_out, k, want, inv, what):
@@ -252,12 +142,6 @@ def check_entry_points(scores, k, v, kr, ns, what, order=None, inv=None):
             assert_idx(idx, want, w + " scores_compress_rerotate")
             assert_gather(v_out, v, want, w + " rerotate V'")
             assert_rerotated(k_out, kr, want, inv, w + " rerotate")
-
-
-def kv_for(B, H, S, D, dtype, gen):
-    """K, V of random bit patterns (NaN payloads included), and finite keys for the re-rotating call"""
-    return (rand_bits((B, H, S, D), gen, dtype), rand_bits((B, H, S, D), gen, dtype),
-            torch.randn(B, H, S, D, generator=gen, device=DEV).to(dtype))
 
 
 def n_kept_values(S: int):
@@ -383,23 +267,6 @@ def test_reference_shortcut_is_the_oracle():
 # ---------------------------------------------------------------------------------------------------
 # 1. the whole key space
 # ---------------------------------------------------------------------------------------------------
-def key_space_n_kept(keys: torch.Tensor, dtype):
-    """n_kept at every high-byte boundary c_b = #{key >> 8 >= b} and c_b +- 1, at every low-byte boundary of the bins
-    of NaN, +inf, -inf, +-0 and the subnormals, and 1, S - 1, S"""
-    S = keys.numel()
-    hi = keys >> 8
-    ns = {1, S - 1, S}
-    for b in range(256):
-        c = int((hi >= b).sum())
-        ns |= {c - 1, c, c + 1}
-    inf = INF_BITS[dtype]
-    special = torch.tensor([0xFFFF, 0x8000 | inf, (~(0x8000 | inf)) & 0xFFFF], dtype=torch.int64)  # NaN, +inf, -inf
-    sub = torch.arange(1, 1 << (10 if dtype == torch.float16 else 7))
-    bins = set((special >> 8).tolist()) | set((key16(torch.cat([sub, sub | 0x8000, torch.tensor([0])]), dtype) >> 8).tolist())
-    for b in bins:
-        for lo in range(256):
-            ns.add(int((keys >= (b << 8 | lo)).sum()))
-    return sorted(n for n in ns if 1 <= n <= S)
 
 
 @gpu
@@ -425,30 +292,6 @@ PLANT_S = 3 * GROUP_TILES * TILE - 77  # 3 refine groups, the last partial; the 
 THRESHOLDS = ["neg_inf", "most_negative", "nan", "key_lo00", "key_loff", "zero_mixed_sign"]
 PLACEMENTS = ["straddle_tile_and_group", "first_tile_only", "last_tile_only"]
 PLANTED = [(t, p, dt) for t in THRESHOLDS for p in PLACEMENTS for dt in DTYPES]
-
-
-def _pattern_keys(dtype):
-    pats = all_patterns(dtype).view(torch.int16)
-    return pats, key16(pats, dtype)
-
-
-def threshold_patterns(kind: str, dtype) -> torch.Tensor:
-    """the bit patterns of one threshold key (several for NaN and zero)"""
-    pats, keys = _pattern_keys(dtype)
-    inf = INF_BITS[dtype]
-    if kind == "neg_inf":
-        t = keys[pats.long() == (inf | 0x8000) - 65536]
-    elif kind == "most_negative":
-        t = keys[pats.long() == ((inf - 1) | 0x8000) - 65536]
-    elif kind == "nan":
-        t = torch.tensor([0xFFFF])
-    elif kind == "zero_mixed_sign":
-        t = torch.tensor([0x8000])
-    elif kind == "key_lo00":  # a negative value whose key ends in 0x00
-        t = torch.tensor([0x4000])
-    else:  # key_loff: a positive value whose key ends in 0xFF
-        t = torch.tensor([0xBFFF])
-    return pats[keys == int(t[0])]
 
 
 def planted_row(kind, placement, dtype, gen, n_t=40):
