@@ -1,5 +1,6 @@
 """Helpers shared by the GPU tests: the library, the float64 references and input generators of the scorers, and the
 bars their kernels are held to (each bar is described in the module docstring of the test file that states it)."""
+import ctypes
 import math
 import re
 from pathlib import Path
@@ -36,6 +37,47 @@ def tiny_gpu_llama(head_dim=64):
 
 def gpu_ids(n=240):
     return distinct_ids(n, seed=11, device=DEV)
+
+
+# ---------------------------------------------------------------------------------------------------
+# the launchers' dispatch and schedule rules (expected_attention.cu: launch_ea_t, snapkv.cu: launch_snap_t)
+# ---------------------------------------------------------------------------------------------------
+def ea_instantiation(dtype, D: int, G: int):
+    """<T, D, GR> of ea_logits_kernel: GR query heads resident per unit."""
+    gr = 4 if G % 4 == 0 else (1 if G == 1 else 2)
+    return (_name(dtype), D, gr)
+
+
+def snap_parts(R: int, S: int, window: int, sm: int):
+    """(ctas_per_row, parts holding tiles in pass 1, in pass 2) of launch_snap_t's row split."""
+    n_tiles = (S + 127) // 128
+    cpr = max(1, min(sm // R, n_tiles, 640))
+    used = []
+    for n in (n_tiles, min(n_tiles, (S - window + 127) // 128)):
+        per = (n + cpr - 1) // cpr
+        used.append((n + per - 1) // per)
+    return cpr, used[0], used[1]
+
+
+def ea_schedule(R: int, G: int, S: int):
+    """CTA item ranges and per-unit (first CTA, CTA count) of the ExpectedAttention launch, from the library's own
+    partition (kvp_debug_ea_pair_partition) and the launcher's worker count."""
+    lib = ctypes.CDLL(str(_native().library_path()))
+    fn = lib.kvp_debug_ea_pair_partition
+    fn.restype = ctypes.c_int
+    fn.argtypes = [ctypes.c_int] * 5 + [ctypes.POINTER(ctypes.c_longlong)]
+    gr = ea_instantiation(torch.bfloat16, 128, G)[2]
+    n_units, n_tp = R * ((G + gr - 1) // gr), (S + 127) // 128
+    n_workers = min(_sm_count(), 160, n_units * n_tp)
+    out = (ctypes.c_longlong * 4)()
+    ranges, spans = [], []
+    for p in range(n_workers):
+        assert fn(n_units, n_tp, n_workers, p, 0, out) == 0
+        ranges.append((out[0], out[1]))
+    for u in range(n_units):
+        assert fn(n_units, n_tp, n_workers, 0, u, out) == 0
+        spans.append((out[2], out[3]))
+    return n_tp, n_workers, ranges, spans
 
 
 UNIT_ROUNDOFF = {torch.bfloat16: 2.0 ** -7, torch.float16: 2.0 ** -10}

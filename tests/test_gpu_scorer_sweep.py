@@ -15,7 +15,6 @@ Measured on an H100 80GB HBM3 (132 SMs, 700 W power limit) over every case of th
 rounded fp64 score; at most 4e-4 of a case's positions at 1 ulp for ExpectedAttention and 2.1e-3 for SnapKV (fp16,
 window 1); the worst row bias is 0.30 of its bound. Each bar is asserted as stated above, not at the measured values.
 """
-import ctypes
 import re
 from pathlib import Path
 
@@ -23,8 +22,9 @@ import pytest
 import torch
 
 from oracle import press_oracle as O
-from tests.gpu_support import (assert_compress, assert_vs_ref64, ea_inputs, ea_ref64, _forced_head, _forced_tail,
-                               _gather, _layout, LAYOUTS, _name, _native, _sm_count, snap_inputs, snap_ref64)
+from tests.gpu_support import (assert_compress, assert_vs_ref64, ea_inputs, ea_instantiation, ea_ref64, ea_schedule,
+                               _forced_head, _forced_tail, _gather, _layout, LAYOUTS, _name, _native, _sm_count,
+                               snap_inputs, snap_parts, snap_ref64)
 
 gpu = pytest.mark.gpu
 DEV = "cuda:0"
@@ -35,28 +35,11 @@ DTYPES = [torch.bfloat16, torch.float16]
 # ---------------------------------------------------------------------------------------------------
 # the launchers' dispatch rules (expected_attention.cu: launch_ea_t, snapkv.cu: launch_snap_d / launch_snap_t)
 # ---------------------------------------------------------------------------------------------------
-def ea_instantiation(dtype, D: int, G: int):
-    """<T, D, GR> of ea_logits_kernel: GR query heads resident per unit."""
-    gr = 4 if G % 4 == 0 else (1 if G == 1 else 2)
-    return (_name(dtype), D, gr)
-
-
 def snap_instantiation(dtype, D: int, G: int, window: int):
     """<T, D, NQP> of snap_stats_kernel / snap_colsum_kernel: the G * window query rows padded to 128 / 256 / 512."""
     nq = G * window
     nqp = 128 if nq <= 128 else (256 if nq <= 256 else 512)
     return (_name(dtype), D, nqp)
-
-
-def snap_parts(R: int, S: int, window: int, sm: int):
-    """(ctas_per_row, parts holding tiles in pass 1, in pass 2) of launch_snap_t's row split."""
-    n_tiles = (S + 127) // 128
-    cpr = max(1, min(sm // R, n_tiles, 640))
-    used = []
-    for n in (n_tiles, min(n_tiles, (S - window + 127) // 128)):
-        per = (n + cpr - 1) // cpr
-        used.append((n + per - 1) // per)
-    return cpr, used[0], used[1]
 
 
 # the instantiation sweep: (dtype, D, G) for ExpectedAttention, (dtype, D, G, window) for SnapKV
@@ -241,27 +224,6 @@ def test_snapkv_press_window_300_on_a_multi_head_llama():
 # ---------------------------------------------------------------------------------------------------
 # 3. persistent schedules: each shape asserts the regime it is meant to reach on this device
 # ---------------------------------------------------------------------------------------------------
-def ea_schedule(R: int, G: int, S: int):
-    """CTA item ranges and per-unit (first CTA, CTA count) of the ExpectedAttention launch, from the library's own
-    partition (kvp_debug_ea_pair_partition) and the launcher's worker count."""
-    lib = ctypes.CDLL(str(_native().library_path()))
-    fn = lib.kvp_debug_ea_pair_partition
-    fn.restype = ctypes.c_int
-    fn.argtypes = [ctypes.c_int] * 5 + [ctypes.POINTER(ctypes.c_longlong)]
-    gr = ea_instantiation(torch.bfloat16, 128, G)[2]
-    n_units, n_tp = R * ((G + gr - 1) // gr), (S + 127) // 128
-    n_workers = min(_sm_count(), 160, n_units * n_tp)
-    out = (ctypes.c_longlong * 4)()
-    ranges, spans = [], []
-    for p in range(n_workers):
-        assert fn(n_units, n_tp, n_workers, p, 0, out) == 0
-        ranges.append((out[0], out[1]))
-    for u in range(n_units):
-        assert fn(n_units, n_tp, n_workers, 0, u, out) == 0
-        spans.append((out[2], out[3]))
-    return n_tp, n_workers, ranges, spans
-
-
 def _crosses(lo, hi, n_tp):
     """the range [lo, hi) holds items of more than one unit"""
     return lo // n_tp != (hi - 1) // n_tp
