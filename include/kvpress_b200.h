@@ -20,6 +20,7 @@
  *     kvp_cur_*                <- kvpress/presses/cur_press.py (approximate K / V leverage scores, from K and V only)
  *     kvp_merging_*            <- kvpress/presses/merging_press.py (evicted values folded into their nearest kept row)
  *     kvp_think_prune          <- kvpress/presses/think_press.py (key channels zeroed in place; no positions removed)
+ *     kvp_cam_compress         <- kvpress/presses/cam_press.py (evicted values merged into the kept rows after them)
  *     kvp_scores_compress      <- scorer_press.py:93-100 for an arbitrary score tensor
  *                                 (what wrapper presses / user ScorerPress subclasses need)
  *
@@ -86,7 +87,8 @@ typedef enum kvp_scorer {
     KVP_SCORER_CUR = 11,
     KVP_SCORER_MERGING = 13, /* kvp_merging_*: the selection of the caller's scores, then the merge */
     KVP_SCORER_THINK = 14,   /* kvp_think_prune: key channels, not positions */
-    KVP_SCORER_FINCH = 16    /* kvp_finch_*, kvp_scores_compress_chunked */
+    KVP_SCORER_FINCH = 16,   /* kvp_finch_*, kvp_scores_compress_chunked */
+    KVP_SCORER_CAM = 17      /* kvp_cam_compress */
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -460,6 +462,67 @@ kvp_status kvp_scores_compress_chunked(const kvp_problem* p, const void* scores,
                                        const void* V, const float* inv_freq, void* K_out, void* V_out,
                                        int32_t* idx_out, void* workspace, size_t workspace_bytes,
                                        kvp_stream_t stream);
+
+/* ---- CAMPress (kvpress/presses/cam_press.py, CaM, https://openreview.net/forum?id=LCTmppB165) ----------------------
+ * DecodingPress's compaction with merge-before-prune: some evicted values are folded into the kept rows that follow
+ * them, with a probability set by the running sum of the attention each position received while decoding. One
+ * compaction of one layer, per batch element b (all kv heads share one selection, as in the reference), with the
+ * base press's scores [B, Hkv, S] (cache dtype), the fp32 running sum A [B, Hkv, S], n_kept = target_size,
+ * n_merge = min(k, S - n_kept) (k: the layer's steps since its last compaction), merge_budget >= 1 and caller uniforms
+ * u [B, Hkv, n_merge] in [0, 1):
+ *   1. m[s] = (sum of the Hkv scores in ascending head order, fp32) / Hkv, rounded once to the cache dtype.
+ *   2. kept: the n_kept largest m, ranked as kvp_scores_compress ranks 16-bit keys (NaN above every number, -0 == +0),
+ *      ties to the LOWEST positions; kept[0 .. n_kept) ascending. evicted: exactly the other S - n_kept positions.
+ *   3. candidates: the n_merge evicted positions ranked first by (m descending, position descending), NaN above every
+ *      number (the reference's flip + stable argsort: ties go to the LATER position; under StreamingLLM every evicted
+ *      m is 0 and the candidates are the n_merge evicted positions just before the recent window); e[0 .. n_merge)
+ *      ascending.
+ *   4. t_i = the number of kept positions below e_i; the window of candidate i is the kept ranks
+ *      [t_i, min(t_i + merge_budget, n_kept)), n_i its size (0 when e_i is above every kept position).
+ *   5. per head j: mean_i = (sum of A[kept[r]] over the window, ascending r, fp32) / max(n_i, 1);
+ *      p_i = A[e_i] / mean_i with NaN -> 0 (0 / 0: a zero running sum) and +inf -> 1 (a zero mean under a positive
+ *      A[e_i]), then clamped to [0, 1]; mask_i = u[b, j, i] < p_i, a Bernoulli(p_i) draw reproducible from u.
+ *   6. for each kept rank r: K_out[r] = K[kept[r]] and attn_out[r] = A[kept[r]] exactly;
+ *      V_out[r] = round(V[kept[r]] + sum of (mask_i / n_i) V[e_i] over the candidates whose window holds r, ascending i),
+ *      accumulated in fp32 from V[kept[r]], each term one fused multiply-add, rounded once to the cache dtype.
+ *   A row can receive far more than merge_budget terms: under StreamingLLM all n_merge candidates share one t_i, so
+ *   each of the first merge_budget recent rows receives all of them. The kernels assume no bound but n_merge.
+ * Deviations from the reference: the running sum is fp32, not the cache dtype; the evicted set is the complement of
+ * the kept set (the reference's two topk calls can make a tied position both kept and evicted, or neither); the merge
+ * sums are fp32, in a fixed order and rounded once, not a bf16 atomic scatter_add_; ties among the kept rows go to the
+ * lowest positions. With fp32 inputs the reference computes in fp32, and steps 1-6 agree with it to fp32 rounding.
+ * NaN / inf: a NaN score ranks above every number in both selections. A non-finite A gives p_i by the rules above. A
+ * non-finite evicted value reaches every row of its window even when its draw fails (0 * inf = NaN), as in the
+ * reference. Against the float64 definition (the same kept set, candidates and draws),
+ *   |V_out[r] - V64[r]| <= ulp(V64[r]) / 2 + (c_r + 2) 2^-24 (|V[kept[r]]| + sum of (mask_i / n_i) |V[e_i]|)
+ * elementwise, c_r being the number of terms of row r.
+ * Arguments:
+ *   scores      [B, Hkv, S] in K's dtype, element strides score_stride (b, h), s contiguous, 2-byte aligned.
+ *   attn_sum    fp32 [B, Hkv, S], element strides attn_stride (b, h), s contiguous: the view may sit in a capacity
+ *               buffer. attn_out likewise [B, Hkv, n_kept] with attn_out_stride; it must not overlap attn_sum.
+ *   uniforms    fp32 [B, Hkv, n_merge] contiguous; may be null when n_merge == 0.
+ *   K_out, V_out contiguous [B, Hkv, n_kept, D].
+ *   idx_out     nullable, int32 [B, n_kept]: the kept positions, ascending.
+ *   merge_idx_out nullable, int32 [B, n_merge]: the candidates e, ascending.
+ *   merge_prob_out nullable, fp32 [B, Hkv, n_merge]: p_i.
+ * Every head_dim the problem validates. Indexing is 64-bit. Every sum has a fixed order: two calls give bitwise-equal
+ * results, and a row's results do not depend on the batch, the SM count or the strides.
+ * Check order (the first failure is returned): validate the problem -> n_kept == 0 returns KVP_OK and enqueues nothing
+ * -> K / V / K_out / V_out null and 16-byte alignment -> scores, score_stride, attn_sum, attn_stride, attn_out,
+ * attn_out_stride null, uniforms null with n_merge != 0 -> scores 2-byte and attn_sum, attn_out, uniforms, idx_out,
+ * merge_idx_out, merge_prob_out 4-byte alignment -> merge_budget < 1 or n_merge outside [0, S - n_kept] gives
+ * KVP_ERR_BAD_ARGUMENT -> workspace null -> its 16-byte alignment -> its size.
+ * kvp_workspace_bytes(KVP_SCORER_CAM) does not depend on n_merge or merge_budget: the selection regions of B rows
+ * (kvp_scores_select's for a [B, 1, S] problem), then 4 B n_kept (kept positions) + 4 B (S - n_kept) twice
+ * (candidates, t) + 4 B Hkv (S - n_kept) (weights mask_i / n_i), each region rounded up to 256 bytes. A call takes 6
+ * launches (memset, head mean + keys, select, candidates, probabilities, merge + compaction), 4 when n_merge == 0.
+ * Memory beyond the workspace: none.
+ * The return type is kvp_status, an int-sized enum with the values of every other entry point's int. */
+kvp_status kvp_cam_compress(const kvp_problem* p, const void* scores, const int64_t* score_stride, const void* K,
+                            const void* V, const float* attn_sum, const int64_t* attn_stride, int32_t n_merge,
+                            int32_t merge_budget, const float* uniforms, void* K_out, void* V_out, float* attn_out,
+                            const int64_t* attn_out_stride, int32_t* idx_out, int32_t* merge_idx_out,
+                            float* merge_prob_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

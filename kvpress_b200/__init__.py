@@ -7,6 +7,7 @@ from kvpress_b200.pipeline import KVPressTextGenerationPipeline
 from kvpress_b200.presses.adakv_press import AdaKVPress
 from kvpress_b200.presses.base_press import SUPPORTED_MODELS, BasePress
 from kvpress_b200.presses.block_press import BlockPress
+from kvpress_b200.presses.cam_press import CAMPress
 from kvpress_b200.presses.chunk_press import ChunkPress
 from kvpress_b200.presses.chunkkv_press import ChunkKVPress
 from kvpress_b200.presses.composed_press import ComposedPress
@@ -48,6 +49,7 @@ __all__ = [
     "StreamingLLMPress",
     "TOVAPress",
     "DecodingPress",
+    "CAMPress",
     "KeyRerotationPress",
     "KeyDiffPress",
     "AdaKVPress",

@@ -76,7 +76,8 @@ static int largest_window(const Dims& d, int scorer) {
 // query rows n_q of ObservedAttention. Returns the total bytes and, in *zeroed, the
 // leading bytes every call clears with one memset: the histograms, the counters and the tile prefixes. The
 // histograms are whole KiB per row, so hist_lo and the counters follow hist_hi without padding.
-static size_t layout(const Dims& d, int scorer, int window, void* base, Workspace* ws, size_t* zeroed) {
+static size_t layout(const Dims& d_call, int scorer, int window, void* base, Workspace* ws, size_t* zeroed) {
+    const Dims d = scorer == KVP_SCORER_CAM ? cam_selection_dims(d_call) : d_call;
     Carve c(base);
     ws->R = d.R;
     if (scorer == KVP_SCORER_THINK) {  // no selection of positions: the channel statistics alone (think.cu)
@@ -106,6 +107,7 @@ static size_t layout(const Dims& d, int scorer, int window, void* base, Workspac
                        : scorer == KVP_SCORER_CUR                  ? cur_scratch_bytes(d)
                        : scorer == KVP_SCORER_MERGING              ? merging_scratch_bytes(d)
                        : scorer == KVP_SCORER_FINCH                ? finch_scratch_bytes(d, window)
+                       : scorer == KVP_SCORER_CAM                  ? cam_scratch_bytes(d_call)
                                                                    : 0;
     ws->scorer = c.take<char>(ws->scorer_bytes);
     return c.bytes;
@@ -279,7 +281,7 @@ int kvp_workspace_check(const kvp_problem* p, int scorer, const void* workspace,
     if (scorer == KVP_SCORER_THINK) return KVP_OK;  // its kernels have no bounded waits
     uint32_t flag = 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    cudaError_t e = cudaMemcpyAsync(&flag, c.ws.counters + kCounterErrSlot(c.d.R), sizeof(flag),
+    cudaError_t e = cudaMemcpyAsync(&flag, c.ws.counters + kCounterErrSlot(c.ws.R), sizeof(flag),
                                     cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) return status(e);
@@ -319,6 +321,8 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         case KVP_SCORER_THINK: *launches_out = 3; break;  // memset, reduce + select, zero
         // unchunked: memset, stats, merge, column sums, finalize, select+compact (chunked: one more, see the header)
         case KVP_SCORER_FINCH: *launches_out = 6; break;
+        // memset, head mean + keys, select, candidates, probabilities, merge + compaction (4 when n_merge == 0)
+        case KVP_SCORER_CAM: *launches_out = 6; break;
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -843,6 +847,33 @@ kvp_status kvp_scores_compress_chunked(const kvp_problem* p, const void* scores,
     // the Finch layout at the smallest window: the selection regions and the kept positions
     return static_cast<kvp_status>(run(Kind::compress, p, KVP_SCORER_FINCH, 1, io, operands,
                                        keys_from(p, scores, score_stride), workspace, workspace_bytes, stream));
+}
+
+// ---- CaM -----------------------------------------------------------------------------------------------------------
+kvp_status kvp_cam_compress(const kvp_problem* p, const void* scores, const int64_t* score_stride, const void* K,
+                            const void* V, const float* attn_sum, const int64_t* attn_stride, int32_t n_merge,
+                            int32_t merge_budget, const float* uniforms, void* K_out, void* V_out, float* attn_out,
+                            const int64_t* attn_out_stride, int32_t* idx_out, int32_t* merge_idx_out,
+                            float* merge_prob_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!scores || !score_stride || !attn_sum || !attn_stride || !attn_out || !attn_out_stride)
+            return KVP_ERR_NULL_POINTER;
+        if (!uniforms && n_merge != 0) return KVP_ERR_NULL_POINTER;
+        if (!aligned2(scores) || !aligned4(attn_sum) || !aligned4(attn_out) || !aligned4(uniforms) ||
+            !aligned4(idx_out) || !aligned4(merge_idx_out) || !aligned4(merge_prob_out))
+            return KVP_ERR_BAD_STRIDE;
+        if (merge_budget < 1 || n_merge < 0 || n_merge > d.S - d.n_kept) return KVP_ERR_BAD_ARGUMENT;
+        return KVP_OK;
+    };
+    Call c;
+    int rc = prepare(Kind::compress, p, KVP_SCORER_CAM, 0, {K, V, K_out, V_out, idx_out, nullptr}, operands, workspace,
+                     workspace_bytes, stream, &c);
+    if (rc || c.d.n_kept == 0) return static_cast<kvp_status>(rc);
+    if ((rc = c.zero())) return static_cast<kvp_status>(rc);
+    return static_cast<kvp_status>(status(launch_cam_compress(
+        c.d, p->dtype, scores, score_stride[0], score_stride[1], K, V, attn_sum, attn_stride[0], attn_stride[1],
+        n_merge, merge_budget, uniforms, K_out, V_out, attn_out, attn_out_stride[0], attn_out_stride[1], idx_out,
+        merge_idx_out, merge_prob_out, c.ws, c.st)));
 }
 
 }  // extern "C"

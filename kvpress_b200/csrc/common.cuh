@@ -498,5 +498,16 @@ size_t think_scratch_bytes(const Dims& d);
 // a memset of the row tickets, the reduce + select kernel and the zero kernel on `scratch` (think_scratch_bytes)
 cudaError_t launch_think_prune(const Dims& d, int dtype, void* K, const void* q, int window, int n_pruned,
                                int32_t* pruned_out, float* scores_out, void* scratch, cudaStream_t st);
+// CAMPress selects once per batch element, on the head mean of the scores: its selection regions are laid out for
+// the B rows of cam_selection_dims(d), and cam_scratch_bytes(d) (sized for n_merge = S - n_kept) follows them.
+Dims cam_selection_dims(const Dims& d);
+size_t cam_scratch_bytes(const Dims& d);
+// head mean + keys, selection, and with n_merge > 0 candidates and probabilities, then the merge + compaction; `ws`
+// is carved for cam_selection_dims(d) and its selection regions are cleared
+cudaError_t launch_cam_compress(const Dims& d, int dtype, const void* scores, int64_t sb, int64_t sh, const void* K,
+                                const void* V, const float* A, int64_t ab, int64_t ah, int n_merge, int budget,
+                                const float* u, void* K_out, void* V_out, float* A_out, int64_t ob, int64_t oh,
+                                int32_t* idx_out, int32_t* merge_idx_out, float* prob_out, const Workspace& ws,
+                                cudaStream_t st);
 
 }  // namespace kvp

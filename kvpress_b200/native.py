@@ -24,6 +24,7 @@ SCORER_CUR = 11  # KVP_SCORER_CUR; id 10 is not assigned
 SCORER_MERGING = 13  # KVP_SCORER_MERGING; id 12 is not assigned
 SCORER_THINK = 14  # KVP_SCORER_THINK: kvp_think_prune
 SCORER_FINCH = 16  # KVP_SCORER_FINCH: kvp_finch_*, kvp_scores_compress_chunked; id 15 is not assigned
+SCORER_CAM = 17  # KVP_SCORER_CAM: kvp_cam_compress
 LAG_MAX = 1024  # the largest lag_size the LagKV kernel scores (kLagMax in csrc/common.cuh)
 CUR_WINDOW_MAX = 1024  # the largest local_window_size the CUR kernel scores (kCurWindowMax in csrc/common.cuh)
 CUR_RANK_MAX = 32  # the most projection columns the CUR kernel scores (kCurRankMax)
@@ -102,6 +103,8 @@ SIGNATURES = {
     "kvp_finch_score": (ctypes.c_int, [_PP, _P, _P, _I, _I, _P, _P, _SZ, _P]),
     "kvp_finch_compress": (ctypes.c_int, [_PP, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _SZ, _P]),
     "kvp_scores_compress_chunked": (ctypes.c_int, [_PP, _P, _PI64, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_cam_compress": (
+        ctypes.c_int, [_PP, _P, _PI64, _P, _P, _P, _PI64, _I, _I, _P, _P, _P, _P, _PI64, _P, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -865,3 +868,51 @@ def scores_compress_chunked(scores: torch.Tensor, keys, values, compression_rati
     return _compress("kvp_scores_compress_chunked", SCORER_FINCH, keys, values, n_kept,
                      (scores, sstride, L, chunk_kept, tail_kept, keys, values, _inv_freq(inv_freq, keys)),
                      return_indices)
+
+
+# --------------------------------------------------------------------------------------------------
+# CaM (CAMPress: evicted values merged into the kept rows after them, then pruned)
+# --------------------------------------------------------------------------------------------------
+def _attn_view(a: torch.Tensor, shape: tuple, keys: torch.Tensor, name: str):
+    """A float32 [B, Hkv, n] view with unit stride along n (it may sit in a capacity buffer) and its (b, h) strides."""
+    if a.dtype != torch.float32 or tuple(a.shape) != shape or a.device != keys.device or (shape[2] > 1 and a.stride(2) != 1):
+        raise RuntimeError(f"{name} must be a float32 {list(shape)} view with unit stride along the last dim on "
+                           f"{keys.device}, got {a.dtype} {tuple(a.shape)} on {a.device}")
+    return (ctypes.c_int64 * 2)(*(a.stride(d) if a.shape[d] > 1 else 0 for d in range(2)))
+
+
+def cam_compress(scores: torch.Tensor, keys, values, attn_sum: torch.Tensor, attn_out: torch.Tensor, n_merge: int,
+                 merge_budget: int, uniforms: Optional[torch.Tensor], n_kept: int, return_indices: bool = False,
+                 return_plan: bool = False):
+    """CAMPress.compress (include/kvpress_b200.h, kvp_cam_compress): the n_kept best head means of `scores` are kept
+    (one selection per batch element), the n_merge best evicted positions are merged, each with probability
+    clamp(A[e] / window mean of A), into the merge_budget kept rows after it, and K, V and the running sum attn_sum
+    (float32 [B, Hkv, S]) are compacted; the pruned sum is written into attn_out (float32 [B, Hkv, n_kept]). uniforms:
+    float32 [B, Hkv, n_merge] in [0, 1), the draws. Returns (k_out, v_out, idx, merge_idx, merge_prob): idx (int32
+    [B, n_kept]) with return_indices, and with return_plan the candidates (int32 [B, n_merge]) and their
+    probabilities (float32 [B, Hkv, n_merge]); None otherwise."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    scores, sstride = _caller_scores(scores, keys)
+    B, H, S, D = keys.shape
+    astride = _attn_view(attn_sum, (B, H, S), keys, "attn_sum")
+    ostride = _attn_view(attn_out, (B, H, n_kept), keys, "attn_out")
+    if not 0 <= n_merge <= S - n_kept or merge_budget < 1:
+        raise ValueError(f"need 0 <= n_merge <= {S - n_kept} and merge_budget >= 1, got {n_merge}, {merge_budget}")
+    if n_merge > 0:
+        if uniforms is None or tuple(uniforms.shape) != (B, H, n_merge) or uniforms.device != keys.device:
+            raise RuntimeError(f"uniforms must be [{B}, {H}, {n_merge}] on {keys.device}")
+        uniforms = uniforms.to(torch.float32).contiguous()
+    else:
+        uniforms = None
+    dev = keys.device
+    k_out = torch.empty((B, H, n_kept, D), dtype=keys.dtype, device=dev)
+    v_out = torch.empty_like(k_out)
+    idx = torch.empty((B, n_kept), dtype=torch.int32, device=dev) if return_indices else None
+    merge_idx = torch.empty((B, n_merge), dtype=torch.int32, device=dev) if return_plan else None
+    merge_prob = torch.empty((B, H, n_merge), dtype=torch.float32, device=dev) if return_plan else None
+    if n_kept > 0:
+        _enqueue("kvp_cam_compress", dev, make_problem(keys, values, n_kept), scores, sstride, keys, values, attn_sum,
+                 astride, int(n_merge), int(merge_budget), uniforms, k_out, v_out, attn_out, ostride, idx, merge_idx,
+                 merge_prob, scorer=SCORER_CAM)
+    return k_out, v_out, idx, merge_idx, merge_prob

@@ -119,6 +119,7 @@ class DecodingPress(BasePress):
         q_len = hidden_states.shape[1]
         layer_idx = module.layer_idx
         if hook_is_prefilling(module, kwargs):
+            self._on_prefill(layer_idx)
             return output  # prefill is some other press's business
 
         buffering = self.hidden_states_buffer_size > 0 and getattr(self.base_press, "needs_hidden_states", True)
@@ -129,9 +130,10 @@ class DecodingPress(BasePress):
         elif length_only:
             self.hidden_states_lens[layer_idx].append(q_len)
         self.layer_step_counts[layer_idx] += 1
+        self._on_decoding_step(module, hidden_states, kwargs)
 
         target = self._resolve_target_size(kwargs)
-        if self.layer_step_counts[layer_idx] >= self.compression_interval or q_len >= target:
+        if self._should_compress(layer_idx, q_len, target, cache):
             logger.debug(f"Applying decoding compression at layer {layer_idx}: "
                          f"step {self.layer_step_counts[layer_idx]} / interval {self.compression_interval}")
             keys, values = extract_keys_and_values(cache, layer_idx)
@@ -155,6 +157,15 @@ class DecodingPress(BasePress):
         elif length_only:
             self.hidden_states_lens[layer_idx] = self.hidden_states_lens[layer_idx][-self.hidden_states_buffer_size:]
         return output
+
+    def _on_prefill(self, layer_idx: int) -> None:
+        """Called by the hook on a prefill forward of a layer (DecodingPress keeps its state)."""
+
+    def _on_decoding_step(self, module: nn.Module, hidden_states: torch.Tensor, kwargs: dict) -> None:
+        """Called by the hook on every decoding forward of a layer, after the step is counted, before any compaction."""
+
+    def _should_compress(self, layer_idx: int, q_len: int, target: int, cache) -> bool:
+        return self.layer_step_counts[layer_idx] >= self.compression_interval or q_len >= target
 
     def reset(self):
         self.hidden_states_buffer = defaultdict(list)

@@ -17,7 +17,7 @@ from torch import nn
 
 from kvpress_b200 import native
 from kvpress_b200.presses.scorer_press import ScorerPress
-from kvpress_b200.utils import apply_rope, get_prerope_query_states
+from kvpress_b200.utils import last_query
 
 
 @dataclass
@@ -26,9 +26,7 @@ class TOVAPress(ScorerPress):
 
     def last_query(self, module: nn.Module, hidden_states: torch.Tensor, kwargs: dict) -> torch.Tensor:
         """RoPE'd query of the last position, [B, Hq, D]."""
-        q = get_prerope_query_states(module, hidden_states[:, -1:])
-        cos, sin = kwargs["position_embeddings"]
-        return apply_rope(q, cos[:, -1:], sin[:, -1:])[:, :, 0].contiguous()
+        return last_query(module, hidden_states, kwargs)
 
     def score(self, module: nn.Module, hidden_states, keys: torch.Tensor, values, attentions, kwargs) -> torch.Tensor:
         H = keys.shape[1]

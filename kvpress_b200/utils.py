@@ -45,3 +45,10 @@ def rotate_half(x: torch.Tensor) -> torch.Tensor:
 def apply_rope(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch.Tensor:
     """x: [B, H, L, D]; cos/sin: [B or 1, L, D] (the `position_embeddings` HF passes to attention)."""
     return x * cos.unsqueeze(1) + rotate_half(x) * sin.unsqueeze(1)
+
+
+def last_query(module: nn.Module, hidden_states: torch.Tensor, kwargs: dict) -> torch.Tensor:
+    """RoPE'd query of the last position of `hidden_states`, [B, Hq, D] (TOVAPress's score, CAMPress's decode step)."""
+    q = get_prerope_query_states(module, hidden_states[:, -1:])
+    cos, sin = kwargs["position_embeddings"]
+    return apply_rope(q, cos[:, -1:], sin[:, -1:])[:, :, 0].contiguous()
