@@ -21,6 +21,8 @@
  *     kvp_merging_*            <- kvpress/presses/merging_press.py (evicted values folded into their nearest kept row)
  *     kvp_think_prune          <- kvpress/presses/think_press.py (key channels zeroed in place; no positions removed)
  *     kvp_cam_compress         <- kvpress/presses/cam_press.py (evicted values merged into the kept rows after them)
+ *     kvp_kvzap_*              <- kvpress/presses/kvzap_press.py (a surrogate model of the hidden states)
+ *     kvp_threshold_evict      <- kvpress/presses/dms_press.py (the positions whose score is below a threshold)
  *     kvp_scores_compress      <- scorer_press.py:93-100 for an arbitrary score tensor
  *                                 (what wrapper presses / user ScorerPress subclasses need)
  *
@@ -88,7 +90,8 @@ typedef enum kvp_scorer {
     KVP_SCORER_MERGING = 13, /* kvp_merging_*: the selection of the caller's scores, then the merge */
     KVP_SCORER_THINK = 14,   /* kvp_think_prune: key channels, not positions */
     KVP_SCORER_FINCH = 16,   /* kvp_finch_*, kvp_scores_compress_chunked */
-    KVP_SCORER_CAM = 17      /* kvp_cam_compress */
+    KVP_SCORER_CAM = 17,     /* kvp_cam_compress */
+    KVP_SCORER_KVZAP = 18    /* kvp_kvzap_* */
 } kvp_scorer;
 
 /* One ScorerPress.compress call on one layer's cache. */
@@ -523,6 +526,75 @@ kvp_status kvp_cam_compress(const kvp_problem* p, const void* scores, const int6
                             int32_t merge_budget, const float* uniforms, void* K_out, void* V_out, float* attn_out,
                             const int64_t* attn_out_stride, int32_t* idx_out, int32_t* merge_idx_out,
                             float* merge_prob_out, void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+
+/* ---- KVzapPress (kvpress/presses/kvzap_press.py, https://arxiv.org/abs/2601.07891) ---------------------------------
+ * Scores from a small per-layer surrogate model of the attention module's input hidden states x [B, S, hidden] (S =
+ * p->S); no queries, attention weights or K / V are read. Per (b, kv head j, s), with gelu(t) = t/2 (1 + erf(t/sqrt 2))
+ * (nn.GELU's default) and every weight in the cache dtype p->dtype:
+ *   hd > 0 (MLP):    score = b2[j] + sum_c W2[j, c] gelu(b1[c] + sum_k W1[c, k] x[b, s, k])
+ *                    W1 [hd, hidden], b1 [hd], W2 [Hkv, hd], b2 [Hkv], contiguous as nn.Linear stores them.
+ *   hd == 0 (linear): score = b[j] + sum_k W[j, k] x[b, s, k], with W [Hkv, hidden] passed as w1, b [Hkv] as b1;
+ *                    w2 and b2 are not read.
+ * Every sum is fp32 in an order fixed by the shape: the pre-activation is the K-ordered tensor-core accumulation
+ * (B S > 32) or the CUDA-core sum of 8-element slices added lane by lane, then across the warp (B S <= 32); then
+ * b1 and the GELU in fp32; the W2 products are added per chunk of 128 units (8 when B S <= 32), the chunks in
+ * ascending order, then b2. The score is rounded ONCE to the cache dtype and written into scores_out
+ * [B, Hkv, S] contiguous.
+ * Deviation from the reference: it evaluates Linear -> GELU -> Linear in the cache dtype and rounds after each layer;
+ * here nothing is rounded between the layers. Against the float64 evaluation s64 of the same 16-bit inputs, with
+ * a_c = b1[c] + sum_k W1[c, k] x_k, A_c = |b1[c]| + sum_k |W1[c, k] x_k|, e_c = (hidden + 2) 2^-22 A_c,
+ * E_c = 1.2 e_c + 2^-20 (|a_c| + e_c) and h_c = gelu(a_c),
+ *   |score_fp32 - s64| <= E = sum_c |W2[j, c]| E_c + (hd + 260) 2^-23 (|b2[j]| + sum_c |W2[j, c]| (|h_c| + E_c))
+ * (linear: E = (hidden + 2) 2^-22 (|b[j]| + sum_k |W[j, k] x_k|)), so the score lies in [RD(s64 - E), RU(s64 + E)],
+ * RD / RU rounding down / up to the cache dtype. Two calls give bitwise-equal scores, and a row's score does not
+ * depend on the other rows, the strides or the SM count (it does on whether B S <= 32, which picks the order above).
+ * Arguments:
+ *   x        [B, S, hidden] in the cache dtype, element strides x_stride (b, s), the hidden dim contiguous, 16-byte
+ *            aligned; a stride of a size-1 dim is not read.
+ *   w1       16-byte aligned; b1, w2, b2 2-byte aligned.
+ * Supported: hidden a multiple of 8 up to 16384, hd 0 or a multiple of 8 up to 2048, Hkv up to 32, both dtypes;
+ * anything else is KVP_ERR_UNSUPPORTED_SHAPE (the press then scores with cuBLAS in fp32).
+ * Check order (the first failure is returned): validate the problem -> (compress) n_kept == 0 returns KVP_OK and
+ * enqueues nothing -> (compress) K / V / K_out / V_out null and 16-byte alignment -> (score) scores_out null ->
+ * scores_out 2-byte alignment -> x, x_stride, w1, b1 null, and w2, b2 null when hd > 0 -> x, w1 16-byte and b1, w2,
+ * b2 2-byte alignment -> hidden < 1 or hd < 0 gives KVP_ERR_BAD_ARGUMENT -> x_stride negative or not a multiple of 8,
+ * or x_stride[1] < hidden with S > 1, gives KVP_ERR_BAD_STRIDE -> the supported shapes -> workspace null -> its
+ * 16-byte alignment -> its size.
+ * kvp_workspace_bytes(KVP_SCORER_KVZAP): the selection regions (as kvp_scores_compress), then
+ * 4 B P Hkv B S for the partials, P = 256 when B S <= 32 and 16 otherwise (enough for hd = 2048), then 2 B B Hkv S
+ * for the scores a compress call selects on, each region rounded up to 256 bytes. kvp_launches_per_compress says 5
+ * (memset, scores, reduce of the partials, keys, select + compact); the linear model takes 4 (no reduce), a score
+ * call 2 (MLP) or 1 (linear). Memory beyond the workspace: none.
+ * The return type is kvp_status, an int-sized enum with the values of every other entry point's int. */
+kvp_status kvp_kvzap_score(const kvp_problem* p, const void* x, const int64_t* x_stride, int32_t hidden, int32_t hd,
+                           const void* w1, const void* b1, const void* w2, const void* b2, void* scores_out,
+                           void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+/* The scores above, then the selection and compaction of kvp_scores_compress: 16-bit keys, NaN above every number,
+ * -0 == +0, ties to the lowest positions. scores_out is nullable here. */
+kvp_status kvp_kvzap_compress(const kvp_problem* p, const void* x, const int64_t* x_stride, int32_t hidden, int32_t hd,
+                              const void* w1, const void* b1, const void* w2, const void* b2, const void* K,
+                              const void* V, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
+                              void* workspace, size_t workspace_bytes, kvp_stream_t stream);
+
+/* ---- DMSPress (kvpress/presses/dms_press.py): threshold eviction --------------------------------------------------
+ * Every (b, h, s) with s < n_evict and scores[b, h, s] < threshold, for scores [B, Hkv, n] in dtype (bf16 / fp16),
+ * element strides score_stride (b, h), s contiguous, 2-byte aligned. The comparison is made in the score dtype: the
+ * threshold is first rounded to nearest-even in that dtype, as torch does for `scores < python_float` (a bf16 score
+ * of 0.099609375 is not below 0.0998). NaN is never evicted; -0 is not below +0.
+ * Output: b_out, h_out, s_out (int64, capacity B Hkv n_evict) get b, h and s + shift of every evicted position in
+ * torch.where order (b, then h, then s ascending), and *count_out (int64, device) their number. The result is exact:
+ * per-(row, 4096-position tile) counts, one scan, an ordered write, no atomics.
+ * Check order: dtype -> B, Hkv, n < 1 or B Hkv ceil(n / 4096) >= 2^31 gives KVP_ERR_UNSUPPORTED_SHAPE -> n_evict outside [0, n]
+ * gives KVP_ERR_BAD_ARGUMENT -> scores, score_stride, count_out null, and b_out, h_out, s_out null when n_evict > 0 ->
+ * scores 2-byte alignment, negative strides, b_out, h_out, s_out, count_out 8-byte alignment (KVP_ERR_BAD_STRIDE) ->
+ * workspace null -> its 16-byte alignment -> its size: 8 B Hkv ceil(n / 4096) bytes rounded up to 256 (the
+ * per-tile counts).
+ * 3 launches (counts, scan, write). Memory beyond the workspace: none.
+ * The return type is kvp_status, an int-sized enum with the values of every other entry point's int. */
+kvp_status kvp_threshold_evict(int32_t dtype, int32_t B, int32_t Hkv, int32_t n, const void* scores,
+                               const int64_t* score_stride, int32_t n_evict, float threshold, int64_t shift,
+                               int64_t* b_out, int64_t* h_out, int64_t* s_out, int64_t* count_out, void* workspace,
+                               size_t workspace_bytes, kvp_stream_t stream);
 
 /* ---- selection only: the n_kept best positions of every [S] score row, ascending, into idx_out
  * [B, Hkv, n_kept]; no K/V are touched (p->D and the K/V strides are ignored). What head-wise presses need:

@@ -15,11 +15,13 @@ from kvpress_b200.presses.compression_ratio_decoding_press import CompressionRat
 from kvpress_b200.presses.criticalkv_press import CriticalAdaKVPress, CriticalKVPress
 from kvpress_b200.presses.cur_press import CURPress
 from kvpress_b200.presses.decoding_press import DecodingPress
+from kvpress_b200.presses.dms_press import DMSPress
 from kvpress_b200.presses.expected_attention_press import ExpectedAttentionPress
 from kvpress_b200.presses.expected_attention_with_stats import ExpectedAttentionStatsPress
 from kvpress_b200.presses.key_rerotation_press import KeyRerotationPress
 from kvpress_b200.presses.keydiff_press import KeyDiffPress
 from kvpress_b200.presses.knorm_press import KnormPress
+from kvpress_b200.presses.kvzap_press import KVzapConfig, KVzapModel, KVzapPress
 from kvpress_b200.presses.lagkv_press import LagKVPress
 from kvpress_b200.presses.merging_press import MergingPress
 from kvpress_b200.presses.non_causal_attention_press import NonCausalAttnPress
@@ -50,6 +52,10 @@ __all__ = [
     "TOVAPress",
     "DecodingPress",
     "CAMPress",
+    "KVzapPress",
+    "KVzapModel",
+    "KVzapConfig",
+    "DMSPress",
     "KeyRerotationPress",
     "KeyDiffPress",
     "AdaKVPress",

@@ -17,7 +17,7 @@ LIB_PATH = PKG_DIR / "libkvpress_b200.so"
 STAMP = PKG_DIR / "build" / "stamp.txt"
 SOURCES = ["api.cu", "knorm.cu", "knorm_cluster.cu", "keydiff.cu", "select_compact.cu", "snapkv.cu", "expected_attention.cu",
            "criticalkv.cu", "observed_attention.cu", "non_causal_attention.cu", "lagkv.cu", "cur.cu", "merging.cu",
-           "think.cu", "finch.cu", "cam.cu", "tmap.cu"]
+           "think.cu", "finch.cu", "cam.cu", "kvzap.cu", "tmap.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",

@@ -108,6 +108,7 @@ static size_t layout(const Dims& d_call, int scorer, int window, void* base, Wor
                        : scorer == KVP_SCORER_MERGING              ? merging_scratch_bytes(d)
                        : scorer == KVP_SCORER_FINCH                ? finch_scratch_bytes(d, window)
                        : scorer == KVP_SCORER_CAM                  ? cam_scratch_bytes(d_call)
+                       : scorer == KVP_SCORER_KVZAP                ? kvzap_scratch_bytes(d)
                                                                    : 0;
     ws->scorer = c.take<char>(ws->scorer_bytes);
     return c.bytes;
@@ -323,6 +324,8 @@ int kvp_launches_per_compress(const kvp_problem* p, int scorer, int* launches_ou
         case KVP_SCORER_FINCH: *launches_out = 6; break;
         // memset, head mean + keys, select, candidates, probabilities, merge + compaction (4 when n_merge == 0)
         case KVP_SCORER_CAM: *launches_out = 6; break;
+        // memset, scores (gemm or W1-spread), reduce, keys, select+compact (the linear model: 4, no reduce)
+        case KVP_SCORER_KVZAP: *launches_out = 5; break;
         default: return KVP_ERR_BAD_ARGUMENT;
     }
     return KVP_OK;
@@ -726,6 +729,10 @@ static int merging_args(float similarity_threshold, double merge_fraction) {
 }
 
 static bool aligned4(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+static bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; }
+static size_t threshold_evict_workspace_bytes(int B, int Hkv, int n) {
+    return align256((size_t)B * Hkv * ((n + kEvictTile - 1) / kEvictTile) * 8);
+}
 
 int kvp_merging_compress(const kvp_problem* p, const void* scores, const int64_t* score_stride, const void* K,
                          const void* V, float similarity_threshold, double merge_fraction, void* K_out, void* V_out,
@@ -874,6 +881,82 @@ kvp_status kvp_cam_compress(const kvp_problem* p, const void* scores, const int6
         c.d, p->dtype, scores, score_stride[0], score_stride[1], K, V, attn_sum, attn_stride[0], attn_stride[1],
         n_merge, merge_budget, uniforms, K_out, V_out, attn_out, attn_out_stride[0], attn_out_stride[1], idx_out,
         merge_idx_out, merge_prob_out, c.ws, c.st)));
+}
+
+// ---- KVzap ---------------------------------------------------------------------------------------------------------
+// The operand checks both entry points share, after the problem's (see kvp_kvzap_score in the header).
+static int kvzap_args(const Dims& d, const void* x, const int64_t* x_stride, int32_t hidden, int32_t hd,
+                      const void* w1, const void* b1, const void* w2, const void* b2) {
+    if (!x || !x_stride || !w1 || !b1 || (hd > 0 && (!w2 || !b2))) return KVP_ERR_NULL_POINTER;
+    if (!aligned16(x) || !aligned16(w1) || !aligned2(b1) || !aligned2(w2) || !aligned2(b2)) return KVP_ERR_BAD_STRIDE;
+    if (hidden < 1 || hd < 0) return KVP_ERR_BAD_ARGUMENT;
+    for (int i = 0; i < 2; ++i)
+        if (x_stride[i] < 0 || x_stride[i] % 8 != 0) return KVP_ERR_BAD_STRIDE;
+    if (d.S > 1 && x_stride[1] < hidden) return KVP_ERR_BAD_STRIDE;
+    if (hidden % 8 != 0 || hidden > kZapMaxHidden || hd % 8 != 0 || hd > kZapMaxHd || d.H > kZapMaxHeads)
+        return KVP_ERR_UNSUPPORTED_SHAPE;
+    return KVP_OK;
+}
+
+kvp_status kvp_kvzap_score(const kvp_problem* p, const void* x, const int64_t* x_stride, int32_t hidden, int32_t hd,
+                           const void* w1, const void* b1, const void* w2, const void* b2, void* scores_out,
+                           void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!scores_out) return KVP_ERR_NULL_POINTER;
+        if (!aligned2(scores_out)) return KVP_ERR_BAD_STRIDE;
+        return kvzap_args(d, x, x_stride, hidden, hd, w1, b1, w2, b2);
+    };
+    auto score = [&](const Call& c) {
+        return launch_kvzap_score(c.d, p->dtype, x, x_stride[0], x_stride[1], hidden, hd, w1, b1, w2, b2, c.ws,
+                                  scores_out, c.st);
+    };
+    // no selection: nothing to clear
+    return static_cast<kvp_status>(run(Kind::score, p, KVP_SCORER_KVZAP, 0, {}, operands, score, workspace,
+                                       workspace_bytes, stream, false));
+}
+
+kvp_status kvp_kvzap_compress(const kvp_problem* p, const void* x, const int64_t* x_stride, int32_t hidden, int32_t hd,
+                              const void* w1, const void* b1, const void* w2, const void* b2, const void* K,
+                              const void* V, void* K_out, void* V_out, int32_t* idx_out, void* scores_out,
+                              void* workspace, size_t workspace_bytes, kvp_stream_t stream) {
+    auto operands = [&](const Dims& d) -> int {
+        if (!aligned2(scores_out)) return KVP_ERR_BAD_STRIDE;
+        return kvzap_args(d, x, x_stride, hidden, hd, w1, b1, w2, b2);
+    };
+    auto score = [&](const Call& c) {
+        void* out = scores_out ? scores_out : kvzap_scratch_scores(c.d, c.ws);
+        cudaError_t e = launch_kvzap_score(c.d, p->dtype, x, x_stride[0], x_stride[1], hidden, hd, w1, b1, w2, b2,
+                                           c.ws, out, c.st);
+        if (e == cudaSuccess)
+            e = launch_keys_from_scores(c.d, p->dtype, out, (int64_t)c.d.H * c.d.S, c.d.S, c.ws, c.st);
+        return e;
+    };
+    return static_cast<kvp_status>(run(Kind::compress, p, KVP_SCORER_KVZAP, 0, {K, V, K_out, V_out, idx_out, nullptr},
+                                       operands, score, workspace, workspace_bytes, stream));
+}
+
+// ---- DMS threshold eviction -----------------------------------------------------------------------------------------
+kvp_status kvp_threshold_evict(int32_t dtype, int32_t B, int32_t Hkv, int32_t n, const void* scores,
+                               const int64_t* score_stride, int32_t n_evict, float threshold, int64_t shift,
+                               int64_t* b_out, int64_t* h_out, int64_t* s_out, int64_t* count_out, void* workspace,
+                               size_t workspace_bytes, kvp_stream_t stream) {
+    if (dtype != KVP_BF16 && dtype != KVP_F16) return KVP_ERR_UNSUPPORTED_DTYPE;
+    // one CTA per (row, tile of kEvictTile positions) on gridDim.x
+    if (B <= 0 || Hkv <= 0 || n <= 0 || (int64_t)B * Hkv * ((n + kEvictTile - 1) / kEvictTile) > 0x7FFFFFFF)
+        return KVP_ERR_UNSUPPORTED_SHAPE;
+    if (n_evict < 0 || n_evict > n) return KVP_ERR_BAD_ARGUMENT;
+    if (!scores || !score_stride || !count_out || (n_evict > 0 && (!b_out || !h_out || !s_out)))
+        return KVP_ERR_NULL_POINTER;
+    if (!aligned2(scores) || score_stride[0] < 0 || score_stride[1] < 0 || !aligned8(b_out) || !aligned8(h_out) ||
+        !aligned8(s_out) || !aligned8(count_out))
+        return KVP_ERR_BAD_STRIDE;
+    if (workspace == nullptr) return KVP_ERR_NULL_POINTER;
+    if (!aligned16(workspace)) return KVP_ERR_BAD_STRIDE;
+    if (workspace_bytes < threshold_evict_workspace_bytes(B, Hkv, n)) return KVP_ERR_WORKSPACE_TOO_SMALL;
+    return static_cast<kvp_status>(status(launch_threshold_evict(dtype, B, Hkv, scores, score_stride[0],
+                                                                 score_stride[1], n_evict, threshold, shift, b_out,
+                                                                 h_out, s_out, count_out, workspace,
+                                                                 static_cast<cudaStream_t>(stream))));
 }
 
 }  // extern "C"

@@ -510,4 +510,23 @@ cudaError_t launch_cam_compress(const Dims& d, int dtype, const void* scores, in
                                 int32_t* idx_out, int32_t* merge_idx_out, float* prob_out, const Workspace& ws,
                                 cudaStream_t st);
 
+// KVzapPress (kvzap.cu): the shapes the kernels take, and the B S at or below which the W1-spread kernel runs
+constexpr int kZapMaxHidden = 16384;
+constexpr int kZapMaxHd = 2048;
+constexpr int kZapMaxHeads = 32;
+constexpr int kZapGemvRows = 32;
+constexpr int kZapGemvUnits = 8;  // hidden units per CTA of the W1-spread kernel
+// the partials [parts][Hkv][B S] fp32 (parts for hd = kZapMaxHd), then the scores a compress call selects on
+size_t kvzap_scratch_bytes(const Dims& d);
+void* kvzap_scratch_scores(const Dims& d, const Workspace& ws);
+// hd == 0: the linear model (w1 = W, b1 = b); hd > 0: partials into ws.scorer, then the reduce
+cudaError_t launch_kvzap_score(const Dims& d, int dtype, const void* x, int64_t xb, int64_t xs, int hidden, int hd,
+                               const void* w1, const void* b1, const void* w2, const void* b2, const Workspace& ws,
+                               void* scores_out, cudaStream_t st);
+// per-(row, tile of kEvictTile positions) counts into `scratch` (8 B each), their scan, the ordered write
+constexpr int kEvictTile = 4096;
+cudaError_t launch_threshold_evict(int dtype, int B, int H, const void* scores, int64_t sb, int64_t sh, int n_evict,
+                                   float threshold, int64_t shift, int64_t* b_out, int64_t* h_out, int64_t* s_out,
+                                   int64_t* count_out, void* scratch, cudaStream_t st);
+
 }  // namespace kvp

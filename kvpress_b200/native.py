@@ -25,6 +25,10 @@ SCORER_MERGING = 13  # KVP_SCORER_MERGING; id 12 is not assigned
 SCORER_THINK = 14  # KVP_SCORER_THINK: kvp_think_prune
 SCORER_FINCH = 16  # KVP_SCORER_FINCH: kvp_finch_*, kvp_scores_compress_chunked; id 15 is not assigned
 SCORER_CAM = 17  # KVP_SCORER_CAM: kvp_cam_compress
+SCORER_KVZAP = 18  # KVP_SCORER_KVZAP: kvp_kvzap_*
+KVZAP_MAX_HIDDEN = 16384  # the shapes the KVzap kernels take (kZapMax* in csrc/common.cuh)
+KVZAP_MAX_HD = 2048
+KVZAP_MAX_HEADS = 32
 LAG_MAX = 1024  # the largest lag_size the LagKV kernel scores (kLagMax in csrc/common.cuh)
 CUR_WINDOW_MAX = 1024  # the largest local_window_size the CUR kernel scores (kCurWindowMax in csrc/common.cuh)
 CUR_RANK_MAX = 32  # the most projection columns the CUR kernel scores (kCurRankMax)
@@ -105,6 +109,11 @@ SIGNATURES = {
     "kvp_scores_compress_chunked": (ctypes.c_int, [_PP, _P, _PI64, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _SZ, _P]),
     "kvp_cam_compress": (
         ctypes.c_int, [_PP, _P, _PI64, _P, _P, _P, _PI64, _I, _I, _P, _P, _P, _P, _PI64, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_kvzap_score": (ctypes.c_int, [_PP, _P, _PI64, _I, _I, _P, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_kvzap_compress": (
+        ctypes.c_int, [_PP, _P, _PI64, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _SZ, _P]),
+    "kvp_threshold_evict": (
+        ctypes.c_int, [_I, _I, _I, _I, _P, _PI64, _I, ctypes.c_float, _I64, _P, _P, _P, _P, _P, _SZ, _P]),
 }
 
 _lib: Optional[ctypes.CDLL] = None
@@ -916,3 +925,76 @@ def cam_compress(scores: torch.Tensor, keys, values, attn_sum: torch.Tensor, att
                  astride, int(n_merge), int(merge_budget), uniforms, k_out, v_out, attn_out, ostride, idx, merge_idx,
                  merge_prob, scorer=SCORER_CAM)
     return k_out, v_out, idx, merge_idx, merge_prob
+
+
+# --------------------------------------------------------------------------------------------------
+# KVzap (KVzapPress: a surrogate model of the hidden states) and DMS (DMSPress: threshold eviction)
+# --------------------------------------------------------------------------------------------------
+def kvzap_supported(hidden: int, hd: int, n_heads: int) -> bool:
+    """The shapes kvp_kvzap_* take (include/kvpress_b200.h); KVzapPress scores others with cuBLAS."""
+    return (hidden % 8 == 0 and 0 < hidden <= KVZAP_MAX_HIDDEN and hd % 8 == 0 and 0 <= hd <= KVZAP_MAX_HD
+            and 0 < n_heads <= KVZAP_MAX_HEADS)
+
+
+def _kvzap_inputs(hidden_states: torch.Tensor, keys: torch.Tensor, weights: tuple):
+    """(x, its (b, s) strides, hidden, hd, w1, b1, w2, b2) of a kvp_kvzap_* call. weights = (w1, b1, w2, b2) in the
+    cache dtype on its device (MLP), or (W, b, None, None) (linear)."""
+    B, H, S, _ = keys.shape
+    x = hidden_states
+    if x.dim() != 3 or x.shape[0] != B or x.shape[1] != S or x.dtype != keys.dtype or x.device != keys.device:
+        raise RuntimeError(f"hidden_states must be [{B}, {S}, hidden] {keys.dtype} on {keys.device}, got "
+                           f"{tuple(x.shape)} {x.dtype} on {x.device}")
+    if x.stride(2) != 1 or x.data_ptr() % 16 or any(x.shape[d] > 1 and (x.stride(d) % 8 or x.stride(d) < 0)
+                                                    for d in range(2)):
+        x = x.contiguous()
+    w1, b1, w2, b2 = weights
+    hd = 0 if w2 is None else int(w1.shape[0])
+    for t in (w1, b1, w2, b2):
+        if t is not None and (t.dtype != keys.dtype or t.device != keys.device or not t.is_contiguous()):
+            raise RuntimeError(f"KVzap weights must be contiguous {keys.dtype} on {keys.device}")
+    xstride = (ctypes.c_int64 * 2)(*(x.stride(d) if x.shape[d] > 1 else 0 for d in range(2)))
+    return x, xstride, int(x.shape[2]), hd, w1, b1, w2, b2
+
+
+def kvzap_score(hidden_states: torch.Tensor, keys: torch.Tensor, values: torch.Tensor, weights: tuple) -> torch.Tensor:
+    """KVzapPress.score (kvp_kvzap_score): the surrogate model's scores [B, Hkv, S] in the cache dtype."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    return _score("kvp_kvzap_score", SCORER_KVZAP, keys, make_problem(keys, values, 0),
+                  *_kvzap_inputs(hidden_states, keys, weights))
+
+
+def kvzap_compress(hidden_states: torch.Tensor, keys, values, weights: tuple, n_kept: int,
+                   return_indices: bool = False, return_scores: bool = False):
+    """KVzapPress.compress (kvp_kvzap_compress): the scores above, the n_kept best per head, K / V compacted.
+    Returns (k_out, v_out, idx, scores)."""
+    _require_cuda_kv(keys, values)
+    keys, values = _normalise(keys), _normalise(values)
+    return _compress("kvp_kvzap_compress", SCORER_KVZAP, keys, values, n_kept,
+                     (*_kvzap_inputs(hidden_states, keys, weights), keys, values), return_indices, return_scores)
+
+
+def threshold_evict(scores: torch.Tensor, n_evict: int, threshold: float, shift: int) -> list:
+    """DMSPress's eviction (kvp_threshold_evict): [b, h, s + shift] (int64) of every scores[b, h, s] < threshold with
+    s < n_evict, in torch.where order, the threshold rounded to the score dtype as torch does. One host read (the
+    count)."""
+    if not scores.is_cuda or scores.dtype not in _DTYPES or scores.dim() != 3:
+        raise RuntimeError(f"scores must be a CUDA bf16/fp16 [B, Hkv, n] tensor, got {scores.dtype} "
+                           f"{tuple(scores.shape)} on {scores.device}")
+    B, H, n = scores.shape
+    if not 0 <= n_evict <= n:
+        raise ValueError(f"need 0 <= n_evict <= {n}, got {n_evict}")
+    if n > 1 and scores.stride(2) != 1 or scores.data_ptr() % 2:
+        scores = scores.contiguous()
+    sstride = (ctypes.c_int64 * 2)(*(scores.stride(d) if scores.shape[d] > 1 else 0 for d in range(2)))
+    dev = scores.device
+    out = torch.empty((3, B * H * n_evict), dtype=torch.int64, device=dev)
+    count = torch.empty((1,), dtype=torch.int64, device=dev)
+    ws = torch.empty(((B * H * -(-n // 4096) * 8 + 255) // 256 * 256,), dtype=torch.uint8, device=dev)
+    with _guard(dev):
+        _check(load().kvp_threshold_evict(_DTYPES[scores.dtype], B, H, n, _ptr(scores), sstride, int(n_evict),
+                                          float(threshold), int(shift), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]),
+                                          _ptr(count), _ptr(ws), ws.numel(), _stream()), "kvp_threshold_evict")
+    c = int(count.item())
+    # copies of exactly the count, as torch.where returns: DMSPress keeps them for the rest of the generation
+    return list(out[:, :c].clone().unbind(0))

@@ -19,6 +19,7 @@ from transformers.pipelines import PIPELINE_REGISTRY
 
 from kvpress_b200.presses.base_press import BasePress
 from kvpress_b200.presses.decoding_press import DecodingPress
+from kvpress_b200.presses.dms_press import DMSPress
 from kvpress_b200.presses.finch_press import FinchPress
 from kvpress_b200.presses.key_rerotation_press import KeyRerotationPress
 from kvpress_b200.presses.prefill_decoding_press import PrefillDecodingPress
@@ -85,9 +86,12 @@ class KVPressTextGenerationPipeline(Pipeline):
 
     def _forward(self, input_tensors, max_new_tokens: int = 50, press: Optional[BasePress] = None,
                  cache: Optional[Cache] = None):
-        # pipeline.py:202-230 of the reference: a DecodingPress is live only while generating, a
-        # PrefillDecodingPress in both phases, everything else only during prefill
-        decoding = isinstance(press, (DecodingPress, PrefillDecodingPress))
+        # pipeline.py:202-233 of the reference: a DecodingPress is live only while generating, a
+        # PrefillDecodingPress and a DMSPress with decoding=True in both phases, everything else only during prefill.
+        # Unlike the reference, a decoding DMSPress also refuses several questions: the positions it masks while
+        # answering one would outlive _remove_answer_from_cache and mask the next question's tokens.
+        decoding = isinstance(press, (DecodingPress, PrefillDecodingPress)) or (
+            isinstance(press, DMSPress) and press.decoding)
         prefilling = press is not None and not isinstance(press, DecodingPress)
         if decoding and len(input_tensors["questions_ids"]) > 1:
             raise ValueError("DecodingPress is not compatible with multiple questions. Please specify a single question.")
